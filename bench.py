@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/sec of the PPO hot path (rollout + GAE + update) on N B200s.
+"""bench.py -- env-steps/sec of the PPO hot path (rollout + GAE + update) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
@@ -56,8 +56,41 @@ def parse():
     ap.add_argument("--cpu-budget-s", type=float, default=600.0,
                     help="wall-clock budget of the CPU arm; whole epochs are dropped (never shortened) beyond it")
     ap.add_argument("--matmul", default="tc3", choices=["fp32", "tf32x3", "tc3"],
-                    help="MLP GEMM path: tc3 = hand-written tcgen05 3xTF32 kernel on the 256-wide layers (default), fp32 = cuBLAS SIMT everywhere, tf32x3 = 3 cuBLAS TF32 GEMMs")
+                    help="MLP GEMM path: tc3 = hand-written wgmma 3xTF32 kernel on the 256-wide layers (default), fp32 = cuBLAS SIMT everywhere, tf32x3 = 3 cuBLAS TF32 GEMMs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last device-timed step computed (rollout buffer, "
+                         "advantages / returns, updated network parameters, logged update scalars) as DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_MAX_ELEMS = 1 << 20      # per array; larger arrays are dumped as a fixed, seeded sample of their rows
+
+
+def dump_outputs(out_dir, agent, buf):
+    """What the timed path hands its caller after its last step, as float32 / float64 .npy files (< 64 MB in all):
+    every rollout-buffer array (rows = time x env), the updated policy / value parameters and the logged update
+    scalars.  The inputs depend only on the command-line arguments (fixed seeds), so two builds run with the same
+    arguments can be compared file by file."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for key in sorted(buf._keys):
+        t = getattr(buf, "_" + key).detach()
+        arrays["buffer_" + key] = t.reshape(t.shape[0] * t.shape[1], -1) if t.dim() >= 2 else t.reshape(-1, 1)
+    arrays["pf_params"] = torch.nn.utils.parameters_to_vector(agent.pf.parameters()).detach()
+    arrays["vf_params"] = torch.nn.utils.parameters_to_vector(agent.vf.parameters()).detach()
+    for key in ("log32", "log64"):
+        if key in agent._mb_state:
+            arrays["update_" + key] = agent._mb_state[key].detach()
+    rng = np.random.default_rng(0)
+    for name, t in arrays.items():
+        a = t.cpu().numpy()
+        a = a.astype(np.float64 if a.dtype in (np.float64, np.int64) else np.float32)
+        if a.size > DUMP_MAX_ELEMS:
+            rows = max(1, DUMP_MAX_ELEMS // max(1, a[0].size))
+            a = a[np.sort(rng.choice(a.shape[0], size=rows, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def measured_peaks():
@@ -65,7 +98,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 # ----------------------------------------------------------------------------------------- clocks
@@ -629,8 +662,8 @@ def run_ours(args):
         else:
             col.rollout_no_sync()
             # bound the launch queue (no data copied): the public-API leg waits here too (it reads the episode
-            # count), and a queue holding the rollout's 128 AND the update's 320 graph launches measured ~8 % slower
-            # on B200 than two shorter ones; with several ranks this also aligns them before the collective-bearing
+            # count), and a queue holding the rollout's 128 AND the update's 320 graph launches was measured slower
+            # than two shorter ones; with several ranks this also aligns them before the collective-bearing
             # update graphs
             torch.cuda.current_stream(device).synchronize()
             agent.update_per_epoch(flush_infos=False)
@@ -678,12 +711,14 @@ def run_ours(args):
         marks[k + 1].record()
         if os.environ.get("BENCH_VALUE_SYNC", "1") == "1":
             # bound the launch queue: wait (no data copied) until the epoch has drained before queueing
-            # the next ~450 graph launches; an unbounded queue measured ~15% slower on B200
+            # the next ~450 graph launches; an unbounded queue was measured slower
             torch.cuda.current_stream(device).synchronize()
     torch.cuda.synchronize(device)
     sampler.mark_end()
     ctx.barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and ctx.rank == 0:
+        dump_outputs(args.dump_outputs, agent, buf)
     t_dev = ctx.max_over_ranks(marks[0].elapsed_time(marks[-1]) * 1e-3)
     step_ms = [round(marks[k].elapsed_time(marks[k + 1]), 3) for k in range(args.steps)]    # this rank's steps
     launches = _lib.launch_count() - launches0
@@ -748,10 +783,10 @@ def run_ours(args):
                                       "with the gradient norms, csrc/comm.cu)" % ctx.world_size,
                        "matmul": {"fp32": "fp32 cuBLAS SIMT (TF32 off)",
                                   "tf32x3": "3xTF32 error-compensated tensor-core GEMMs (fp32-faithful), cuBLAS",
-                                  "tc3": "256-wide layers: hand-written tcgen05 3xTF32 GEMM on CTA pairs (fp32-faithful, "
+                                  "tc3": "256-wide layers: hand-written wgmma 3xTF32 GEMM (fp32-faithful, "
                                          "csrc/gemm_pair.cu); 17-wide / <=8-wide layers: HBM-bound fp32 kernels (csrc/skinny.cu)"}[args.matmul], "cuda_graphs": not args.no_graph,
                        "l2": "each step rewrites the whole 100 MB rollout working set and all activations "
-                             "(> 126 MB L2 per epoch); the GAE roofline launch flushes L2 explicitly"},
+                             "(> 50 MB L2 per epoch); the GAE roofline launch flushes L2 explicitly"},
             "e2e": {"value": e2e_value, "unit": "env-steps/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": t_e2e / args.steps * 1e3},
             "gpu_launches": launches,

@@ -1,4 +1,4 @@
-/* torchrl_b200.h -- C ABI of libtorchrl_b200.so (sm_100a kernels for the torchrl hot path).
+/* torchrl_b200.h -- C ABI of libtorchrl_b200.so (sm_90a kernels for the torchrl hot path).
  *
  * The reference (RchalYang/torchrl, pure Python) has no FFI of its own; these are the
  * entry points a ctypes binding of the reference would call in place of the Python/NumPy
@@ -253,8 +253,8 @@ int64_t trl_comm_ll_recv_bytes(int world, int nmax);
 int trl_allreduce_f64_ll(const double* local, void* const* peer_recv, int rank, int world, double* out, int n, int nmax,
                          int gather, unsigned* ll_seq, void* stream);
 
-/* ---- fp32-faithful tensor-core GEMM for the 256-wide MLP layers (tcgen05.mma kind::tf32, 3xTF32 split in
- * shared memory, TMA operand loads, TMEM accumulator): C (M x 256) = A (M x K) . B (256 x K)^T, A/B row-major.
+/* ---- fp32-faithful tensor-core GEMM for the 256-wide MLP layers (wgmma tf32, 3xTF32 split in
+ * shared memory, TMA operand loads, register accumulator): C (M x 256) = A (M x K) . B (256 x K)^T, A/B row-major.
  * Serves MLPBase's Linear forward / dgrad / wgrad (networks/base.py:24-44) when the layer width is 256.
  * splits > 1: deterministic split-K (workspace: splits*M*256 floats).  bias != NULL (splits == 1): the Linear
  * epilogue C = act(A B^T + bias) is fused (act: 0 none, 1 tanh, 2 relu). */
@@ -264,8 +264,8 @@ int trl_gemm_tf32x3_nt(const float* A, const float* B, float* C, int64_t M, int6
 int trl_gemm_tf32x3_tn(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
                        float* workspace, void* stream);
 int trl_transpose_f32(const float* in, float* out, int64_t rows, int cols, void* stream);
-/* The same three shapes on CTA PAIRS (tcgen05 cta_group::2, csrc/gemm_pair.cu): one MMA covers 256 x 256, each
- * CTA stages half of B, 3-stage ring, coalesced epilogue.  C (M x 256) = act(A (M x K) . B + bias):
+/* The same three shapes for the hot path (csrc/gemm_pair.cu): pre-split weight planes, N-major dgrad operand,
+ * MUFU tanh, 8-way split-K reduce.  C (M x 256) = act(A (M x K) . B + bias):
  * b_nmajor == 0: B is (256 x K) row-major (Linear forward, networks/base.py:24-44: x W^T + b);
  * b_nmajor != 0: B is (K x 256) row-major (the dgrad shape g W, no transpose of the weights).
  * b_lo != NULL: (b_hi, b_lo) are pre-split TF32 planes of B (trl_split_tf32 / trl_adam_step / trl_polyak_update);

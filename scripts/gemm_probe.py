@@ -1,4 +1,4 @@
-"""Hardware check of the CTA-pair 3xTF32 GEMM (csrc/gemm_pair.cu) against fp64 and against the single-CTA kernel.
+"""Hardware check of the hot-path 3xTF32 GEMM (csrc/gemm_pair.cu) against fp64 and against csrc/gemm_tf32x3.cu.
 
     python scripts/gemm_probe.py            # every case in its own subprocess under a 90 s timeout
     python scripts/gemm_probe.py case nt    # one case in this process
@@ -12,7 +12,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CASES = ("nt", "nt_split", "nn", "nn_split", "tn", "time", "trace")
+CASES = ("nt", "nt_split", "nn", "nn_split", "tn", "time")
 
 
 def timeit(fn, n=50):
@@ -32,67 +32,6 @@ def timeit(fn, n=50):
 def planes(w):
     from torchrl_b200.networks import fused
     return fused.split_tf32(w)
-
-
-SLOTS = 136
-
-
-def trace_case():
-    """Per-phase clock64() stamps of one CTA of the pair kernel (built with -DTRL_PAIR_TRACE into its own .so)."""
-    import ctypes
-    import torch
-    csrc = os.path.join(ROOT, "torchrl_b200", "csrc")
-    lib_path = os.path.join(ROOT, "torchrl_b200", "lib", "libtrl_pair_trace.so")
-    subprocess.run(["nvcc", "-DTRL_PAIR_TRACE", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17",
-                    "-lineinfo", "-Xcompiler", "-fPIC", "-shared", os.path.join(csrc, "gemm_pair.cu"),
-                    os.path.join(csrc, "errors.cu"), "-o", lib_path], check=True)
-    lib = ctypes.CDLL(lib_path)
-    vp, i64, i32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int
-    lib.trl_gemm3_pair.argtypes = [vp, vp, vp, vp, i64, i64, i32, vp, i32, vp]
-    lib.trl_gemm3_pair_tn.argtypes = [vp, vp, vp, i64, i64, i32, vp, vp]
-    lib.trl_pair_set_trace.argtypes = [vp, ctypes.c_uint]
-    dev = "cuda"
-    M, K = 16384, 256
-    a = torch.randn(M, K, device=dev)
-    w = torch.randn(256, K, device=dev) / 16
-    hi, lo = planes(w)
-    bias = torch.randn(256, device=dev) * 0.1
-    out = torch.empty(M, 256, device=dev)
-    buf = torch.zeros(SLOTS, dtype=torch.int64, device=dev)
-    st = torch.cuda.current_stream().cuda_stream
-
-    def show(tag, fn, ctas=(0, 1, 64)):
-        for cta in ctas:
-            lib.trl_pair_set_trace(buf.data_ptr(), cta)
-            for _ in range(3):
-                fn()
-            torch.cuda.synchronize()
-            buf.zero_()
-            fn()
-            torch.cuda.synchronize()
-            t = buf.cpu().numpy()
-            t0 = t[0]
-            rel = lambda i: int(t[i] - t0) if t[i] else -1
-            nkb = 8
-            print("%s cta %d: setup %d  tmem_full %d  tmem->smem %d  stored %d  end %d (clocks from kernel entry)" %
-                  (tag, cta, rel(1), rel(2), rel(3), rel(4), rel(5)))
-            print("   tma issue   " + " ".join("%6d" % rel(8 + k) for k in range(nkb)))
-            print("   full seen   " + " ".join("%6d" % rel(24 + k) for k in range(nkb)))
-            print("   conv done   " + " ".join("%6d" % rel(40 + k) for k in range(nkb)))
-            print("   mma start   " + " ".join("%6d" % rel(72 + k) for k in range(nkb)))
-            print("   mma issued  " + " ".join("%6d" % rel(104 + k) for k in range(nkb)))
-            print("   epi chunk   " + " ".join("%6d" % rel(120 + k) for k in range(8)), flush=True)
-
-    show("nt split + tanh", lambda: lib.trl_gemm3_pair(a.data_ptr(), hi.data_ptr(), lo.data_ptr(), out.data_ptr(), M, K, 0,
-                                                        bias.data_ptr(), 1, st))
-    show("nt raw, no epilogue", lambda: lib.trl_gemm3_pair(a.data_ptr(), w.data_ptr(), None, out.data_ptr(), M, K, 0, None, 0,
-                                                            st), ctas=(0,))
-    g = torch.randn(16384, 256, device=dev)
-    x = torch.randn(16384, 256, device=dev)
-    ws = torch.empty(64 * 256 * 256, device=dev)
-    dw = torch.empty(256, 256, device=dev)
-    show("tn (wgrad) 64 splits", lambda: lib.trl_gemm3_pair_tn(g.data_ptr(), x.data_ptr(), dw.data_ptr(), 256, 16384, 64,
-                                                                ws.data_ptr(), st), ctas=(0,))
 
 
 def run_case(name):
@@ -119,7 +58,7 @@ def run_case(name):
             err_r = (got_r.double() - torch.relu(ref + bias.double())).abs().max().item() / scale
             print("%-9s M=%6d K=%4d  rel err %.2e  tanh abs err %.2e  relu rel err %.2e" % (name, M, K, err, err_t, err_r),
                   flush=True)
-            # 3xTF32 with fp32 TMEM accumulation: ~2e-6 of max|C| at K = 256, growing linearly with K
+            # 3xTF32 with the tensor core's fp32 accumulation: ~2e-6 of max|C| at K = 256, growing linearly with K
             tol = 5e-6 * max(1, K // 256)
             assert err < tol and err_t < tol * max(1.0, scale) and err_r < tol, "accuracy"
     elif name == "tn":
@@ -158,8 +97,6 @@ def run_case(name):
         t3 = timeit(lambda: torch.mm(g.t(), x))
         print("wgrad 256x256, K=16384, 64 splits (incl. reduce): pair %.1f us  single %.1f us  cublas %.1f us" % (t1, t2, t3),
               flush=True)
-    elif name == "trace":
-        trace_case()
     else:
         raise SystemExit("unknown case " + name)
     print("CASE %s OK" % name, flush=True)

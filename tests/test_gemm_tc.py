@@ -1,4 +1,4 @@
-"""tcgen05 3xTF32 GEMM (csrc/gemm_tf32x3.cu) vs float64: fp32-faithful (error of the order of the cuBLAS fp32
+"""wgmma 3xTF32 GEMM (csrc/gemm_tf32x3.cu) vs float64: fp32-faithful (error of the order of the cuBLAS fp32
 SIMT GEMM's own error, ~1e-6 relative to max|C|), for the forward/dgrad shape and the split-K wgrad shape."""
 import numpy as np
 import pytest
@@ -19,7 +19,7 @@ def test_gemm_tf32x3_matches_fp64(M, K, splits):
     scale = ref.abs().max().item()
     err = (out.double() - ref).abs().max().item() / scale
     err32 = ((a @ b.t()).double() - ref).abs().max().item() / scale
-    print("M=%d K=%d splits=%d  rel err 3xTF32(tcgen05) %.2e  fp32 cuBLAS %.2e" % (M, K, splits, err, err32))
+    print("M=%d K=%d splits=%d  rel err 3xTF32(wgmma) %.2e  fp32 cuBLAS %.2e" % (M, K, splits, err, err32))
     # fp32-faithful: within a small multiple of the fp32 SIMT GEMM's own error (plain TF32 sits at ~3e-4)
     assert err < 8 * err32 + 5e-7, (err, err32)
 
@@ -27,7 +27,7 @@ def test_gemm_tf32x3_matches_fp64(M, K, splits):
 @pytest.mark.gpu
 def test_gemm_tf32x3_error_grows_with_per_cta_reduction_length():
     """The tensor core's fp32 accumulation truncates, so the error grows ~linearly with the number of K steps
-    accumulated in TMEM (2e-6 at 256, ~7e-6 at 1024, relative to max|C|): callers keep K/splits <= 256.
+    accumulated by one CTA (2e-6 at 256, ~7e-6 at 1024, relative to max|C|): callers keep K/splits <= 256.
     Still ~40x better than plain TF32 at the same length."""
     import torch
     from torchrl_b200 import ops
@@ -70,6 +70,6 @@ def test_gemm_tf32x3_tn_matches_fp64(M, K, splits):
     scale = ref.abs().max().item()
     err = (out.double() - ref).abs().max().item() / scale
     err32 = ((a.t() @ b).double() - ref).abs().max().item() / scale
-    print("tn M=%d K=%d splits=%d  rel err 3xTF32(tcgen05) %.2e  fp32 cuBLAS %.2e" % (M, K, splits, err, err32))
+    print("tn M=%d K=%d splits=%d  rel err 3xTF32(wgmma) %.2e  fp32 cuBLAS %.2e" % (M, K, splits, err, err32))
     # fp32-faithful: within a small multiple of the fp32 SIMT GEMM's own error (plain TF32 sits at ~3e-4)
     assert err < 8 * err32 + 5e-7, (err, err32)

@@ -110,7 +110,7 @@ def test_tf32x3_mlp_matches_fp32_mlp():
 
 @pytest.mark.gpu
 def test_tc3_mlp_matches_fp32_mlp():
-    """MLP(256,256) forward/backward with the hand-written tcgen05 3xTF32 GEMM on the 256-wide layer."""
+    """MLP(256,256) forward/backward with the hand-written wgmma 3xTF32 GEMM on the 256-wide layer."""
     import copy
     import torch
     import torch.nn as nn

@@ -1,20 +1,28 @@
-"""A2C, V-MPO and TRPO on the device against the EXECUTED reference (oracle/_ref or /root/reference behind oracle/shims,
-torch CPU): same initial weights (state_dict copied from the reference's networks), the same explicit batches through
-`update(batch)` -- the reference's own entry point -- then the logged scalars of every update and the parameters after
-the last one are compared.  SURVEY.md 8(f).4.
+"""A2C, V-MPO and TRPO on the device against the reference's own `update(batch)` (torch CPU, the unmodified reference
+behind oracle/shims), recorded in tests/golden/onpolicy_reference.npz by oracle/make_golden_onpolicy.py: same initial
+weights (the reference networks' state_dicts), the same explicit batches, then the logged scalars of every update and
+the parameters after the last one are compared.  SURVEY.md 8(f).4.
 
 Stated tolerances (fp32 device kernels vs torch-CPU fp32): logged scalars rtol 2e-3 + atol 2e-4 (TRPO policy loss /
 KL-driven quantities 5e-3), parameters atol 2e-4 (TRPO: 1e-3 of the step, the conjugate-gradient solve amplifies
 rounding).  The device epoch loop (captured graphs) is checked against the eager `update` path of the same agent.
 """
+import os
+
 import numpy as np
 import pytest
 
-from oracle import reference_loader
+from oracle import make_golden_onpolicy as gold
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not reference_loader.available(), reason="no copy of the reference")]
+pytestmark = pytest.mark.gpu
 
-O, A, HID = 11, 3, (32, 32)
+O, A, HID = gold.O, gold.A, gold.HID
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "onpolicy_reference.npz")
+
+
+@pytest.fixture(scope="module")
+def ref():
+    return gold.load(GOLDEN)
 
 
 class _NullLogger:
@@ -38,41 +46,12 @@ class _Col:
     epoch_frames = 64
 
 
-def _batches(n, B, seed, lead=None):
-    rs = np.random.RandomState(seed)
-    out = []
-    for _ in range(n):
-        shape = (B,) if lead is None else lead
-        obs = rs.randn(*shape, O)
-        acts = np.tanh(0.4 * rs.randn(*shape, A))
-        out.append(dict(obs=obs, acts=acts, advs=rs.randn(*shape, 1), estimate_returns=rs.randn(*shape, 1),
-                        values=rs.randn(*shape, 1)))
-    return out
-
-
-def _reference_agent(kind, tmp_path, **algo_kw):
+def _state(rec, net):
     import torch
-    reference_loader.load()                  # puts the gym / tensorboardX shims on sys.path
-    import gym
-    import torchrl.networks as networks
-    import torchrl.policies as policies
-    from torchrl.algo import A2C, TRPO, VMPO
-
-    class Env:
-        action_space = gym.spaces.Box(-np.ones(A), np.ones(A))
-        observation_space = gym.spaces.Box(-np.ones(O), np.ones(O))
-    torch.manual_seed(3)
-    net = dict(hidden_shapes=list(HID), append_hidden_shapes=[], base_type=networks.MLPBase, activation_func=torch.nn.Tanh)
-    pf = policies.GuassianContPolicyBasicBias(input_shape=O, output_shape=A, tanh_action=True, **net)
-    vf = networks.Net(input_shape=(O,), output_shape=1, **net)
-    cls = {"a2c": A2C, "vmpo": VMPO, "trpo": TRPO}[kind]
-    agent = cls(pf=pf, vf=vf, env=Env(), replay_buffer=None, collector=_Col(), logger=_NullLogger(), discount=0.99,
-                num_epochs=10, batch_size=64, gae=True, device="cpu", save_dir=str(tmp_path), shuffle=True, tau=0.95,
-                **algo_kw)
-    return agent
+    return {k[len(net) + 1:]: torch.as_tensor(v, dtype=torch.float32) for k, v in rec.items() if k.startswith(net + ".")}
 
 
-def _device_agent(kind, ref_agent, **algo_kw):
+def _device_agent(kind, init):
     import torch
     import torchrl_b200.networks as networks
     import torchrl_b200.policies as policies
@@ -85,12 +64,17 @@ def _device_agent(kind, ref_agent, **algo_kw):
     net = dict(hidden_shapes=list(HID), append_hidden_shapes=[], base_type=networks.MLPBase, activation_func=torch.nn.Tanh)
     pf = policies.GuassianContPolicyBasicBias(input_shape=O, output_shape=A, tanh_action=True, **net)
     vf = networks.Net(input_shape=(O,), output_shape=1, **net)
-    pf.load_state_dict(ref_agent.pf.state_dict())
-    vf.load_state_dict(ref_agent.vf.state_dict())
+    pf.load_state_dict(_state(init, "pf"))
+    vf.load_state_dict(_state(init, "vf"))
     cls = {"a2c": A2C, "vmpo": VMPO, "trpo": TRPO}[kind]
     return cls(pf=pf, vf=vf, env=Env(), replay_buffer=None, collector=_Col(), logger=_NullLogger(), discount=0.99,
                num_epochs=10, batch_size=64, gae=True, device="cuda:0", save_dir=None, shuffle=True, tau=0.95,
-               use_cuda_graph=False, **algo_kw)
+               use_cuda_graph=False, **gold.KW[kind])
+
+
+def _batches(case):
+    kind, n, B, seed, lead = gold.CASES[case]
+    return gold.batches(n, B, seed, lead)
 
 
 def _params(agent, names=("pf", "vf")):
@@ -112,70 +96,55 @@ def _compare_infos(mine, ref, rtol=2e-3, atol=2e-4, skip=()):
             assert abs(m[k] - v) <= rtol * abs(v) + atol, (u, k, m[k], v)
 
 
-def test_a2c_update_matches_reference(tmp_path):
-    kw = dict(plr=1e-3, vlr=1e-3, entropy_coeff=0.01)
-    ref = _reference_agent("a2c", tmp_path, **kw)
-    mine = _device_agent("a2c", ref, **kw)
-    batches = _batches(4, 64, 0)
-    r_infos = [ref.update(b) for b in batches]
-    m_infos = [mine.update(b) for b in batches]
-    _compare_infos(m_infos, r_infos)
-    pr, pm = _params(ref), _params(mine)
-    for k in pr:
-        np.testing.assert_allclose(pm[k], pr[k], atol=2e-4, err_msg=k)
+def test_a2c_update_matches_reference(ref):
+    r = ref["a2c"]
+    mine = _device_agent("a2c", r["init"])
+    m_infos = [mine.update(b) for b in _batches("a2c")]
+    _compare_infos(m_infos, [r["info%d" % u] for u in range(len(m_infos))])
+    pm = _params(mine)
+    for k, v in r["final"].items():
+        np.testing.assert_allclose(pm[k], v, atol=2e-4, err_msg=k)
 
 
-def test_vmpo_update_matches_reference(tmp_path):
-    kw = dict(plr=1e-3, vlr=1e-3, opt_epochs=2, alpha_eps=0.01)
-    ref = _reference_agent("vmpo", tmp_path, **kw)
-    mine = _device_agent("vmpo", ref, **kw)
-    batches = _batches(4, 64, 1)
-    r_infos = [ref.update(b) for b in batches]
-    m_infos = [mine.update(b) for b in batches]
-    _compare_infos(m_infos, r_infos)
-    pr, pm = _params(ref), _params(mine)
-    for k in pr:
-        np.testing.assert_allclose(pm[k], pr[k], atol=2e-4, err_msg=k)
-    assert abs(float(mine.dual[0]) - float(ref.eta)) < 2e-4 and abs(float(mine.dual[1]) - float(ref.alpha)) < 2e-4
+def test_vmpo_update_matches_reference(ref):
+    r = ref["vmpo"]
+    mine = _device_agent("vmpo", r["init"])
+    m_infos = [mine.update(b) for b in _batches("vmpo")]
+    _compare_infos(m_infos, [r["info%d" % u] for u in range(len(m_infos))])
+    pm = _params(mine)
+    for k, v in r["final"].items():
+        np.testing.assert_allclose(pm[k], v, atol=2e-4, err_msg=k)
+    assert abs(float(mine.dual[0]) - r["dual"]["eta"]) < 2e-4 and abs(float(mine.dual[1]) - r["dual"]["alpha"]) < 2e-4
 
 
 @pytest.mark.parametrize("lead", [None, (8, 16)])
-def test_trpo_update_matches_reference(tmp_path, lead):
+def test_trpo_update_matches_reference(ref, lead):
     """Flat (B, .) batches (per-sample KL) and the (T, N, .) whole-rollout form the reference's update_per_epoch
     passes (its KL sums over the env axis: the N / act_dim quirk)."""
-    kw = dict(plr=3e-4, vlr=1e-3, max_kl=0.01, cg_damping=0.1, cg_iters=10, residual_tol=1e-10, entropy_coeff=0.01,
-              v_opt_times=2)
-    ref = _reference_agent("trpo", tmp_path, **kw)
-    mine = _device_agent("trpo", ref, **kw)
-    # actions the policy could have produced (log-probs of arbitrary actions underflow exp() in the reference's ratio)
-    import torch
-    batches = _batches(2, 128, 2, lead)
-    for b in batches:
-        with torch.no_grad():
-            o = torch.as_tensor(b["obs"], dtype=torch.float32)
-            mean, std, _ = ref.pf(o)
-            b["acts"] = torch.tanh(mean + std * torch.randn_like(mean)).numpy().astype(np.float64)
-    p0 = _params(ref, ("pf",))
-    for b in batches:
-        r_info = ref.update(b)
+    case = "trpo_flat" if lead is None else "trpo_lead"
+    r = ref[case]
+    mine = _device_agent("trpo", r["init"])
+    batches = _batches(case)
+    for i, b in enumerate(batches):   # actions the reference policy sampled (recorded with the reference run)
+        b["acts"] = r["acts"][str(i)]
+    p0 = {k: v for k, v in r["init"].items() if k.startswith("pf.")}
+    for i, b in enumerate(batches):
         m_info = mine.update(b)
-        _compare_infos([m_info], [r_info], rtol=5e-3, atol=5e-4)
-        pr, pm = _params(ref, ("pf",)), _params(mine, ("pf",))
+        _compare_infos([m_info], [r["info%d" % i]], rtol=5e-3, atol=5e-4)
+        pr, pm = r["pf%d" % i], _params(mine, ("pf",))
         step = max(np.abs(pr[k] - p0[k]).max() for k in pr)
         assert step > 1e-5, "the reference took no step: the test would be vacuous"
         for k in pr:
             np.testing.assert_allclose(pm[k], pr[k], atol=2e-2 * step + 1e-5, err_msg=k)
-        # continue both from the SAME parameters so that one update's rounding does not leak into the next
-        mine.pf.load_state_dict(ref.pf.state_dict())
+        # continue from the reference's parameters so that one update's rounding does not leak into the next
+        mine.pf.load_state_dict(_state(pr, "pf"))
         p0 = pr
     flat = [dict(obs=b["obs"].reshape(-1, O), estimate_returns=b["estimate_returns"].reshape(-1, 1)) for b in batches]
-    for b in flat:
-        r_info = ref.update_vf(b)
-        m_info = mine.update_vf(b)
-        _compare_infos([m_info], [r_info])
-    pr, pm = _params(ref, ("vf",)), _params(mine, ("vf",))
-    for k in pr:
-        np.testing.assert_allclose(pm[k], pr[k], atol=2e-4, err_msg=k)
+    for i, b in enumerate(flat):
+        _compare_infos([mine.update_vf(b)], [r["vfinfo%d" % i]])
+    pm = _params(mine, ("vf",))
+    for k, v in r["final"].items():
+        np.testing.assert_allclose(pm[k], v, atol=2e-4, err_msg=k)
 
 
 @pytest.mark.parametrize("kind", ["a2c", "vmpo", "trpo"])

@@ -1,4 +1,4 @@
-"""End-to-end parity AT THE BENCHMARK'S SIZES: the device path bench.py times -- tcgen05 pair GEMMs with pre-split
+"""End-to-end parity AT THE BENCHMARK'S SIZES: the device path bench.py times -- wgmma 3xTF32 GEMMs with pre-split
 weight planes, the fused MLP tail, skinny-layer kernels, direct gradient writes, CUDA graphs -- against the CPU oracle
 port (oracle/ref_port.py, pinned bit-for-bit to the unmodified reference by tests/test_oracle_vs_reference.py) on the
 same seeds and the same exploration noise.

@@ -1,4 +1,4 @@
-"""torchrl_b200 -- B200-native (sm_100a) implementation of the RchalYang/torchrl hot path.
+"""torchrl_b200 -- H100-native (sm_90a) implementation of the RchalYang/torchrl hot path.
 
 The package mirrors the reference's agent / collector / replay-buffer / env Python API
 (reference: /root/reference/torchrl) with all rollout data resident on the GPU and every

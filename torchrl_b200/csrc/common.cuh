@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the torchrl_b200 sm_100a kernels.
+// common.cuh -- shared helpers for the torchrl_b200 sm_90a kernels.
 //
 // Conventions of every entry point in this library (see include/torchrl_b200.h):
 //   * plain device pointers + sizes, no torch types; the caller owns all memory;
@@ -19,7 +19,7 @@
 
 namespace trl {
 
-constexpr int kNumSM = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSM = 132;  // H100 SXM
 
 // thread-local last-error text (host side)
 void set_error(const char* fmt, ...);

@@ -1,439 +1,20 @@
-// gemm_pair.cu -- fp32-faithful (3xTF32) tensor-core GEMM on CTA PAIRS (tcgen05 cta_group::2) for the 256-wide
-// MLP layers of the hot path (SURVEY.md section 8(a) K3/K8: the Linear layers of
-// /root/reference/torchrl/networks/base.py:24-44 in the rollout, the cached old-log-prob pass and the PPO / SAC
-// minibatch update).  Successor of csrc/gemm_tf32x3.cu (single-CTA tiles, kept for comparison): that kernel is
-// shared-memory-bandwidth bound (tensor pipe 23.5 % in profiles/tc_kernels_ncu_r1.json) because every CTA re-reads
-// a full 256-row B tile for each of the three products and re-splits the weights into hi/lo for every tile.
-//
-//   C[M x 256] (+ bias, activation) = A . B          3 products per 8-deep K step: lo*hi, hi*lo, hi*hi
-//
-// What changes here:
-//   * one MMA covers 256 x 256: CTA r of the pair stages its own 128 rows of A and only 128 of the 256 columns of
-//     B; the tensor cores of both SMs read both halves (per CTA and 32-deep K block: 96 KB of operand reads
-//     instead of 144 KB);
-//   * B can arrive PRE-SPLIT (b_lo != NULL): the weights are split into hi = tf32(w), lo = w - hi once per
-//     optimizer step (csrc/optim.cu writes both planes), TMA loads both planes and only the activation operand
-//     A is converted in shared memory (16 KB instead of 48 KB per stage);
+// gemm_pair.cu -- the hot path's fp32-faithful (3xTF32) tensor-core GEMMs for the 256-wide MLP layers (SURVEY.md
+// section 8(a) K3/K8: the Linear layers in the rollout, the cached old-log-prob pass and the PPO / SAC minibatch
+// update), on the warpgroup-MMA kernel of gemm_wgmma.cuh.  Unlike the csrc/gemm_tf32x3.cu entry points:
+//   * B can arrive PRE-SPLIT (b_lo != NULL): the weights are split into hi = tf32(w), lo = w - hi once per optimizer
+//     step (csrc/optim.cu writes both planes), TMA loads both planes and only the activation operand A is split;
 //   * B may be N-major (b_nmajor): the dgrad shape dX = G . W reads W (K x 256, row-major) directly -- no per-
 //     minibatch transpose of the weights;
-//   * a 64 KB stage instead of 96 KB -> 3-stage ring;
-//   * the epilogue streams 32 columns at a time through a warp-private transposition buffer and stores whole
-//     128-byte row segments; tanh = 1 - 2/(exp(2x)+1) on the MUFU unit (abs err < 2e-7, same as csrc/skinny.cu).
-// Shapes (one template each):
+//   * tanh = 1 - 2/(exp(2x)+1) on the MUFU unit (abs err < 2e-7, same as csrc/skinny.cu);
+//   * split-K slabs are summed by an 8-way balanced tree (pair_splitk_reduce_kernel).
+// Shapes:
 //   nt   : A (M x K) row-major, B (256 x K) row-major      forward  y = act(x W^T + b)
 //   nn   : A (M x K) row-major, B (K x 256) row-major      dgrad    dX = G W
 //   tn   : A (K x M) row-major, B (K x 256) row-major      wgrad    dW = G^T X (split-K, deterministic reduce)
-//
-// Roles per CTA (576 threads, identical in both CTAs so that shared-memory offsets match):
-//   warp 0      TMA producer : this CTA's A tile and its half of B -> LOCAL full[s]
-//   warps 2..17 converters   : raw -> (hi in place, lo twin) for what is not pre-split, then one arrival per warp
-//                              on the LEADER's conv[s] (remote arrive through mapa for rank 1)
-//   warp 1      MMA issuer   : rank 0 only: waits conv[s] (32 arrivals), issues 12 tcgen05.mma.cta_group::2 per
-//                              stage, commits with multicast to empty[s] of BOTH CTAs; last commit -> tmem_full
-//   warps 2..17 epilogue     : each CTA drains its own 128 accumulator rows from its own TMEM, four warps per lane
-//                              quadrant (measured: with one warp per quadrant the epilogue was latency-bound at 16 k
-//                              cycles with tanh, 8.5 k without -- more than the 12 k cycles of tensor work)
-#include "common.cuh"
-#include <cuda.h>
+#include "gemm_wgmma.cuh"
 
 namespace trl {
 namespace pair {
-
-constexpr int kBM = 128, kBNHalf = 128, kBN = 256, kBK = 32;
-constexpr int kStages = 3;
-constexpr int kUmmaK = 8;                               // tf32: 32 bytes per MMA K-step
-constexpr int kTileBytes = kBM * kBK * 4;               // 16 KB: one (128 x 32) fp32 operand tile
-constexpr int kStageBytes = 4 * kTileBytes;             // 64 KB: A hi | A lo | B hi | B lo
-constexpr int kWorkWarps = 16;                           // converter / epilogue warps: 4 per SM sub-partition
-constexpr int kWorkThreads = 32 * kWorkWarps;            // 512
-constexpr int kThreads = 64 + kWorkThreads;              // + TMA warp + MMA warp
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ + 1024 /*bias*/;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-// NOTE on scopes: explicit `.release.cluster` / `.acquire.cluster` qualifiers compile to MEMBAR.ALL.GPU + ERRBAR on
-// every arrive and CCTL.IVALL (L1 invalidate) after every wait -- measured at ~1.4 k cycles per K block in the
-// converter loop (profiles/pair_gemm_r2.md).  The data these barriers order is shared memory handed to the async
-// proxy (fence.proxy.async before the arrive) and TMEM (tcgen05 fences), so the default CTA-scope semantics that
-// CUTLASS' ClusterBarrier uses are sufficient.
-__device__ __forceinline__ void mbar_arrive_local(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 remote;\n\t"
-      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c_inner, int c_outer) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer)
-      : "memory");
-}
-// K-major SWIZZLE_128B canonical layout: 8-row atoms of 1024 B, SBO = 1024 B, version 1 (Blackwell)
-__device__ __forceinline__ uint64_t desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;                     // SWIZZLE_128B
-  return d;
-}
-// M/N-major fp32 operands: SWIZZLE_128B_BASE32B (the only layout tcgen05 accepts for M/N-major tf32; what TMA's
-// SWIZZLE_128B_ATOM_32B writes): rows of 128 B = 32 contiguous M/N elements at one reduction index, atoms of 4 rows
-// (512 B); SBO = 512 B between 4-row atoms along K, LBO = distance between groups of 32 M/N elements (4096 B here).
-__device__ __forceinline__ uint64_t desc_mn_sw128_32b(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((4096 >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(1) << 61;                     // SWIZZLE_128B_BASE32B
-  return d;
-}
-// kind::tf32, fp32 accumulate, M = 256 (two CTAs x 128 rows), N = 256; bit 15 / 16: A / B is M/N-major
-__device__ __forceinline__ uint32_t idesc_tf32_256x256(bool a_mn, bool b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u) |
-         (static_cast<uint32_t>(kBN >> 3) << 17) | (static_cast<uint32_t>((2 * kBM) >> 4) << 24);
-}
-__device__ __forceinline__ void umma_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior MMAs of this thread -> one arrival on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-// explicit shared-state-space accesses: the stage / park pointers are derived from an aligned integer address, which
-// makes plain C++ accesses GENERIC loads / stores that the compiler must order against every global access
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t addr, const float4 v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w));
-}
-#ifdef TRL_PAIR_TRACE
-// per-phase clock64() stamps of one CTA (scripts/gemm_probe.py `trace`): slot layout in the probe script
-#define TRL_TRACE(slot) do { if (p.trace && blockIdx.x == p.trace_cta && blockIdx.y == 0) p.trace[(slot)] = clock64(); } while (0)
-#else
-#define TRL_TRACE(slot) do { } while (0)
-#endif
-__device__ __forceinline__ void split4(const float4 v, float4& h, float4& l) {
-  unsigned u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.x)); h.x = __uint_as_float(u); l.x = v.x - h.x;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.y)); h.y = __uint_as_float(u); l.y = v.y - h.y;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.z)); h.z = __uint_as_float(u); l.z = v.z - h.z;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.w)); h.w = __uint_as_float(u); l.w = v.w - h.w;
-}
-__device__ __forceinline__ float tanh_mufu(float x) { return ::trl::tanh_ex2(x); }   // common.cuh, as csrc/skinny.cu
-
-struct Params {
-  const float* __restrict__ bias;  // (256) added in the epilogue, or nullptr
-  int act;                         // 0 none, 1 tanh, 2 relu (after the bias)
-  float* __restrict__ C;           // (splits, M, 256) when splits > 1 else (M, 256)
-  long long M;                     // output rows
-  int k_blocks_per_split;          // K blocks (of 32) accumulated by one CTA pair
-#ifdef TRL_PAIR_TRACE
-  long long* trace;
-  unsigned trace_cta;
-#endif
-};
-
-// AMN / BMN: operand is M/N-major (reduction index = row index of the row-major source) instead of K-major.
-// BSPLIT: B arrives as two pre-split planes (map_b = hi, map_b2 = lo); otherwise map_b is the raw fp32 matrix.
-template <bool AMN, bool BMN, bool BSPLIT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm3_pair_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                  const __grid_constant__ CUtensorMap map_b2, const __grid_constant__ CUtensorMap map_c, const Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  auto a_hi = [&](int s) { return smem + s * kStageBytes; };
-  auto a_lo = [&](int s) { return smem + s * kStageBytes + kTileBytes; };
-  auto b_hi = [&](int s) { return smem + s * kStageBytes + 2 * kTileBytes; };
-  auto b_lo = [&](int s) { return smem + s * kStageBytes + 3 * kTileBytes; };
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* full = bars;                  // [kStages] local TMA -> local converters
-  uint64_t* conv = bars + kStages;        // [kStages] converters of both CTAs -> MMA (used in the leader only)
-  uint64_t* empty = bars + 2 * kStages;   // [kStages] MMA (multicast commit) -> local TMA
-  uint64_t* tmem_full = bars + 3 * kStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 1);
-  float* bias_s = reinterpret_cast<float*>(smem + kStages * kStageBytes + 256);   // (256) staged once per CTA
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  if (threadIdx.x == 0) TRL_TRACE(0);
-  float bias_r0 = 0.f;                    // first 256 work threads: one bias value each, parked in smem after set-up
-  if (warp >= 2 && threadIdx.x - 64 < kBN && p.bias) bias_r0 = p.bias[threadIdx.x - 64];
-  const int m_blk = blockIdx.x;           // this CTA's 128 output rows
-  const int split = blockIdx.y;
-  const int nkb = p.k_blocks_per_split;
-  const int kb0 = split * nkb;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
-    if (BSPLIT) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b2)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < kStages; ++s) {
-        mbar_init(&full[s], 1);
-        mbar_init(&conv[s], 2 * kWorkWarps);   // every converter warp of both CTAs
-        mbar_init(&empty[s], 1);
-      }
-      mbar_init(tmem_full, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    // the same warp of both CTAs allocates: 256 fp32 accumulator columns at the same address in both SMs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  cluster_sync_all();                     // the peer's barriers are initialised before anyone arrives on them
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-  if (threadIdx.x == 0) TRL_TRACE(1);
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (kb / kStages) & 1;
-        mbar_wait(&empty[s], ph ^ 1);
-        TRL_TRACE(8 + kb);
-        mbar_arrive_expect_tx(&full[s], (BSPLIT ? 3 : 2) * kTileBytes);
-        const int k0 = (kb0 + kb) * kBK;
-        if (!AMN) {
-          tma_load_2d(a_hi(s), &map_a, &full[s], k0, m_blk * kBM);
-        } else {
-#pragma unroll
-          for (int g = 0; g < kBM / 32; ++g)      // one (32 M elements x 32 reduction rows) box per 32 output rows
-            tma_load_2d(a_hi(s) + g * 4096, &map_a, &full[s], m_blk * kBM + g * 32, k0);
-        }
-        const int n0 = static_cast<int>(rank) * kBNHalf;
-        if (!BMN) {
-          tma_load_2d(b_hi(s), &map_b, &full[s], k0, n0);
-          if (BSPLIT) tma_load_2d(b_lo(s), &map_b2, &full[s], k0, n0);
-        } else {
-#pragma unroll
-          for (int g = 0; g < kBNHalf / 32; ++g) {
-            tma_load_2d(b_hi(s) + g * 4096, &map_b, &full[s], n0 + g * 32, k0);
-            if (BSPLIT) tma_load_2d(b_lo(s) + g * 4096, &map_b2, &full[s], n0 + g * 32, k0);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only)
-    if (rank == 0 && lane == 0) {
-      const uint32_t idesc = idesc_tf32_256x256(AMN, BMN);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (kb / kStages) & 1;
-        mbar_wait(&conv[s], ph);
-        TRL_TRACE(72 + kb);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t da_hi = AMN ? desc_mn_sw128_32b(smem_u32(a_hi(s))) : desc_k_sw128(smem_u32(a_hi(s)));
-        const uint64_t da_lo = AMN ? desc_mn_sw128_32b(smem_u32(a_lo(s))) : desc_k_sw128(smem_u32(a_lo(s)));
-        const uint64_t db_hi = BMN ? desc_mn_sw128_32b(smem_u32(b_hi(s))) : desc_k_sw128(smem_u32(b_hi(s)));
-        const uint64_t db_lo = BMN ? desc_mn_sw128_32b(smem_u32(b_lo(s))) : desc_k_sw128(smem_u32(b_lo(s)));
-#pragma unroll
-        for (int k = 0; k < kBK / kUmmaK; ++k) {
-          // K-major: +32 B per K-step inside the 128 B swizzle row; MN-major: +1024 B = 8 reduction rows further
-          const uint64_t adv_a = static_cast<uint64_t>((AMN ? k * 1024 : k * kUmmaK * 4) >> 4);
-          const uint64_t adv_b = static_cast<uint64_t>((BMN ? k * 1024 : k * kUmmaK * 4) >> 4);
-          umma_pair(tmem_base, da_lo + adv_a, db_hi + adv_b, idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_pair(tmem_base, da_hi + adv_a, db_lo + adv_b, idesc, 1u);
-          umma_pair(tmem_base, da_hi + adv_a, db_hi + adv_b, idesc, 1u);
-        }
-        umma_commit_multicast(&empty[s], 0b11);            // both CTAs may refill their stage s
-        TRL_TRACE(104 + kb);
-      }
-      umma_commit_multicast(tmem_full, 0b11);              // both accumulator halves are complete
-    }
-  } else {
-    // ------------------------------------------------------------------ converters (warps 2..17), then epilogue
-    const int ct = threadIdx.x - 64;                       // 0..511
-    if (ct < kBN) bias_s[ct] = bias_r0;
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % kStages;
-      const uint32_t ph = (kb / kStages) & 1;
-      mbar_wait(&full[s], ph);
-      if (ct == 0) TRL_TRACE(24 + kb);
-      // all loads of this thread first (independent 16-byte accesses in flight), then convert and store
-      constexpr int kPer = kTileBytes / 16 / kWorkThreads; // 2 float4 per thread and tile
-      constexpr int kStep = kWorkThreads * 16;
-      const uint32_t a_addr = smem_u32(a_hi(s)) + ct * 16, b_addr = smem_u32(b_hi(s)) + ct * 16;
-      float4 va[kPer], vb[kPer];
-#pragma unroll
-      for (int i = 0; i < kPer; ++i) va[i] = lds128(a_addr + i * kStep);
-      if (!BSPLIT) {
-#pragma unroll
-        for (int i = 0; i < kPer; ++i) vb[i] = lds128(b_addr + i * kStep);
-      }
-#pragma unroll
-      for (int i = 0; i < kPer; ++i) {
-        float4 h, l;
-        split4(va[i], h, l);
-        sts128(a_addr + i * kStep, h);
-        sts128(a_addr + kTileBytes + i * kStep, l);
-      }
-      if (!BSPLIT) {
-#pragma unroll
-        for (int i = 0; i < kPer; ++i) {
-          float4 h, l;
-          split4(vb[i], h, l);
-          sts128(b_addr + i * kStep, h);
-          sts128(b_addr + kTileBytes + i * kStep, l);
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to UMMA
-      __syncwarp();
-      if (lane == 0) {
-        if (rank == 0) mbar_arrive_local(&conv[s]);
-        else mbar_arrive_remote(&conv[s], 0);
-      }
-      if (ct == 0) TRL_TRACE(40 + kb);
-    }
-    // epilogue: TMEM lane quadrant of this warp = warp % 4.  The operand stages are free now (tmem_full fires after
-    // the last MMA of the pair has read them): the epilogue's output boxes are staged there.
-    asm volatile("bar.sync 1, %0;" ::"n"(kWorkThreads) : "memory");   // the epilogue warps: bias_s is complete
-    mbar_wait(tmem_full, 0);
-    if (ct == 0) TRL_TRACE(2);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // Streaming epilogue, 32 columns at a time: TMEM -> registers (this thread = one accumulator row) -> bias /
-    // activation -> a warp-private (32 rows x 128 bytes) box in the free operand stages, written in the 128-byte
-    // swizzle (16-byte piece j of row r at piece j ^ (r & 7): conflict-free STS.128) -> ONE TMA store per box
-    // (cp.async.bulk.tensor, full 128-byte lines, rows beyond M clipped by the tensor map).  No shared-memory read-back
-    // and no per-thread global stores: the copy engine drains box c while the warp loads and transforms box c + 1.
-    // 4 warps per TMEM lane quadrant (a warp may only touch lanes 32 (warp % 4) ..): each takes 2 of the 8 chunks, so
-    // that every SM sub-partition has 4 warps to hide the TMEM-load / MUFU / shared-memory latencies behind
-    const int quad = warp & 3, sub = (warp - 2) >> 2;
-    constexpr int kChunksPerWarp = (kBN / 32) / (kWorkWarps / 4);
-    constexpr uint32_t kBoxBytes = 32 * 128;
-    static_assert(kWorkWarps * kChunksPerWarp * kBoxBytes <= static_cast<uint32_t>(kStages) * kStageBytes, "boxes fit in the stages");
-    const uint32_t boxes = smem_u32(smem) + static_cast<uint32_t>(warp - 2) * (kChunksPerWarp * kBoxBytes);
-    const uint32_t my_row = boxes + static_cast<uint32_t>(lane) * 128u;
-    const uint32_t swz = static_cast<uint32_t>(lane & 7) << 4;
-    const uint32_t bias_addr = smem_u32(bias_s);
-    const bool has_bias = p.bias != nullptr;
-    const int act = p.act;
-    const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(quad * 32) << 16);
-    const long long row0 = static_cast<long long>(m_blk) * kBM + quad * 32;
-    const int crow = static_cast<int>(static_cast<long long>(split) * p.M + row0);   // row coordinate in map_c
-    const bool any_rows = row0 < p.M;
-#define TRL_TMEM_LD32(R, ADDR)                                                                                        \
-    asm volatile(                                                                                                     \
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                                     \
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                     \
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"                     \
-        : "=r"(R[0]), "=r"(R[1]), "=r"(R[2]), "=r"(R[3]), "=r"(R[4]), "=r"(R[5]), "=r"(R[6]), "=r"(R[7]), "=r"(R[8]),  \
-          "=r"(R[9]), "=r"(R[10]), "=r"(R[11]), "=r"(R[12]), "=r"(R[13]), "=r"(R[14]), "=r"(R[15]), "=r"(R[16]),      \
-          "=r"(R[17]), "=r"(R[18]), "=r"(R[19]), "=r"(R[20]), "=r"(R[21]), "=r"(R[22]), "=r"(R[23]), "=r"(R[24]),     \
-          "=r"(R[25]), "=r"(R[26]), "=r"(R[27]), "=r"(R[28]), "=r"(R[29]), "=r"(R[30]), "=r"(R[31])                   \
-        : "r"(ADDR))
-    uint32_t ra[32], rb[32];
-    const int c_first = sub * kChunksPerWarp;
-    TRL_TMEM_LD32(ra, taddr0 + static_cast<uint32_t>(c_first * 32));
-#pragma unroll
-    for (int cc = 0; cc < kChunksPerWarp; ++cc) {
-      const int c = c_first + cc;
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      uint32_t (&cur)[32] = (cc & 1) ? rb : ra;
-      uint32_t (&nxt)[32] = (cc & 1) ? ra : rb;
-      if (cc + 1 < kChunksPerWarp) TRL_TMEM_LD32(nxt, taddr0 + static_cast<uint32_t>((c + 1) * 32));
-      const uint32_t row_box = my_row + static_cast<uint32_t>(cc) * kBoxBytes;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 v = make_float4(__uint_as_float(cur[4 * j]), __uint_as_float(cur[4 * j + 1]), __uint_as_float(cur[4 * j + 2]),
-                               __uint_as_float(cur[4 * j + 3]));
-        if (has_bias) {   // fused Linear epilogue: z + b, then the activation (same op order as bias_act_fwd_kernel)
-          const float4 b = lds128(bias_addr + static_cast<uint32_t>((c * 32 + 4 * j) * 4));   // broadcast
-          v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
-          if (act == 1) {
-            v.x = tanh_mufu(v.x); v.y = tanh_mufu(v.y); v.z = tanh_mufu(v.z); v.w = tanh_mufu(v.w);
-          } else if (act == 2) {
-            v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-          }
-        }
-        sts128(row_box + ((static_cast<uint32_t>(j) << 4) ^ swz), v);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the copy engine
-      __syncwarp();
-      if (lane == 0 && any_rows) {
-        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                     ::"l"(reinterpret_cast<uint64_t>(&map_c)), "r"(boxes + static_cast<uint32_t>(cc) * kBoxBytes),
-                       "r"(c * 32), "r"(crow)
-                     : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-      if ((ct & 127) == 0 && lane == 0) TRL_TRACE(120 + c);
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // boxes read before smem goes away
-#undef TRL_TMEM_LD32
-    if (ct == 0) TRL_TRACE(3);
-    if (ct == 0) TRL_TRACE(4);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  cluster_sync_all();                     // nobody frees TMEM / exits while the peer still reads or is being read
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
-  }
-  if (threadIdx.x == 0) TRL_TRACE(5);
-}
 
 // C[i] = sum_s P[s][i]   (fixed order: 8 interleaved partial sums per element, combined as a balanced tree).  512
 // threads = 64 float4 elements x 8 groups; a group's loads are independent, eight of them in flight.
@@ -467,100 +48,17 @@ __global__ void __launch_bounds__(512) pair_splitk_reduce_kernel(const float* __
   }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-  }
-  return fn;
-}
-
-// (rows x cols) fp32 row-major matrix, box = (32 contiguous elements, box_rows).  K-major operands: cols = K,
-// SWIZZLE_128B, box_rows = 128; M/N-major operands: cols = M or N, SWIZZLE_128B_ATOM_32B, box_rows = 32.
-// Out-of-range rows / columns of a box are filled with zeros (ragged M).
-static bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, bool mn_major) {
-  PFN_encodeTiled enc = get_encode();
-  if (!enc) return false;
-  const cuuint64_t gdim[2] = {cols, rows};
-  const cuuint64_t gstride[1] = {cols * sizeof(float)};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kBK), static_cast<cuuint32_t>(mn_major ? 32 : kBM)};
-  const cuuint32_t estr[2] = {1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// the output (rows x 256) fp32 row-major: 32-column x 32-row boxes in the 128-byte swizzle, for the epilogue's TMA stores
-static bool make_map_c(CUtensorMap* map, float* base, uint64_t rows) {
-  PFN_encodeTiled enc = get_encode();
-  if (!enc) return false;
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(kBN), rows};
-  const cuuint64_t gstride[1] = {kBN * sizeof(float)};
-  const cuuint32_t box[2] = {32, 32};
-  const cuuint32_t estr[2] = {1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-#ifdef TRL_PAIR_TRACE
-static long long* g_trace = nullptr;
-static unsigned g_trace_cta = 0;
-#endif
-
-template <bool AMN, bool BMN, bool BSPLIT>
-static int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mb2, const Params& p, unsigned ctas_m,
-                  unsigned splits, cudaStream_t st, const char* what) {
-  CUtensorMap mc;
-  if (!make_map_c(&mc, p.C, static_cast<uint64_t>(splits) * static_cast<uint64_t>(p.M))) {
-    set_error("%s: cuTensorMapEncodeTiled failed for the output", what);
-    return TRL_EUNSUPPORTED;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm3_pair_kernel<AMN, BMN, BSPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         kSmemBytes);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return static_cast<int>(e); }
-    attr_set = true;
-  }
-#ifdef TRL_PAIR_TRACE
-  Params q = p;
-  q.trace = g_trace;
-  q.trace_cta = g_trace_cta;
-  gemm3_pair_kernel<AMN, BMN, BSPLIT><<<dim3(ctas_m, splits), kThreads, kSmemBytes, st>>>(ma, mb, mb2, mc, q);
-#else
-  gemm3_pair_kernel<AMN, BMN, BSPLIT><<<dim3(ctas_m, splits), kThreads, kSmemBytes, st>>>(ma, mb, mb2, mc, p);
-#endif
-  return check_launch(what);
-}
-
 }  // namespace pair
 }  // namespace trl
 
-#ifdef TRL_PAIR_TRACE
-// probe builds only (scripts/gemm_probe.py): 136 clock64() slots of CTA `cta` are written to `buf` by every launch
-TRL_API int trl_pair_set_trace(long long* buf, unsigned cta) {
-  trl::pair::g_trace = buf;
-  trl::pair::g_trace_cta = cta;
-  return 0;
-}
-#endif
-
-// C (M x 256) = act(A (M x K) . B + bias) on CTA pairs.  B is the (256 x K) row-major matrix (b_nmajor == 0: C = A B^T,
+// C (M x 256) = act(A (M x K) . B + bias) on the tensor cores.  B is the (256 x K) row-major matrix (b_nmajor == 0: C = A B^T,
 // the Linear forward) or the (K x 256) row-major matrix (b_nmajor != 0: C = A B, the dgrad shape).  b_lo == NULL: b_hi is
 // the raw fp32 matrix and is split in shared memory; b_lo != NULL: (b_hi, b_lo) are the pre-split planes of
 // trl_split_tf32 / trl_adam_step.  K % 32 == 0, 16-byte aligned pointers, any M >= 1 (ragged tail rows are masked).
 TRL_API int trl_gemm3_pair(const float* A, const float* b_hi, const float* b_lo, float* C, int64_t M, int64_t K,
                            int b_nmajor, const float* bias, int act, void* stream) {
   using namespace trl;
-  using namespace trl::pair;
+  using namespace trl::wg;
   TRL_REQUIRE(M >= 1 && K >= kBK && K % kBK == 0, "trl_gemm3_pair: bad sizes M=%lld K=%lld (K must be a multiple of 32)",
               (long long)M, (long long)K);
   TRL_REQUIRE(A && b_hi && C, "trl_gemm3_pair: null pointer");
@@ -568,7 +66,7 @@ TRL_API int trl_gemm3_pair(const float* A, const float* b_hi, const float* b_lo,
               "trl_gemm3_pair: pointers must be 16-byte aligned");
   TRL_REQUIRE(act >= 0 && act <= 2, "trl_gemm3_pair: unknown activation %d", act);
   CUtensorMap ma, mb, mb2;
-  const uint64_t b_rows = b_nmajor ? static_cast<uint64_t>(K) : kBN, b_cols = b_nmajor ? kBN : static_cast<uint64_t>(K);
+  const uint64_t b_rows = b_nmajor ? static_cast<uint64_t>(K) : kN, b_cols = b_nmajor ? kN : static_cast<uint64_t>(K);
   if (!make_map(&ma, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), false) ||
       !make_map(&mb, b_hi, b_rows, b_cols, b_nmajor != 0) ||
       !make_map(&mb2, b_lo ? b_lo : b_hi, b_rows, b_cols, b_nmajor != 0)) {
@@ -576,14 +74,13 @@ TRL_API int trl_gemm3_pair(const float* A, const float* b_hi, const float* b_lo,
     return TRL_EUNSUPPORTED;
   }
   Params p{bias, act, C, M, static_cast<int>(K / kBK)};
-  const unsigned ctas = 2u * static_cast<unsigned>(ceil_div<long long>(M, 2 * kBM));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (b_nmajor) {
-    if (b_lo) return launch<false, true, true>(ma, mb, mb2, p, ctas, 1, st, "gemm3_pair_kernel<nn,split>");
-    return launch<false, true, false>(ma, mb, mb2, p, ctas, 1, st, "gemm3_pair_kernel<nn>");
+    if (b_lo) return launch<false, true, true, true>(ma, mb, mb2, p, 1, st, "gemm3_wgmma_kernel<nn,split>");
+    return launch<false, true, false, true>(ma, mb, mb2, p, 1, st, "gemm3_wgmma_kernel<nn>");
   }
-  if (b_lo) return launch<false, false, true>(ma, mb, mb2, p, ctas, 1, st, "gemm3_pair_kernel<nt,split>");
-  return launch<false, false, false>(ma, mb, mb2, p, ctas, 1, st, "gemm3_pair_kernel<nt>");
+  if (b_lo) return launch<false, false, true, true>(ma, mb, mb2, p, 1, st, "gemm3_wgmma_kernel<nt,split>");
+  return launch<false, false, false, true>(ma, mb, mb2, p, 1, st, "gemm3_wgmma_kernel<nt>");
 }
 
 // C (M x 256) = A (K x M)^T . B (K x 256): the weight-gradient shape dW = g^T x, both operands consumed M/N-major
@@ -592,8 +89,8 @@ TRL_API int trl_gemm3_pair(const float* A, const float* b_hi, const float* b_lo,
 TRL_API int trl_gemm3_pair_tn(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
                               float* workspace, void* stream) {
   using namespace trl;
-  using namespace trl::pair;
-  TRL_REQUIRE(M >= 2 * kBM && M % (2 * kBM) == 0 && K >= kBK && splits >= 1,
+  using namespace trl::wg;
+  TRL_REQUIRE(M >= kN && M % kN == 0 && K >= kBK && splits >= 1,
               "trl_gemm3_pair_tn: bad sizes M=%lld K=%lld splits=%d (M must be a multiple of 256)", (long long)M,
               (long long)K, splits);
   TRL_REQUIRE(K % (static_cast<int64_t>(kBK) * splits) == 0, "trl_gemm3_pair_tn: K=%lld must be a multiple of 32*splits",
@@ -603,16 +100,15 @@ TRL_API int trl_gemm3_pair_tn(const float* A, const float* B, float* C, int64_t 
               "trl_gemm3_pair_tn: pointers must be 16-byte aligned");
   CUtensorMap ma, mb;
   if (!make_map(&ma, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), true) ||
-      !make_map(&mb, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kBN), true)) {
+      !make_map(&mb, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), true)) {
     set_error("trl_gemm3_pair_tn: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }
   Params p{nullptr, 0, splits > 1 ? workspace : C, M, static_cast<int>(K / kBK / splits)};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = launch<true, true, false>(ma, mb, mb, p, static_cast<unsigned>(M / kBM), static_cast<unsigned>(splits), st,
-                                     "gemm3_pair_kernel<tn>");
+  int rc = launch<true, true, false, true>(ma, mb, mb, p, static_cast<unsigned>(splits), st, "gemm3_wgmma_kernel<tn>");
   if (rc != TRL_OK || splits == 1) return rc;
-  const long long mn = M * kBN;
-  pair_splitk_reduce_kernel<<<static_cast<unsigned>(ceil_div<long long>(mn / 4, 64)), 512, 0, st>>>(workspace, C, mn, splits);
+  const long long mn = M * kN;
+  pair::pair_splitk_reduce_kernel<<<static_cast<unsigned>(ceil_div<long long>(mn / 4, 64)), 512, 0, st>>>(workspace, C, mn, splits);
   return check_launch("pair_splitk_reduce_kernel");
 }

@@ -1,335 +1,18 @@
-// gemm_tf32x3.cu -- fp32-faithful tensor-core GEMM for the 256-wide MLP layers (K3/K8 support).
+// gemm_tf32x3.cu -- entry points of the fp32-faithful 3xTF32 GEMM for the 256-wide MLP layers (K3/K8 support).
 //
-//   C[M x 256] = A[M x K] * B[256 x K]^T          (A, B row-major with K contiguous = "K-major")
+//   nt: C[M x 256] = act(A[M x K] . B[256 x K]^T + bias)      (A, B row-major with K contiguous = "K-major")
+//   tn: C[M x 256] = A[K x M]^T . B[K x 256]                   (the weight-gradient shape, split-K)
 //
-// The policy / value / Q networks of the hot path are MLP(256,256)s (SURVEY.md section 8(a) K3, K8); profiles
-// (profiles/launches_ppo_step_r1.md) show their three big GEMM shapes -- forward (x W^T), dgrad (g W) and
-// wgrad (g^T x) -- at ~50 % of a PPO minibatch on cuBLAS' fp32 SIMT kernels (~45 TFLOP/s).  This kernel
-// runs them on the 5th-gen tensor cores WITHOUT giving up fp32 accuracy: every operand element is split
-// in shared memory into x = hi + lo (hi = TF32-rounded, lo = exact remainder) and each 8-deep K step
-// issues three tcgen05.mma.kind::tf32 (lo*hi, hi*lo, hi*hi) into the same fp32 TMEM accumulator
-// ("3xTF32"; the dropped lo*lo term is O(2^-22) relative, measured error equals the SIMT sgemm's).
-//
-// Structure (one CTA per 128x256 output tile and K-slab, 192 threads):
-//   warp 0      TMA producer : cp.async.bulk.tensor 2D loads of the raw fp32 A (128x32) / B (256x32) tiles,
-//                              SWIZZLE_128B, 2-stage ring, mbarrier complete_tx
-//   warps 2..5  converters   : split raw -> (hi in place, lo in a twin buffer); the 128B swizzle permutes 16-byte
-//                              chunks, so a chunk-wise elementwise pass preserves the canonical UMMA layout;
-//                              fence.proxy.async + mbarrier arrive hands the stage to the MMA warp
-//   warp 1      MMA issuer   : one elected lane issues 12 tcgen05.mma per stage (4 K-steps x 3 products),
-//                              tcgen05.commit releases the stage / signals the epilogue; owns the 256 TMEM columns
-//   warps 2..5  epilogue     : tcgen05.ld 32x32b -> registers -> global (optionally a split-K partial slab)
+// The policy / value / Q networks of the hot path are MLP(256,256)s (SURVEY.md section 8(a) K3, K8); their three big
+// GEMM shapes -- forward (x W^T), dgrad (g W) and wgrad (g^T x) -- run on the tensor cores without giving up fp32
+// accuracy through the warpgroup-MMA kernel of gemm_wgmma.cuh (every operand split into hi + lo, three tf32 products).
+// These entry points take raw fp32 operands, apply tanh with libdevice tanhf and sum split-K slabs in a fixed order
+// (splitk_reduce_kernel, deterministic); csrc/gemm_pair.cu serves the hot path with pre-split weights.
 // Accuracy: the tensor core's fp32 accumulation truncates, so the error grows ~linearly with the reduction length
-// accumulated in TMEM: 2e-6 (relative to max|C|) at 256, 7e-6 at 1024 -- vs 7e-7 for the SIMT sgemm and 3e-4 for
-// plain TF32.  Callers keep K/splits <= 256 (the MLP layers here: K = 256; wgrad: 16384/64).
-// Split-K (gridDim.y slabs) serves the wgrad shape (tiny output, K = minibatch): partials are summed in a fixed
-// order by splitk_reduce_kernel (deterministic).
-#include "common.cuh"
-#include <cuda.h>
-#include <cstdlib>
+// accumulated by one CTA.  Callers keep K/splits <= 256 (the MLP layers here: K = 256; wgrad: 16384/64).
+#include "gemm_wgmma.cuh"
 
 namespace trl {
-
-constexpr int kBM = 128, kBN = 256, kBK = 32;          // tile; kBK fp32 = one 128-byte swizzle row
-constexpr int kStages = 2;
-constexpr int kUmmaK = 8;                              // tf32: 32 bytes per MMA K-step
-constexpr int kABytes = kBM * kBK * 4;                 // 16 KB
-constexpr int kBBytes = kBN * kBK * 4;                 // 32 KB
-constexpr int kStageBytes = 2 * (kABytes + kBBytes);   // hi + lo of A and B = 96 KB
-constexpr int kGemmThreads = 192;
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c_inner, int c_outer) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer)
-      : "memory");
-}
-// K-major, SWIZZLE_128B canonical layout: 8-row atoms of 1024 B; SBO = 1024 B; LBO unused (1); version 1.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);        // start address  [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                           // leading byte offset (ignored for swizzled K-major)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;                   // stride byte offset [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                           // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                           // layout type: SWIZZLE_128B
-  return d;
-}
-// MN-major fp32 operands: the ONLY shared-memory layout tcgen05 accepts for M/N-major tf32 is
-// SWIZZLE_128B_BASE32B (layout type 1; cutlass sm100_common.inl: "for mn-major tf32 operands, SW128_32B is the
-// only available smem layout"): rows of 128 B = 32 contiguous M/N elements at one reduction index, atoms of
-// 4 such rows (512 B) in which the 32-byte unit index is XORed with the row index (Swizzle<2,5,2> on byte
-// addresses) -- exactly what TMA's CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B writes.  SBO = 512 B between successive
-// 4-row atoms along K, LBO = byte distance between successive groups of 32 M/N elements.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128_32b(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(1) << 61;                           // layout type: SWIZZLE_128B_BASE32B
-  return d;
-}
-// kind::tf32, fp32 accumulate, M = 128, N = 256; MN = both operands M/N-major instead of K-major
-template <bool MN>
-__device__ __forceinline__ uint32_t umma_idesc_tf32_128x256() {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (MN ? (1u << 15) | (1u << 16) : 0u) |
-         (static_cast<uint32_t>(kBN >> 3) << 17) | (static_cast<uint32_t>(kBM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void split4(const float4 v, float4& h, float4& l) {
-  unsigned u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.x)); h.x = __uint_as_float(u); l.x = v.x - h.x;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.y)); h.y = __uint_as_float(u); l.y = v.y - h.y;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.z)); h.z = __uint_as_float(u); l.z = v.z - h.z;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.w)); h.w = __uint_as_float(u); l.w = v.w - h.w;
-}
-
-__device__ __forceinline__ float tanh_mufu(float x) { return ::trl::tanh_ex2(x); }   // common.cuh, as csrc/skinny.cu
-
-struct GemmParams {
-  const float* __restrict__ bias;  // (256) added in the epilogue, or nullptr
-  int act;                         // 0 none, 1 tanh, 2 relu (applied after the bias)
-  float* __restrict__ C;       // (splits, M, 256) when splits > 1 else (M, 256)
-  long long M;
-  int k_blocks_per_split;      // K-blocks (of 32) handled by one CTA
-  int ldc;                     // 256
-};
-
-// MN == false: C = A . B^T with A (M x K), B (256 x K) row-major (K-major operands).
-// MN == true : C = A^T . B  with A (K x M), B (K x 256) row-major (M/N-major operands; the wgrad shape).
-// STAGED (opt-in, TORCHRL_B200_GEMM_STAGED=1; not yet validated on hardware): the epilogue goes through shared
-// memory so that every global store instruction of a warp writes 512 contiguous bytes instead of 16 bytes of 32
-// different rows, and tanh uses two MUFU ops (|abs err| < 2e-7) instead of libdevice tanhf on only four warps.
-template <bool MN, bool STAGED>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                   const GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  // stage s: [A_hi | A_lo | B_hi | B_lo]
-  auto a_hi = [&](int s) { return smem + s * kStageBytes; };
-  auto a_lo = [&](int s) { return smem + s * kStageBytes + kABytes; };
-  auto b_hi = [&](int s) { return smem + s * kStageBytes + 2 * kABytes; };
-  auto b_lo = [&](int s) { return smem + s * kStageBytes + 2 * kABytes + kBBytes; };
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* full = bars;                 // [kStages]  TMA -> converters
-  uint64_t* conv = bars + kStages;       // [kStages]  converters -> MMA
-  uint64_t* empty = bars + 2 * kStages;  // [kStages]  MMA -> TMA
-  uint64_t* tmem_full = bars + 3 * kStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_blk = blockIdx.x, split = blockIdx.y;
-  const int nkb = p.k_blocks_per_split;
-  const int kb0 = split * nkb;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < kStages; ++s) {
-        mbar_init(&full[s], 1);
-        mbar_init(&conv[s], 4);          // one arrival per converter warp
-        mbar_init(&empty[s], 1);
-      }
-      mbar_init(tmem_full, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    // 256 fp32 accumulator columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (kb / kStages) & 1;
-        mbar_wait(&empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&full[s], kABytes + kBBytes);
-        if (!MN) {
-          tma_load_2d(a_hi(s), &map_a, &full[s], (kb0 + kb) * kBK, m_blk * kBM);
-          tma_load_2d(b_hi(s), &map_b, &full[s], (kb0 + kb) * kBK, 0);
-        } else {
-          // one (32 M/N elements x 32 reduction rows) box per group of 32 output rows / columns, 4 KB apart
-#pragma unroll
-          for (int g = 0; g < kBM / 32; ++g)
-            tma_load_2d(a_hi(s) + g * 4096, &map_a, &full[s], m_blk * kBM + g * 32, (kb0 + kb) * kBK);
-#pragma unroll
-          for (int g = 0; g < kBN / 32; ++g)
-            tma_load_2d(b_hi(s) + g * 4096, &map_b, &full[s], g * 32, (kb0 + kb) * kBK);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_tf32_128x256<MN>();
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % kStages;
-        const uint32_t ph = (kb / kStages) & 1;
-        mbar_wait(&conv[s], ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t da_hi = MN ? umma_desc_mn_sw128_32b(smem_u32(a_hi(s)), 4096) : umma_desc_k_sw128(smem_u32(a_hi(s)));
-        const uint64_t da_lo = MN ? umma_desc_mn_sw128_32b(smem_u32(a_lo(s)), 4096) : umma_desc_k_sw128(smem_u32(a_lo(s)));
-        const uint64_t db_hi = MN ? umma_desc_mn_sw128_32b(smem_u32(b_hi(s)), 4096) : umma_desc_k_sw128(smem_u32(b_hi(s)));
-        const uint64_t db_lo = MN ? umma_desc_mn_sw128_32b(smem_u32(b_lo(s)), 4096) : umma_desc_k_sw128(smem_u32(b_lo(s)));
-#pragma unroll
-        for (int k = 0; k < kBK / kUmmaK; ++k) {
-          // K-major: +32 B per K-step inside the 128 B swizzle row; MN-major: +1024 B = 8 reduction rows further
-          const uint64_t adv = static_cast<uint64_t>((MN ? k * 1024 : k * kUmmaK * 4) >> 4);
-          umma_tf32(tmem_base, da_lo + adv, db_hi + adv, idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_tf32(tmem_base, da_hi + adv, db_lo + adv, idesc, 1u);
-          umma_tf32(tmem_base, da_hi + adv, db_hi + adv, idesc, 1u);
-        }
-        umma_commit(&empty[s]);                       // stage free once these MMAs have read it
-      }
-      umma_commit(tmem_full);                         // accumulator complete
-    }
-  } else {
-    // ------------------------------------------------------------------ converters (warps 2..5), then epilogue
-    const int ct = threadIdx.x - 64;                  // 0..127
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % kStages;
-      const uint32_t ph = (kb / kStages) & 1;
-      mbar_wait(&full[s], ph);
-      float4* ah = reinterpret_cast<float4*>(a_hi(s));
-      float4* al = reinterpret_cast<float4*>(a_lo(s));
-#pragma unroll
-      for (int i = 0; i < kABytes / 16 / 128; ++i) {
-        const int c = ct + i * 128;
-        float4 h, l;
-        split4(ah[c], h, l);
-        ah[c] = h;
-        al[c] = l;
-      }
-      float4* bh = reinterpret_cast<float4*>(b_hi(s));
-      float4* bl = reinterpret_cast<float4*>(b_lo(s));
-#pragma unroll
-      for (int i = 0; i < kBBytes / 16 / 128; ++i) {
-        const int c = ct + i * 128;
-        float4 h, l;
-        split4(bh[c], h, l);
-        bh[c] = h;
-        bl[c] = l;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to UMMA
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&conv[s]);
-    }
-    // epilogue: TMEM lane quadrant of this warp = warp % 4
-    mbar_wait(tmem_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int quad = warp & 3;
-    const long long row = static_cast<long long>(m_blk) * kBM + quad * 32 + lane;
-    float* crow = p.C + (static_cast<long long>(split) * p.M + row) * p.ldc;
-    // STAGED: the operand stages are free now (tmem_full fires after the last MMA has read them): this warp's 32
-    // rows are parked there with a pitch of 260 floats (conflict-free 16-byte accesses by row AND by column)
-    constexpr int kPitch = kBN + 4;
-    float* park = reinterpret_cast<float*>(smem) + static_cast<size_t>(quad) * 32 * kPitch;
-#pragma unroll 1
-    for (int c = 0; c < kBN / 32; ++c) {
-      uint32_t r[32];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>(c * 32);
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-          "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-            "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-            "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-            "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (STAGED || row < p.M) {
-        float4* dst = STAGED ? reinterpret_cast<float4*>(park + lane * kPitch + c * 32)
-                             : reinterpret_cast<float4*>(crow + c * 32);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 v = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                                 __uint_as_float(r[4 * j + 3]));
-          if (p.bias) {   // fused Linear epilogue: z + b, then the activation (same op order as bias_act_fwd_kernel)
-            const float4 b = *reinterpret_cast<const float4*>(p.bias + c * 32 + 4 * j);
-            v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
-            if (p.act == 1) {
-              if (STAGED) { v.x = tanh_mufu(v.x); v.y = tanh_mufu(v.y); v.z = tanh_mufu(v.z); v.w = tanh_mufu(v.w); }
-              else { v.x = tanhf(v.x); v.y = tanhf(v.y); v.z = tanhf(v.z); v.w = tanhf(v.w); }
-            } else if (p.act == 2) {
-              v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-            }
-          }
-          dst[j] = v;
-        }
-      }
-    }
-    if (STAGED) {
-      __syncwarp();                                     // the 32 rows of this warp are complete in shared memory
-      const long long row0 = static_cast<long long>(m_blk) * kBM + quad * 32;
-      float* cbase = p.C + (static_cast<long long>(split) * p.M + row0) * p.ldc;
-#pragma unroll 4
-      for (int rr = 0; rr < 32; ++rr) {
-        if (row0 + rr >= p.M) break;
-        const float4* src = reinterpret_cast<const float4*>(park + rr * kPitch);
-        float4* out = reinterpret_cast<float4*>(cbase + static_cast<long long>(rr) * p.ldc);
-        out[lane] = src[lane];                          // 512 contiguous bytes per warp instruction
-        out[lane + 32] = src[lane + 32];
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
-  }
-}
 
 // C[m][n] = sum_s P[s][m][n]   (fixed order: 4 interleaved partial sums per element combined pairwise)
 // CTA = 64 float4 outputs x 4 split groups; group g sums splits g, g+4, ...; groups combined through smem.
@@ -373,44 +56,6 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
   }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-  }
-  return fn;
-}
-
-// rows x K fp32 row-major matrix, box = (32 contiguous elements, box_rows), 128B swizzle
-static bool staged_epilogue() {
-  static const bool on = [] {
-    const char* e = getenv("TORCHRL_B200_GEMM_STAGED");
-    return e && e[0] == '1';
-  }();
-  return on;
-}
-
-static bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t K, uint32_t box_rows,
-                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
-  PFN_encodeTiled enc = get_encode();
-  if (!enc) return false;
-  const cuuint64_t gdim[2] = {K, rows};
-  const cuuint64_t gstride[1] = {K * sizeof(float)};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kBK), box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 }  // namespace trl
 
 // C (M x 256) = act(A (M x K) . B (256 x K)^T [+ bias]) with 3xTF32 tensor-core arithmetic (bias NULL: plain GEMM).
@@ -419,37 +64,28 @@ static bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_
 TRL_API int trl_gemm_tf32x3_nt(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
                                float* workspace, const float* bias, int act, void* stream) {
   using namespace trl;
-  TRL_REQUIRE(M >= 1 && K >= kBK && splits >= 1, "trl_gemm_tf32x3_nt: bad sizes M=%lld K=%lld splits=%d", (long long)M,
+  TRL_REQUIRE(M >= 1 && K >= wg::kBK && splits >= 1, "trl_gemm_tf32x3_nt: bad sizes M=%lld K=%lld splits=%d", (long long)M,
               (long long)K, splits);
-  TRL_REQUIRE(K % (static_cast<int64_t>(kBK) * splits) == 0, "trl_gemm_tf32x3_nt: K=%lld must be a multiple of 32*splits",
+  TRL_REQUIRE(K % (static_cast<int64_t>(wg::kBK) * splits) == 0, "trl_gemm_tf32x3_nt: K=%lld must be a multiple of 32*splits",
               (long long)K);
   TRL_REQUIRE(A && B && C && (splits == 1 || workspace), "trl_gemm_tf32x3_nt: null pointer");
   TRL_REQUIRE(aligned16(A) && aligned16(B) && aligned16(C) && aligned16(workspace) && aligned16(bias),
               "trl_gemm_tf32x3_nt: pointers must be 16-byte aligned");
   TRL_REQUIRE(!(bias && splits > 1), "trl_gemm_tf32x3_nt: the bias/activation epilogue needs splits == 1");
   TRL_REQUIRE(act >= 0 && act <= 2, "trl_gemm_tf32x3_nt: unknown activation %d", act);
+  using namespace trl::wg;
   CUtensorMap map_a, map_b;
-  if (!make_map(&map_a, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), kBM) ||
-      !make_map(&map_b, B, static_cast<uint64_t>(kBN), static_cast<uint64_t>(K), kBN)) {
+  if (!make_map(&map_a, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), false) ||
+      !make_map(&map_b, B, static_cast<uint64_t>(kN), static_cast<uint64_t>(K), false)) {
     set_error("trl_gemm_tf32x3_nt: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-    attr_set = true;
-  }
-  GemmParams p{bias, act, splits > 1 ? workspace : C, M, static_cast<int>(K / kBK / splits), kBN};
-  const dim3 grid(static_cast<unsigned>(ceil_div<long long>(M, kBM)), static_cast<unsigned>(splits));
+  Params p{bias, act, splits > 1 ? workspace : C, M, static_cast<int>(K / kBK / splits)};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (staged_epilogue()) gemm_tf32x3_kernel<false, true><<<grid, kGemmThreads, kSmemBytes, st>>>(map_a, map_b, p);
-  else gemm_tf32x3_kernel<false, false><<<grid, kGemmThreads, kSmemBytes, st>>>(map_a, map_b, p);
-  int rc = check_launch("gemm_tf32x3_kernel<nt>");
+  int rc = launch<false, false, false, false>(map_a, map_b, map_b, p, static_cast<unsigned>(splits), st,
+                                              "gemm3_wgmma_kernel<nt>");
   if (rc != TRL_OK || splits == 1) return rc;
-  const long long mn = M * kBN;
+  const long long mn = M * kN;
   splitk_reduce_kernel<<<static_cast<unsigned>(ceil_div<long long>(mn / 4, 64)), 256, 0, st>>>(workspace, C, mn, splits);
   return check_launch("splitk_reduce_kernel");
 }
@@ -459,36 +95,27 @@ TRL_API int trl_gemm_tf32x3_nt(const float* A, const float* B, float* C, int64_t
 TRL_API int trl_gemm_tf32x3_tn(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
                                float* workspace, void* stream) {
   using namespace trl;
-  TRL_REQUIRE(M >= kBM && M % kBM == 0 && K >= kBK && splits >= 1, "trl_gemm_tf32x3_tn: bad sizes M=%lld K=%lld splits=%d",
+  TRL_REQUIRE(M >= wg::kBM && M % wg::kBM == 0 && K >= wg::kBK && splits >= 1, "trl_gemm_tf32x3_tn: bad sizes M=%lld K=%lld splits=%d",
               (long long)M, (long long)K, splits);
-  TRL_REQUIRE(K % (static_cast<int64_t>(kBK) * splits) == 0, "trl_gemm_tf32x3_tn: K=%lld must be a multiple of 32*splits",
+  TRL_REQUIRE(K % (static_cast<int64_t>(wg::kBK) * splits) == 0, "trl_gemm_tf32x3_tn: K=%lld must be a multiple of 32*splits",
               (long long)K);
   TRL_REQUIRE(A && B && C && (splits == 1 || workspace), "trl_gemm_tf32x3_tn: null pointer");
   TRL_REQUIRE(aligned16(A) && aligned16(B) && aligned16(C) && aligned16(workspace),
               "trl_gemm_tf32x3_tn: pointers must be 16-byte aligned");
+  using namespace trl::wg;
   CUtensorMap map_a, map_b;
-  // (K rows) x (M | 256 contiguous) matrices, boxes of 32 contiguous elements x 32 reduction rows
-  if (!make_map(&map_a, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) ||
-      !make_map(&map_b, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kBN), 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) {
+  // (K rows) x (M | 256 contiguous) matrices, consumed M/N-major
+  if (!make_map(&map_a, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), true) ||
+      !make_map(&map_b, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), true)) {
     set_error("trl_gemm_tf32x3_tn: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-    attr_set = true;
-  }
-  GemmParams p{nullptr, 0, splits > 1 ? workspace : C, M, static_cast<int>(K / kBK / splits), kBN};
-  const dim3 grid(static_cast<unsigned>(M / kBM), static_cast<unsigned>(splits));
+  Params p{nullptr, 0, splits > 1 ? workspace : C, M, static_cast<int>(K / kBK / splits)};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (staged_epilogue()) gemm_tf32x3_kernel<true, true><<<grid, kGemmThreads, kSmemBytes, st>>>(map_a, map_b, p);
-  else gemm_tf32x3_kernel<true, false><<<grid, kGemmThreads, kSmemBytes, st>>>(map_a, map_b, p);
-  int rc = check_launch("gemm_tf32x3_kernel<tn>");
+  int rc = launch<true, true, false, false>(map_a, map_b, map_b, p, static_cast<unsigned>(splits), st,
+                                            "gemm3_wgmma_kernel<tn>");
   if (rc != TRL_OK || splits == 1) return rc;
-  const long long mn = M * kBN;
+  const long long mn = M * kN;
   splitk_reduce_kernel<<<static_cast<unsigned>(ceil_div<long long>(mn / 4, 64)), 256, 0, st>>>(workspace, C, mn, splits);
   return check_launch("splitk_reduce_kernel");
 }

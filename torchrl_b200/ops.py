@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI (include/torchrl_b200.h).
 
 Each function takes torch CUDA tensors, checks dtype / contiguity / device, and launches
-the sm_100a kernel on torch's *current* stream (so every call is CUDA-graph capturable).
+the sm_90a kernel on torch's *current* stream (so every call is CUDA-graph capturable).
 Memory is owned by PyTorch's caching allocator; the library never allocates.  There is no
 CPU implementation: CPU tensors raise.
 """
@@ -431,7 +431,7 @@ def per_insert(prio, row_ptr, max_prio):
 
 # ------------------------------------------------------------------------------------------ tensor-core GEMM
 def gemm_tf32x3_nt(a, b, out=None, splits=1, workspace=None, bias=None, act=0):
-    """out (M,256) = a (M,K) @ b (256,K)^T on the tcgen05 tensor cores with 3xTF32 error compensation
+    """out (M,256) = a (M,K) @ b (256,K)^T on the tensor cores (wgmma) with 3xTF32 error compensation
     (csrc/gemm_tf32x3.cu).  a, b contiguous fp32, K % (32*splits) == 0."""
     M, K = a.shape
     assert b.shape == (256, K), "B must be (256, K)"
@@ -447,7 +447,7 @@ def gemm_tf32x3_nt(a, b, out=None, splits=1, workspace=None, bias=None, act=0):
 
 
 def gemm_tf32x3_tn(a, b, out=None, splits=1, workspace=None):
-    """out (M,256) = a (K,M)^T @ b (K,256): the weight-gradient shape dW = g^T x on the tcgen05 tensor cores
+    """out (M,256) = a (K,M)^T @ b (K,256): the weight-gradient shape dW = g^T x on the tensor cores (wgmma)
     (3xTF32), operands consumed M/N-major straight from their row-major storage (no transposes)."""
     K, M = a.shape
     assert b.shape == (K, 256), "B must be (K, 256)"
@@ -463,7 +463,7 @@ def gemm_tf32x3_tn(a, b, out=None, splits=1, workspace=None):
 
 
 def gemm3_pair(a, b, out=None, planes=None, b_nmajor=False, bias=None, act=0):
-    """out (M,256) = act(a (M,K) @ B + bias) on CTA pairs (csrc/gemm_pair.cu, tcgen05 cta_group::2, 3xTF32).
+    """out (M,256) = act(a (M,K) @ B + bias) on the tensor cores (csrc/gemm_pair.cu, wgmma, 3xTF32).
     b_nmajor False: b is (256,K) and B = b^T (Linear forward); True: b is (K,256) and B = b (dgrad).
     planes = (hi, lo): pre-split TF32 planes of b (same shape), else b is split in shared memory."""
     M, K = a.shape
@@ -482,7 +482,7 @@ def gemm3_pair(a, b, out=None, planes=None, b_nmajor=False, bias=None, act=0):
 
 
 def gemm3_pair_tn(a, b, out=None, splits=1, workspace=None):
-    """out (M,256) = a (K,M)^T @ b (K,256) on CTA pairs: the weight-gradient shape, deterministic split-K."""
+    """out (M,256) = a (K,M)^T @ b (K,256) on the tensor cores: the weight-gradient shape, deterministic split-K."""
     K, M = a.shape
     assert b.shape == (K, 256), "B must be (K, 256)"
     if out is None:
