@@ -146,6 +146,24 @@ int trl_ppo_critic_loss(const float* values, const float* returns, const float* 
 int trl_gaussian_log_prob(const float* mean, const float* log_std, int ls_stride, const float* actions,
                           int64_t B, int act_dim, int tanh_action, float* logp, void* stream);
 
+/* ---- K13: categorical distribution of the discrete on-policy path (csrc/categorical.cu), torch's
+ * Categorical(probs=softmax(logits)): CategoricalDisPolicy.explore / update (policies/discrete_policies.py:123-160).
+ * Logits (M, A) row-major, 1 <= A <= 32; actions are indices stored as float.
+ * Sampling by inverse CDF over p with one uniform per row: u (M) given, or (u NULL) Philox4x32-10 keyed by
+ * (seed, *rng_counter, row).  Rows with a non-finite logit set *nan_flag (may be NULL) and get action 0. */
+int trl_categorical_sample(const float* logits, const float* u, uint64_t seed, const uint64_t* rng_counter, int64_t M,
+                           int num_actions, float* action, float* log_prob, int* nan_flag, void* stream);
+/* log pi(a|s) of stored actions, log(clamp(p_a, eps, 1-eps)) (the old log-probs of PPO, ppo.py:54-56). */
+int trl_categorical_log_prob(const float* logits, const float* actions, int64_t M, int num_actions, float* logp,
+                             void* stream);
+int64_t trl_ppo_categorical_actor_scratch_doubles(int64_t B);
+/* trl_ppo_actor_loss for a categorical policy (ppo.py:41-91 / a2c.py:66-70): old_logp NULL = A2C's plain policy
+ * gradient; writes dL/dlogits (B, A) and the same info16 slots (the log-std slots 7-10 are zero). */
+int trl_ppo_categorical_actor_loss(const float* logits, const float* actions, const float* old_logp, const float* advs,
+                                   const float* adv_stats, const int* adv_stats_pos, int64_t B, int num_actions,
+                                   float clip_para, float entropy_coeff, float* g_logits, float* logp_out,
+                                   float* info16, double* scratch, unsigned* ticket, void* stream);
+
 /* ---- K11: flat-buffer grad-norm clip + Adam, Polyak (algo/utils.py:16-25, ppo.py:72-74,117-119). */
 int trl_grad_sumsq_blocks(int nseg);
 int trl_grad_sumsq(const float* grad, const int64_t* seg_begin_host, int nseg, unsigned active_mask,

@@ -21,6 +21,7 @@ from ...flat import FlatAdam
 from ...networks import fused
 from ..rl_algo import SegmentOptimizer
 from .on_rl_algo import OnRLAlgo
+from .policy_heads import gaussian_outputs, policy_head
 
 _HALF_LOG_2PI = 0.5 * float(np.log(2.0 * np.pi))
 _ADV_KEYS = ['advs/mean', 'advs/std', 'advs/max', 'advs/min']
@@ -47,6 +48,7 @@ class A2C(OnRLAlgo):
         self.vf_criterion = torch.nn.MSELoss()
         self.sample_key = ["obs", "acts", "advs", "estimate_returns"]
         self.tanh_action = bool(getattr(pf, "tanh_action", False))
+        self._head = policy_head(pf)
         self._mb_graph = None
         self._mb_eager_runs = 0
         self._mb_state = None
@@ -80,57 +82,32 @@ class A2C(OnRLAlgo):
 
     def _actor_step(self, batch, info):
         st = self._mb_state
-        mean, raw_ls, clamp, g_ls = self._raw_policy_outputs(self.pf, batch["obs"])
-        g_mean, _, _ = ops.ppo_actor_loss(mean, raw_ls.detach(), batch["acts"].reshape(mean.shape[0], -1), None,
-                                          batch["advs"].reshape(-1), st["adv_table"], 0.0, self.entropy_coeff,
-                                          self.tanh_action, st["scratch"], g_log_std=g_ls, info=info[0:16],
-                                          stats_pos=st["upd"], ls_clamp=clamp)
-        with fused.backward_fork():
-            torch.autograd.backward([mean], [g_mean])
-        # std/* (a2c.py:90-94) derive from the clamped log-std at flush
-        torch.clamp(raw_ls.detach(), clamp[0], clamp[1], out=info[28:28 + raw_ls.numel()])
+        self._head.minibatch_actor(self.pf, batch["obs"], batch["acts"], None, batch["advs"].reshape(-1),
+                                   st["adv_table"], st["upd"], 0.0, self.entropy_coeff, st["scratch"], info)
+        self._head.log_std_row(self.pf, info)
 
     def _pre_update(self):
         """Host-side work of an epoch before the minibatch loop (schedules, target copies)."""
 
     def _decode_info(self, row, norms, gs):
-        a = self.replay_buffer._acts.shape[-1]
-        ls = row[28:28 + a].astype(np.float64)
-        sd = np.exp(ls)
-        B = self._mb_state["B"]
-        m = sd.mean()
-        var = B * ((sd - m) ** 2).sum() / (B * a - 1.0)              # torch.std() of the (B, a) expanded tensor
-        return {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16]),
+        info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16]),
                 'v_pred/mean': float(row[24]), 'v_pred/std': float(row[25]), 'v_pred/max': float(row[26]),
-                'v_pred/min': float(row[27]), 'std/mean': float(m), 'std/std': float(np.sqrt(var)),
-                'std/max': float(sd.max()), 'std/min': float(sd.min()), 'ent': float(row[11]),
-                'log_prob': float(row[1])}
+                'v_pred/min': float(row[27])}
+        info.update(self._head.a2c_std_info(row, self._mb_state["B"], self.replay_buffer._acts.shape[-1]))
+        info['ent'] = float(row[11])
+        info['log_prob'] = float(row[1])
+        return info
 
     # ------------------------------------------------------------------ helpers
     def _policy_outputs(self, pf, obs):
-        mean, _, log_std = pf(obs)
-        if not mean.is_contiguous():
-            mean = mean.contiguous()
-        if not log_std.is_contiguous():
-            log_std = log_std.contiguous()
+        mean, _, log_std = gaussian_outputs(pf, obs)
         return mean, log_std
 
-    def _raw_policy_outputs(self, pf, obs):
-        """Device minibatch path (a shared log-std PARAMETER, _device_path_ok): the mean, the raw parameter, its clamp
-        range and the slice of the flat gradient buffer that belongs to it.  The loss kernel applies the policy's
-        torch.clamp itself and writes the parameter's gradient in place, which removes the clamp / exp / clamp-backward
-        / accumulate launches on six-element tensors from every minibatch."""
-        from ...policies.continuous_policy import LOG_SIG_MIN, LOG_SIG_MAX
-        mean = pf.mean_net(obs)
-        if not mean.is_contiguous():
-            mean = mean.contiguous()
-        return mean, pf.logstd, (LOG_SIG_MIN, LOG_SIG_MAX), pf.logstd.grad
-
     def _device_path_ok(self):
-        """The fused minibatch loop needs a Gaussian policy with a shared log-std vector (GuassianContPolicyBasicBias)
-        over a device rollout buffer; anything else takes the eager `update(batch)` route."""
+        """The fused minibatch loop needs a policy its head supports (a Gaussian policy with a shared log-std vector,
+        or a categorical policy) over a device rollout buffer; anything else takes the eager `update(batch)` route."""
         rb = self.replay_buffer
-        return hasattr(self.pf, "logstd") and rb is not None and hasattr(rb, "gather_rows") and hasattr(rb, "_rewards")
+        return self._head.fused_ok(self.pf) and rb is not None and hasattr(rb, "gather_rows") and hasattr(rb, "_rewards")
 
     def _mb_setup(self):
         rb = self.replay_buffer
@@ -143,7 +120,6 @@ class A2C(OnRLAlgo):
         passes = self._passes()
         U = passes * n_mb
         dev = self.device
-        a = rb._acts.shape[-1]
         st = {
             "b": b, "n_mb": n_mb, "U": U, "B": b * N, "passes": passes,
             # every pass' row order is uploaded up-front: (passes, T) indices, minibatch u of the epoch reads
@@ -155,7 +131,7 @@ class A2C(OnRLAlgo):
             "log_ticket": torch.zeros(1, dtype=torch.int32, device=dev),
             "log32": torch.zeros(U, 64, dtype=torch.float32, device=dev),
             "log64": torch.zeros(U, self.opt.sumsq3.numel(), dtype=torch.float64, device=dev),
-            "scratch": ops.LossScratch(b * N, a, dev),
+            "scratch": self._head.loss_scratch(b * N, rb._acts, dev),
             # advantage statistics of all U minibatches, computed once per epoch (mean, std, max, min per row)
             "adv_table": torch.zeros(U, 4, dtype=torch.float32, device=dev),
             "keys": self._gather_keys(),
@@ -172,6 +148,7 @@ class A2C(OnRLAlgo):
         with fused.direct_grad(), fused.deferred_reduces():
             st, rb = self._mb_state, self.replay_buffer
             batch = rb.gather_rows(st["perm"], st["keys"], pos_ptr=st["upd"], rows=st["b"])
+            batch["obs"] = self._prep_obs(batch["obs"])
             info = st["info"][0]
             if self.overlap_nets:
                 # the critic and the actor branch share nothing but their (read-only) inputs: run them on two streams
@@ -290,21 +267,14 @@ class A2C(OnRLAlgo):
         self.training_update_num += 1
         obs, acts, advs, est_rets = self._minibatch(batch, ('obs', 'acts', 'advs', 'estimate_returns'))
         B = obs.shape[0]
-        acts = acts.reshape(B, -1)
-        scratch = ops.LossScratch(B, acts.shape[1], self.device)
+        scratch = self._head.loss_scratch(B, acts.reshape(B, -1), self.device)
         info32 = torch.zeros(32, dtype=torch.float32, device=self.device)
         adv_stats = ops.vec_stats(advs.reshape(-1), out=info32[20:24])
         values = self.vf(obs)
         g_v, _ = ops.ppo_critic_loss(values.reshape(-1), est_rets.reshape(-1), None, False, 0.0, scratch, info=info32[16:17])
         torch.autograd.backward([values], [g_v.reshape(values.shape)])
-        mean, std, log_std = self.pf(obs)
-        mean = mean if mean.is_contiguous() else mean.contiguous()
-        ls = log_std if log_std.is_contiguous() else log_std.contiguous()
-        if ls.dim() > 1 and ls.shape != mean.shape:
-            ls = ls.expand_as(mean).contiguous()
-        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, ls, acts, None, advs.reshape(-1), adv_stats, 0.0, self.entropy_coeff,
-                                             self.tanh_action, scratch, info=info32[0:16])
-        torch.autograd.backward([mean, ls], [g_mean, g_ls])
+        std = self._head.eager_actor(self.pf, obs, acts, None, advs.reshape(-1), adv_stats, 0.0, self.entropy_coeff,
+                                     scratch, info32[0:16])
         scale, fused_norm = 1.0, False
         if self.dist is not None:
             scale, fused_norm = self.dist.reduce_grads(self.opt)
@@ -312,7 +282,8 @@ class A2C(OnRLAlgo):
         row = info32.cpu().numpy()
         info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16])}
         info.update(self._four_stats('v_pred', values.detach()))
-        info.update(self._four_stats('std', std.detach().expand_as(mean)))
+        if std is not None:
+            info.update(self._four_stats('std', std))
         info['ent'] = float(row[11])
         info['log_prob'] = float(row[1])
         return info

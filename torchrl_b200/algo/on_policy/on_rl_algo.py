@@ -14,13 +14,20 @@ class OnRLAlgo(RLAlgo):
         self.shuffle, self.tau, self.gae = shuffle, tau, gae
         self.sample_key = list(_KEYS)
 
+    def _prep_obs(self, x):
+        """uint8 frames of the pixel env -> float32 * obs_scale in one launch (ScaledFloatFrame,
+        /root/reference/torchrl/env/atari_wrapper.py:171-180); float observations pass through."""
+        if x.dtype != torch.uint8:
+            return x
+        return self.env.to_float(x.contiguous())
+
     def _bootstrap_value(self):
         """V(next_obs[T-1]) * (1 - terminals[T-1]) as a contiguous (N,) device vector (on_rl_algo.py:23-27); no
         host copy."""
         tail = self.replay_buffer.last_sample(['next_obs', 'terminals', 'time_limits'])
         alive = 1.0 - tail['terminals'].reshape(-1).float()
         with torch.no_grad():
-            return (self.vf(tail['next_obs']).reshape(-1) * alive).contiguous()
+            return (self.vf(self._prep_obs(tail['next_obs'])).reshape(-1) * alive).contiguous()
 
     def process_epoch_samples(self):
         """Fill `_advs` / `_estimate_returns` of the buffer: GAE(lambda = tau) or plain discounted returns

@@ -1,0 +1,133 @@
+"""What the on-policy algorithms (A2C, PPO) need to know about the policy's action distribution, in one place: how the
+fused minibatch loop and the eager `update` compute the actor loss and its gradient, the old log-probs and which
+distribution-specific scalars are logged.  `policy_head(pf)` picks the helper once, at construction.
+
+  GaussianHead     -- the (tanh-)Gaussian policies of policies/continuous_policy.py (csrc/ppo_loss.cu);
+  CategoricalHead  -- CategoricalDisPolicy over logits (csrc/categorical.cu).
+"""
+import numpy as np
+import torch
+
+from ... import ops
+from ...networks import fused
+
+
+def gaussian_outputs(pf, obs):
+    """(mean, std, log_std) of a Gaussian policy, mean and log_std made contiguous for the kernels."""
+    mean, std, log_std = pf(obs)
+    mean = mean if mean.is_contiguous() else mean.contiguous()
+    log_std = log_std if log_std.is_contiguous() else log_std.contiguous()
+    return mean, std, log_std
+
+
+class GaussianHead:
+    # keys the reference's PPO.update_actor logs besides the clipped-surrogate statistics (ppo.py:81-84)
+    ppo_extra_keys = ['log_std/mean', 'log_std/std', 'log_std/max', 'log_std/min']
+
+    def __init__(self, pf):
+        self.tanh_action = bool(getattr(pf, "tanh_action", False))
+
+    def fused_ok(self, pf):
+        """The fused minibatch loop needs a shared log-std PARAMETER (GuassianContPolicyBasicBias)."""
+        return hasattr(pf, "logstd")
+
+    def loss_scratch(self, B, acts, device):
+        return ops.LossScratch(B, acts.shape[-1], device)
+
+    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info):
+        """Device minibatch path: the mean, the raw log-std parameter with the policy's clamp applied inside the loss
+        kernel, which writes the parameter's gradient straight into its slice of the flat gradient buffer (this removes
+        the clamp / exp / clamp-backward / accumulate launches on six-element tensors from every minibatch)."""
+        from ...policies.continuous_policy import LOG_SIG_MIN, LOG_SIG_MAX
+        mean = pf.mean_net(obs)
+        if not mean.is_contiguous():
+            mean = mean.contiguous()
+        g_mean, _, _ = ops.ppo_actor_loss(mean, pf.logstd.detach(), acts.reshape(mean.shape[0], -1), old_logp, advs,
+                                          adv_table, clip, ent_coef, self.tanh_action, scratch, g_log_std=pf.logstd.grad,
+                                          info=info[0:16], stats_pos=stats_pos, ls_clamp=(LOG_SIG_MIN, LOG_SIG_MAX))
+        with fused.backward_fork():
+            torch.autograd.backward([mean], [g_mean])
+
+    def log_std_row(self, pf, info):
+        """A2C's std/* (a2c.py:90-94) are derived at flush from the clamped log-std written here."""
+        from ...policies.continuous_policy import LOG_SIG_MIN, LOG_SIG_MAX
+        n = pf.logstd.numel()
+        torch.clamp(pf.logstd.detach(), LOG_SIG_MIN, LOG_SIG_MAX, out=info[28:28 + n])
+
+    def a2c_std_info(self, row, B, a):
+        ls = row[28:28 + a].astype(np.float64)
+        sd = np.exp(ls)
+        m = sd.mean()
+        var = B * ((sd - m) ** 2).sum() / (B * a - 1.0)              # torch.std() of the (B, a) expanded tensor
+        return {'std/mean': float(m), 'std/std': float(np.sqrt(var)), 'std/max': float(sd.max()),
+                'std/min': float(sd.min())}
+
+    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False):
+        """One eager actor step (loss kernel + autograd); returns the extra scalars A2C logs (std/*)."""
+        mean, std, ls = gaussian_outputs(pf, obs)
+        if ls.dim() > 1 and ls.shape != mean.shape:
+            ls = ls.expand_as(mean).contiguous()
+        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, ls, acts.reshape(mean.shape[0], -1), old_logp, advs, adv_stats,
+                                             clip, ent_coef, self.tanh_action, scratch, info=info)
+        if fork:
+            with fused.backward_fork():
+                torch.autograd.backward([mean, ls], [g_mean, g_ls])
+        else:
+            torch.autograd.backward([mean, ls], [g_mean, g_ls])
+        return std.detach().expand_as(mean)
+
+    def old_log_prob(self, pf, obs, acts, out):
+        mean, _, ls = gaussian_outputs(pf, obs)
+        return ops.gaussian_log_prob(mean, ls, acts.reshape(mean.shape[0], -1), self.tanh_action, out=out)
+
+
+class CategoricalHead:
+    # the reference's PPO.update_actor reads out['log_std'] (ppo.py:52), which CategoricalDisPolicy.update does not
+    # return: its discrete PPO raises KeyError.  Here PPO runs and the four log_std/* keys are simply not logged.
+    ppo_extra_keys = []
+
+    def __init__(self, pf):
+        pass
+
+    def fused_ok(self, pf):
+        return True
+
+    def loss_scratch(self, B, acts, device):
+        return ops.LossScratch(B, 1, device, categorical=True)
+
+    @staticmethod
+    def _logits(pf, obs):
+        z = pf.logits(obs)
+        return z if z.is_contiguous() else z.contiguous()
+
+    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info):
+        logits = self._logits(pf, obs)
+        g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1), old_logp, advs, adv_table, clip, ent_coef,
+                                              scratch, info=info[0:16], stats_pos=stats_pos)
+        with fused.backward_fork():
+            torch.autograd.backward([logits], [g])
+
+    def log_std_row(self, pf, info):
+        pass
+
+    def a2c_std_info(self, row, B, a):
+        return {}                                           # a2c.py:90-94 logs std/* only `if 'std' in out`
+
+    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False):
+        logits = self._logits(pf, obs)
+        g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1).contiguous(), old_logp, advs, adv_stats, clip,
+                                              ent_coef, scratch, info=info)
+        if fork:
+            with fused.backward_fork():
+                torch.autograd.backward([logits], [g])
+        else:
+            torch.autograd.backward([logits], [g])
+        return None
+
+    def old_log_prob(self, pf, obs, acts, out):
+        return ops.categorical_log_prob(self._logits(pf, obs), acts.reshape(-1).contiguous(), out=out)
+
+
+def policy_head(pf):
+    from ...policies.discrete_policies import CategoricalDisPolicy
+    return CategoricalHead(pf) if isinstance(pf, CategoricalDisPolicy) else GaussianHead(pf)

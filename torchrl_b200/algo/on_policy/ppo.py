@@ -24,8 +24,9 @@ from ...networks import fused
 from .. import utils as atu
 from .a2c import A2C, _ADV_KEYS
 
+# info slots 0-6 of the actor loss kernels; slots 7-10 hold the head's extra keys (log_std/* of a Gaussian policy)
 _INFO_KEYS_ACTOR = ['Training/policy_loss', 'logprob/mean', 'logprob/std', 'logprob/max', 'logprob/min',
-                    'ratio/max', 'ratio/min', 'log_std/mean', 'log_std/std', 'log_std/max', 'log_std/min']
+                    'ratio/max', 'ratio/min']
 
 
 class PPO(A2C):
@@ -58,29 +59,27 @@ class PPO(A2C):
 
     def _actor_step(self, batch, info):
         st = self._mb_state
-        mean, raw_ls, clamp, g_ls = self._raw_policy_outputs(self.pf, batch["obs"])
-        g_mean, _, _ = ops.ppo_actor_loss(mean, raw_ls.detach(), batch["acts"].reshape(mean.shape[0], -1),
-                                          batch["old_logp"].reshape(-1), batch["advs"].reshape(-1), st["adv_table"],
-                                          self.clip_para, self.entropy_coeff, self.tanh_action, st["scratch"],
-                                          g_log_std=g_ls, info=info[0:16], stats_pos=st["upd"], ls_clamp=clamp)
-        with fused.backward_fork():
-            torch.autograd.backward([mean], [g_mean])
+        self._head.minibatch_actor(self.pf, batch["obs"], batch["acts"], batch["old_logp"].reshape(-1),
+                                   batch["advs"].reshape(-1), st["adv_table"], st["upd"], self.clip_para,
+                                   self.entropy_coeff, st["scratch"], info)
 
     def _cache_old_logp(self):
-        """log pi_old(a|s) for every stored transition, once per epoch (see module docstring)."""
+        """log pi_old(a|s) for every stored transition, once per epoch (see module docstring).  Chunks of whole time
+        rows, sized by the observation so that the chunk's network activations stay small: a 4x84x84 frame stack is
+        113 KB per sample in float32."""
         rb = self.replay_buffer
         if not hasattr(rb, "_old_logp"):
             rb.allocate("old_logp", tuple(rb._rewards.shape[1:]))
         T, N = rb._obs.shape[0], rb._obs.shape[1]
-        rows = max(1, (1 << 16) // N)
+        per_sample = int(np.prod(rb._obs.shape[2:])) * 4
+        samples = max(1, min(1 << 16, (256 << 20) // (16 * per_sample)))
+        rows = max(1, samples // N)
         with torch.no_grad():
             for r0 in range(0, T, rows):
                 r1 = min(T, r0 + rows)
-                obs = rb._obs[r0:r1].reshape(-1, rb._obs.shape[-1])
+                obs = self._prep_obs(rb._obs[r0:r1].reshape((-1,) + tuple(rb._obs.shape[2:])))
                 acts = rb._acts[r0:r1].reshape(obs.shape[0], -1)
-                mean, log_std = self._policy_outputs(self.pf, obs)
-                ops.gaussian_log_prob(mean, log_std, acts, self.tanh_action,
-                                      out=rb._old_logp[r0:r1].reshape(-1))
+                self._head.old_log_prob(self.pf, obs, acts, rb._old_logp[r0:r1].reshape(-1))
 
     def _pre_update(self):
         """ppo.py:29-34: linear LR decay, target <- pf; then the epoch's old log-probs."""
@@ -97,6 +96,8 @@ class PPO(A2C):
         info['grad_norm/vf'] = float(norms[1])
         for i, k in enumerate(_INFO_KEYS_ACTOR):
             info[k] = float(row[i])
+        for i, k in enumerate(self._head.ppo_extra_keys):
+            info[k] = float(row[7 + i])
         info['grad_norm/pf'] = float(norms[0])
         return info
 
@@ -112,27 +113,21 @@ class PPO(A2C):
                                       dtype=torch.float32, device=dev).contiguous()
         obs, acts, advs, rets, old_v = f('obs'), f('acts'), f('advs'), f('estimate_returns'), f('values')
         B = obs.shape[0]
-        acts = acts.reshape(B, -1)
-        scratch = ops.LossScratch(B, acts.shape[1], dev)
+        scratch = self._head.loss_scratch(B, acts.reshape(B, -1), dev)
         info32 = torch.zeros(32, dtype=torch.float32, device=dev)
         adv_stats = ops.vec_stats(advs.reshape(-1), out=info32[20:24])
         if 'old_logp' in batch:
             old_logp = f('old_logp').reshape(-1)
         else:
             with torch.no_grad():
-                tmean, tls = self._policy_outputs(self.target_pf, obs)
-                old_logp = ops.gaussian_log_prob(tmean, tls, acts, self.tanh_action)
+                old_logp = self._head.old_log_prob(self.target_pf, obs, acts, None)
         v = self.vf(obs)
         g_v, _ = ops.ppo_critic_loss(v.reshape(-1), rets.reshape(-1), old_v.reshape(-1), self.clipped_value_loss,
                                      self.clip_para, scratch, info=info32[16:17])
         with fused.backward_fork():
             torch.autograd.backward([v], [g_v.reshape(v.shape)])
-        mean, log_std = self._policy_outputs(self.pf, obs)
-        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, log_std, acts, old_logp, advs.reshape(-1), adv_stats,
-                                             self.clip_para, self.entropy_coeff, self.tanh_action, scratch,
-                                             info=info32[0:16])
-        with fused.backward_fork():
-            torch.autograd.backward([mean, log_std], [g_mean, g_ls])
+        self._head.eager_actor(self.pf, obs, acts, old_logp, advs.reshape(-1), adv_stats, self.clip_para,
+                               self.entropy_coeff, scratch, info32[0:16], fork=True)
         scale, fused_norm = 1.0, False
         if self.dist is not None:
             scale, fused_norm = self.dist.reduce_grads(self.opt)

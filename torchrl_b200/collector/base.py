@@ -300,8 +300,10 @@ class VecCollector:
                 traj_len = torch.zeros(N, 1, dtype=F64, device=self.device)
                 eval_obs = eval_env.reset()
                 steps = 0
+                pixel = getattr(eval_env, "pixel", False)
                 while True:
-                    act = self.pf.eval_act(eval_obs)
+                    # pixel envs hand out uint8 frame stacks: scale them like the training path does
+                    act = self.pf.eval_act(eval_env.to_float(eval_obs) if pixel else eval_obs)
                     if not torch.is_tensor(act):
                         act = torch.as_tensor(act, device=self.device)
                     eval_obs, r, done, _ = eval_env.step(act)

@@ -1,15 +1,22 @@
-"""Off-policy collector for the uint8 pixel env (BASELINE.json config 4): the VecCollector step
+"""Collectors for the uint8 pixel env (BASELINE.json config 4): the VecCollector step
 (/root/reference/torchrl/collector/base.py:184-230) with frames kept uint8 from the env to the replay ring.
 
-Per step (one captured CUDA graph): ring write obs[t] <- frames | u8->f32 scale | epsilon-greedy Q policy |
+Off-policy step (one captured CUDA graph): ring write obs[t] <- frames | u8->f32 scale | epsilon-greedy Q policy |
 env step (frame-stack shift + render, in place) | ring write next_obs[t] <- frames | scalar finalize
 (acts / rewards / terminals / time_limits rows, episode returns, timeout + done -> reset mask) | re-render
 the reset envs | ring advance.  `epsilon` lives in a device scalar refreshed from the host schedule.
+
+On-policy step (PixelVecOnPolicyCollector, the VecOnPolicyCollector of a pixel env,
+/root/reference/torchrl/collector/on_policy.py:94-153): the same graph with V(obs) on a side stream, the policy's
+`act_only` sampler (categorical kernel) in place of epsilon-greedy, V(next frames) for the timeout bootstrap (the env
+is not lock-step, so every step) and the finalize kernel in on-policy mode (values row, r + discount * V(next_obs) on
+rows cut by max_episode_frames, terminals include the cut).
 """
 import numpy as np
 import torch
 
 from .. import _lib, ops
+from ..policies import distribution as D
 from .base import VecCollector
 
 F32, F64, U8, I32 = torch.float32, torch.float64, torch.uint8, torch.int32
@@ -28,6 +35,9 @@ class PixelVecCollector(VecCollector):
         frame = tuple(self.env.observation_space.shape)
         self._dedup = bool(getattr(rb, "frame_dedup", False))
         keys = [("acts", (N,), F32), ("rewards", (N, 1), F32), ("terminals", (N, 1), U8), ("time_limits", (N, 1), U8)]
+        if self.on_policy:
+            keys.append(("values", (N, 1), F32))
+        assert not (self.on_policy and self._dedup), "the on-policy pixel collector stores full frame stacks"
         if self._dedup:
             # frame-de-duplicated ring (replay_buffers/memory_efficient.py): one frame of obs and one of next_obs per
             # row instead of two C-frame stacks
@@ -46,6 +56,7 @@ class PixelVecCollector(VecCollector):
         self._d_state = torch.zeros(N, 1, dtype=F32, device=dev)
         self._d_rows = torch.zeros(self._T, N, 1, dtype=F32, device=dev)
         self._obs_f = torch.empty((N,) + frame, dtype=F32, device=dev)
+        self._next_f = torch.empty((N,) + frame, dtype=F32, device=dev) if self.on_policy else None
         self._any_reset = torch.zeros(2, dtype=I32, device=dev)
         if not self._dedup:
             self._plan_obs = ops.RowCopyPlan([self.env.obs.view(1, -1)], [rb._obs], [ops.row_bytes_of(rb._obs)])
@@ -64,21 +75,39 @@ class PixelVecCollector(VecCollector):
             else:
                 ops.ring_write(self._plan_obs, rb._top_dev)
             env.to_float(env.obs, self._obs_f)
-            out = self.pf.explore(self._obs_f.unsqueeze(0), epsilon=self._eps_dev)
-            self._act.copy_(out["action"].reshape(self._act.shape).to(F32))
+            side = None
+            if self.on_policy:
+                # V(obs) is only needed by the finalize kernel: a parallel branch of the captured step graph
+                main = torch.cuda.current_stream(self.device)
+                side = self._side_stream
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    self._value.copy_(self.vf(self._obs_f).reshape(-1))
+                self.pf.act_only(self._obs_f, action_out=self._act, nan_flag=self._nan_flag)
+            else:
+                out = self.pf.explore(self._obs_f.unsqueeze(0), epsilon=self._eps_dev)
+                self._act.copy_(out["action"].reshape(self._act.shape).to(F32))
             env.launch_step(self._act.reshape(-1))
             if self._dedup:
                 rb.write_next_obs(env.obs)
             else:
                 ops.ring_write(self._plan_next, rb._top_dev)
+            v_next = None
+            if side is not None:
+                main.wait_stream(side)              # one value net, one set of per-stream scratch: V(obs) first
+                self._v_next.copy_(self.vf(env.to_float(env.obs, self._next_f)).reshape(-1))
+                v_next = self._v_next
             _lib.call("trl_collect_finalize", self._d_ob.data_ptr(), self._d_ob.data_ptr(), self._d_state.data_ptr(),
-                      self._act.data_ptr(), None, None, env.reward.data_ptr(), env.done.data_ptr(),
+                      self._act.data_ptr(), None if self._value is None else self._value.data_ptr(),
+                      None if v_next is None else v_next.data_ptr(), env.reward.data_ptr(), env.done.data_ptr(),
                       env.time_limit.data_ptr(), env.elapsed.data_ptr(), env.episode.data_ptr(), env.seeds.data_ptr(),
                       self.current_step.data_ptr(), self.train_rew.data_ptr(), self._epoch_reward.data_ptr(),
                       self._ret_log.data_ptr(), self._n_done.data_ptr(), None, None, None, self._d_ob.data_ptr(),
-                      self._d_rows.data_ptr(), self._d_rows.data_ptr(), rb._acts.data_ptr(), None,
+                      self._d_rows.data_ptr(), self._d_rows.data_ptr(), rb._acts.data_ptr(),
+                      rb._values.data_ptr() if self.on_policy else None,
                       rb._rewards.data_ptr(), rb._terminals.data_ptr(), rb._time_limits.data_ptr(),
-                      rb._top_dev.data_ptr(), self._N, 1, 1, int(self.max_episode_frames), 0.0, 0.0, 10.0, 0, 1,
+                      rb._top_dev.data_ptr(), self._N, 1, 1, int(self.max_episode_frames),
+                      float(getattr(self, "discount", 0.0)), 0.0, 10.0, 1 if self.on_policy else 0, 1,
                       ops._stream())
             # envs whose collector step counter was just zeroed need a fresh episode (done or timeout); the
             # finalize kernel already advanced their episode counter
@@ -91,18 +120,22 @@ class PixelVecCollector(VecCollector):
         return False
 
     def _step(self):
-        self.pf.tick()                                   # host-side epsilon schedule -> device scalar
-        self._eps_host[0] = float(self.pf.epsilon)
-        self._eps_dev.copy_(self._eps_host, non_blocking=True)
-        if not self.use_cuda_graph:
-            self._step_body(False)
-        elif False in self._graphs:
-            self._graphs[False].replay()
+        boot = self.on_policy
+        if not self.on_policy:
+            self.pf.tick()                               # host-side epsilon schedule -> device scalar
+            self._eps_host[0] = float(self.pf.epsilon)
+            self._eps_dev.copy_(self._eps_host, non_blocking=True)
+        # "reference_cpu" sampling draws on the host (torch.multinomial): not capturable
+        eager = not self.use_cuda_graph or (self.on_policy and D.get_noise_mode() == "reference_cpu")
+        if eager:
+            self._step_body(boot)
+        elif boot in self._graphs:
+            self._graphs[boot].replay()
         elif self._eager_steps < 3:
             self._eager_steps += 1
-            self._step_body(False)
+            self._step_body(boot)
         else:
-            g = ops.CapturedGraph(lambda: self._step_body(False))
-            self._graphs[False] = g
+            g = ops.CapturedGraph(lambda: self._step_body(boot))
+            self._graphs[boot] = g
             g.replay()
         self.replay_buffer.advance_host(1)

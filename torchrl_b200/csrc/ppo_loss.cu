@@ -10,7 +10,7 @@
 // the caller seeds torch.autograd.backward at the MLP outputs with these gradients, so no
 // intermediate (B,a) tensors ever round-trip through HBM and nothing syncs with the host.
 // Reductions are two-level (per-CTA partials, last CTA reduces in fixed order): deterministic.
-#include "common.cuh"
+#include "loss_reduce.cuh"
 
 namespace trl {
 
@@ -51,33 +51,6 @@ __device__ __forceinline__ float clamped_ls(const ActorParams& p, float raw, boo
   if (p.ls_min > p.ls_max) { *pass = true; return raw; }
   *pass = (raw >= p.ls_min) && (raw <= p.ls_max);
   return fminf(fmaxf(raw, p.ls_min), p.ls_max);
-}
-
-__device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
-  v = warp_sum(v);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[wid] = v;
-  __syncthreads();
-  double r = 0.0;
-  if (wid == 0) {
-    r = lane < nw ? sh[lane] : 0.0;
-    r = warp_sum(r);
-  }
-  return r;  // valid in warp 0
-}
-__device__ __forceinline__ float block_reduce_max(float v, float* sh) {
-  v = warp_max(v);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[wid] = v;
-  __syncthreads();
-  float r = -INFINITY;
-  if (wid == 0) {
-    r = lane < nw ? sh[lane] : -INFINITY;
-    r = warp_max(r);
-  }
-  return r;
 }
 
 __global__ void __launch_bounds__(kLossThreads) ppo_actor_loss_kernel(const ActorParams p) {

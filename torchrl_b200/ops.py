@@ -223,8 +223,10 @@ def vec_stats(x, out=None):
 class LossScratch:
     """Scratch + ticket for the two-level reductions of the loss kernels (allocated once)."""
 
-    def __init__(self, B, act_dim, device):
-        n = int(_lib.load().trl_ppo_actor_scratch_doubles(int(B), int(act_dim)))
+    def __init__(self, B, act_dim, device, categorical=False):
+        lib = _lib.load()
+        n = int(lib.trl_ppo_categorical_actor_scratch_doubles(int(B)) if categorical
+                else lib.trl_ppo_actor_scratch_doubles(int(B), int(act_dim)))
         self.actor = torch.zeros(max(n, 1), dtype=F64, device=device)
         self.critic = torch.zeros(max((int(B) + 255) // 256, 1), dtype=F64, device=device)
         self.tickets = torch.zeros(4, dtype=I32, device=device)
@@ -278,6 +280,58 @@ def gaussian_log_prob(mean, log_std, actions, tanh_action, out=None):
     _lib.call("trl_gaussian_log_prob", _chk(mean, F32, "mean"), _chk(log_std, F32, "log_std"), ls_stride,
               _chk(actions, F32, "actions"), B, a, int(bool(tanh_action)), _chk(out, F32, "logp"), _stream())
     return out
+
+
+# ------------------------------------------------------------------------------------------ K13 categorical
+def categorical_sample(logits, u=None, rng=None, action_out=None, want_log_prob=False, nan_flag=None):
+    """Action index (as float) ~ Categorical(softmax(logits)) by inverse CDF: u (M,) supplied uniforms in [0,1), or
+    Philox keyed by (rng.seed, rng.counter, row).  Mirrors CategoricalDisPolicy.explore
+    (/root/reference/torchrl/policies/discrete_policies.py:131-144)."""
+    A = logits.shape[-1]
+    M = logits.numel() // A
+    action = action_out if action_out is not None else torch.empty(M, dtype=F32, device=logits.device)
+    assert action.numel() == M
+    logp = torch.empty(M, dtype=F32, device=logits.device) if want_log_prob else None
+    seed, ctr = (0, None)
+    if u is None:
+        if rng is None or rng.counter is None:
+            raise ValueError("categorical_sample needs either u or an rng state")
+        seed, ctr = rng.seed, rng.counter
+    _lib.call("trl_categorical_sample", _chk(logits, F32, "logits"), _opt(u, F32, "u"), ctypes.c_uint64(seed),
+              _opt(ctr, I64, "rng_counter"), M, A, _chk(action, F32, "action"), _opt(logp, F32, "log_prob"),
+              _opt(nan_flag, I32, "nan_flag"), _stream())
+    return (action, logp) if want_log_prob else action
+
+
+def categorical_log_prob(logits, actions, out=None):
+    """log(clamp(softmax(logits)[a], eps, 1-eps)) per row: Categorical.log_prob of stored actions."""
+    A = logits.shape[-1]
+    M = logits.numel() // A
+    if out is None:
+        out = torch.empty(M, dtype=F32, device=logits.device)
+    assert actions.numel() == M and out.numel() == M
+    _lib.call("trl_categorical_log_prob", _chk(logits, F32, "logits"), _chk(actions, F32, "actions"), M, A,
+              _chk(out, F32, "logp"), _stream())
+    return out
+
+
+def ppo_categorical_actor_loss(logits, actions, old_logp, advs, adv_stats, clip_para, entropy_coeff, scratch,
+                               g_logits=None, info=None, logp_out=None, stats_pos=None):
+    """The actor loss of PPO (old_logp given, clipped surrogate) or A2C (old_logp None) for a categorical policy:
+    value, dL/dlogits and the logged statistics in one launch (ppo.py:41-91, a2c.py:66-70).  `scratch` is a
+    LossScratch(..., categorical=True)."""
+    B, A = logits.shape
+    assert scratch.B >= B
+    if g_logits is None:
+        g_logits = torch.empty_like(logits)
+    if info is None:
+        info = torch.zeros(16, dtype=F32, device=logits.device)
+    _lib.call("trl_ppo_categorical_actor_loss", _chk(logits, F32, "logits"), _chk(actions, F32, "actions"),
+              _opt(old_logp, F32, "old_logp"), _chk(advs, F32, "advs"), _opt(adv_stats, F32, "adv_stats"),
+              _opt(stats_pos, I32, "stats_pos"), B, A, float(clip_para), float(entropy_coeff),
+              _chk(g_logits, F32, "g_logits"), _opt(logp_out, F32, "logp_out"), _chk(info, F32, "info"),
+              _chk(scratch.actor, F64, "scratch"), scratch.tickets[0:1].data_ptr(), _stream())
+    return g_logits, info
 
 
 def row_group_moments(x, idx, groups, b, out=None):

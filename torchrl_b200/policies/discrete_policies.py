@@ -11,7 +11,9 @@ import torch.nn as nn
 from torch.distributions import Categorical
 
 from .. import networks
+from .. import ops
 from . import distribution as D
+from .continuous_policy import _DeviceRng
 
 
 class UniformPolicyDiscrete(nn.Module):
@@ -102,12 +104,41 @@ class EpsilonGreedyQRDQNDiscretePolicy(EpsilonGreedyDQNDiscretePolicy):
 
 
 class CategoricalDisPolicy(networks.Net):
+    """softmax over the net's outputs (discrete_policies.py:123-160).  `forward` / `explore` / `update` / `eval_act`
+    keep the reference's torch semantics; the collector's `act_only` and the on-policy algorithms' fused minibatch
+    loop work on the logits with the categorical kernels (csrc/categorical.cu)."""
+
     def __init__(self, **kwargs):
         super().__init__(**kwargs)
         self.continuous = False
+        self._rng = _DeviceRng()
+
+    def logits(self, x):
+        return networks.Net.forward(self, x)
 
     def forward(self, x):
-        return torch.softmax(super().forward(x), dim=-1)
+        return torch.softmax(self.logits(x), dim=-1)
+
+    def act_only(self, x, action_out=None, nan_flag=None, u=None, eps=None):
+        """Collector fast path: one sampled action index per row (as float) into `action_out`, one launch after the
+        net (no softmax launch).  u: optional (M,) uniforms in [0,1) replacing the Philox stream.  In the
+        "reference_cpu" noise mode the action is drawn with torch.multinomial on the CPU generator from the device
+        probabilities, as the reference's Categorical.sample does on a CPU policy (this syncs; not capturable)."""
+        logits = self.logits(x)
+        logits = logits if logits.is_contiguous() else logits.contiguous()
+        if u is None and D.get_noise_mode() == "reference_cpu":
+            probs = torch.softmax(logits.detach(), dim=-1).cpu()
+            act = torch.multinomial(probs.reshape(-1, probs.shape[-1]), 1, True).reshape(-1)
+            if action_out is None:
+                return act.to(logits.device, torch.float32)
+            action_out.reshape(-1).copy_(act.to(torch.float32))
+            return action_out
+        rng = None if u is not None else self._rng.ensure(logits.device)
+        out = ops.categorical_sample(logits.detach(), u=u, rng=rng, nan_flag=nan_flag,
+                                     action_out=None if action_out is None else action_out.reshape(-1))
+        if u is None:
+            ops.counter_advance(rng.counter)
+        return out
 
     def explore(self, x, return_log_probs=False):
         output = self.forward(x)
