@@ -11,8 +11,9 @@
 // entropy = -sum_j p_j l_j.  Gradients wrt x, with m_j = 1 where the clamp passes (eps <= p_j <= 1-eps):
 //   d l_a / d x_k = m_a (delta_ak - p_k)
 //   d ent / d x_k = -p_k (l_k + m_k) + p_k sum_j p_j (l_j + m_j)
-// One thread per row; a row's (<= 32) logits live in registers.
-#include "loss_reduce.cuh"
+// One thread per row; a row's (<= 32) logits live in registers.  The actor loss's reductions are two-level and
+// deterministic (reduce.cuh: block_partials per CTA, then last_cta; the last CTA folds in a fixed order).
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -156,7 +157,6 @@ struct CatLossParams {
 __global__ void __launch_bounds__(kCatThreads) ppo_categorical_actor_loss_kernel(const CatLossParams p) {
   __shared__ double sh_d[kCatThreads / 32][5];
   __shared__ float sh_f[kCatThreads / 32][4];
-  __shared__ unsigned s_last;
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const bool ok = b < p.B;
   const int A = p.A;
@@ -222,12 +222,7 @@ __global__ void __launch_bounds__(kCatThreads) ppo_categorical_actor_loss_kernel
   const float maxs[4] = {ok ? logp : -INFINITY, ok ? -logp : -INFINITY, ok ? ratio : -INFINITY,
                          ok ? -ratio : -INFINITY};
   block_partials<kCatThreads / 32>(sums, maxs, sh_d, sh_f, p.partial + static_cast<long long>(blockIdx.x) * kCatPartials);
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_cta(p.ticket, gridDim.x)) return;
   // last CTA: warp w folds quantities w and w + 8; lane l takes partials l, l+32, ... then a fixed shuffle tree
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   __shared__ double tot[kCatPartials];
@@ -261,7 +256,6 @@ __global__ void __launch_bounds__(kCatThreads) ppo_categorical_actor_loss_kernel
     for (int k = 7; k < 11; ++k) p.info[k] = 0.f;  // the log-std slots of the Gaussian kernel
     p.info[11] = static_cast<float>(ent_mean);
     p.info[12] = static_cast<float>(tot[4] / Bn);
-    *p.ticket = 0u;
   }
 }
 

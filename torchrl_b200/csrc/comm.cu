@@ -13,7 +13,7 @@
 //   * each thread sums its float4 / double slice over the W peer buffers IN RANK ORDER (so every rank computes the
 //     bit-identical result -- parameters never drift apart, no broadcast needed), writes the sum to a local output
 //     buffer and, for the gradient, accumulates the per-segment sum of squares in fp64 (two-level, fixed order: the
-//     role of csrc/optim.cu's grad_sumsq_kernel, incl. Adam step counts and bias corrections in the last block);
+//     role of csrc/optim.cu's grad_sumsq_kernel, with the same last-block tail: reduce.cuh's sumsq_segment_tail);
 //   * block b raises flag[done][b][rank] everywhere and waits: "everybody has finished reading my operand", then
 //     zeroes its slice of the local operand (the gradient buffer is accumulated into by the next backward).
 // Flags carry a sequence number that only grows (kept in device memory, bumped by the last block), so nothing is
@@ -24,7 +24,7 @@
 // in two PUSH rounds of flag-carrying 16-byte packets (22 us at W = 2: NVLink sees 70 k small volatile stores per round),
 // and a deferred second phase on a side stream beside the Adam launch (no measurable gain).  The flag-in-payload push IS
 // the better scheme for the few-hundred-byte fp64 vectors (allreduce_f64_ll_kernel below: 3.5 us against 5.7 us).
-#include "common.cuh"
+#include "reduce.cuh"
 
 namespace trl {
 namespace comm {
@@ -103,7 +103,6 @@ struct GradParams {
 
 __global__ void __launch_bounds__(kThreads) allreduce_grad_kernel(const GradParams p) {
   __shared__ double sh[kThreads / 32][kMaxSeg];
-  __shared__ unsigned s_last;
   const unsigned seq = *p.seq + 1u;
   cross_rank_barrier(p.pe, p.rank, p.world, 0, seq);
   // ---- reduce my slice over the ranks, in rank order -------------------------------------------------------------
@@ -148,36 +147,11 @@ __global__ void __launch_bounds__(kThreads) allreduce_grad_kernel(const GradPara
   }
   // ---- last block to get here: per-segment totals, Adam step counts, bias corrections, sequence number.  Done BEFORE
   // the second cross-rank phase so that this serial tail runs in the shadow of that phase's NVLink round trip.
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    if (threadIdx.x < p.seg.nseg) {
-      const int k = threadIdx.x;
-      if ((p.active_mask >> k) & 1u) {
-        double t = 0.0;
-        for (unsigned b0 = 0; b0 < gridDim.x; b0 += 16) {    // 16 partials in flight, added in block order
-          double v[16];
-#pragma unroll
-          for (int u = 0; u < 16; ++u) v[u] = (b0 + u < gridDim.x) ? __ldcg(p.partial + (b0 + u) * p.seg.nseg + k) : 0.0;
-#pragma unroll
-          for (int u = 0; u < 16; ++u) t += v[u];
-        }
-        p.sumsq3[k] = t;
-        if (p.step) {
-          const int st = p.step[k] + 1;
-          p.step[k] = st;
-          p.sumsq3[p.seg.nseg + 2 * k] = 1.0 - pow_int(p.beta1, st);
-          p.sumsq3[p.seg.nseg + 2 * k + 1] = sqrt(1.0 - pow_int(p.beta2, st));
-        }
-      }
-    }
-    if (threadIdx.x == 0) {
-      *p.ticket = 0u;
-      *p.seq = seq;          // every block read the old value at its start (they all passed the ticket above)
-    }
+  if (last_cta(p.ticket, gridDim.x)) {
+    const int k = threadIdx.x;
+    if (k < p.seg.nseg && ((p.active_mask >> k) & 1u))
+      sumsq_segment_tail(p.partial + k, gridDim.x, p.seg.nseg, k, p.seg.nseg, p.sumsq3, p.step, p.beta1, p.beta2);
+    if (threadIdx.x == 0) *p.seq = seq;  // every block read the old value at its start (they all passed the ticket above)
   }
   // ---- everybody has read my operand: it may be overwritten ------------------------------------------------------------
   cross_rank_barrier(p.pe, p.rank, p.world, 1, seq);

@@ -72,7 +72,7 @@ __device__ __forceinline__ double pow_int(double b, int n) {
   return r;
 }
 
-// ---- warp / block reductions -------------------------------------------------------
+// ---- warp reductions (block level and across CTAs: reduce.cuh) --------------------
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -92,23 +92,6 @@ __device__ __forceinline__ float warp_min(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
-}
-
-// Block-wide sum for blockDim.x a multiple of 32 (<=1024).  `scratch` >= 32 elements.
-template <typename T>
-__device__ __forceinline__ T block_sum(T v, T* scratch) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  v = warp_sum(v);
-  if (lane == 0) scratch[wid] = v;
-  __syncthreads();
-  const int nw = (blockDim.x + 31) >> 5;
-  T r = (threadIdx.x < nw) ? scratch[threadIdx.x] : T(0);
-  if (wid == 0) r = warp_sum(r);
-  if (threadIdx.x == 0) scratch[0] = r;
-  __syncthreads();
-  r = scratch[0];
-  __syncthreads();
-  return r;
 }
 
 // float atomic max/min via CAS-free integer trick (valid for non-NaN values)

@@ -16,7 +16,7 @@
 // are staged in shared memory with flat coalesced loads; A (o x o), B (a x o), c live in
 // shared memory too (49 KB for o=111).  Thread (e, j) produces s'[e][j].  HBM traffic per
 // env-step: read 4(o+a), write 4o + 6 bytes -> HBM/latency-bound, no tensor-core work.
-#include "common.cuh"
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -77,7 +77,6 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
   float* ss = sub + a;
   float* su = ss + E * o;
   float* s2 = su + E * a;
-  __shared__ unsigned s_last;
   const int tid = threadIdx.x, nthr = blockDim.x;
   const long long env_base = static_cast<long long>(blockIdx.x) * E;
   const int ne = static_cast<int>(min(static_cast<long long>(E), p.N - env_base));
@@ -149,12 +148,7 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
       pp[j] = s;
       pp[o + j] = q;
     }
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-    __syncthreads();
-    if (s_last) {
-      __threadfence();
+    if (last_cta(p.ticket, gridDim.x)) {
       // fold the per-CTA partials with all threads: thread (part, c) sums CTAs b = part, part+P, ... of
       // column c (c < 2*o), then `part` results are combined in fixed order (deterministic); the previous
       // version walked all CTAs serially in `o` threads and dominated the kernel's latency
@@ -181,25 +175,10 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
           }
         }
         if (p.batch_sums) { p.batch_sums[j] = s; p.batch_sums[o + j] = q; }
-        if (p.merge) {
-          // Chan et al. merge of (mean,var,count) with the batch (population variance)
-          const double bn = static_cast<double>(p.N);
-          const double bmean = s / bn;
-          double bvar = q / bn - bmean * bmean;
-          if (bvar < 0.0) bvar = 0.0;
-          const double cnt = *p.norm_count;
-          const double tot = cnt + bn;
-          const double delta = bmean - p.norm_mean[j];
-          const double m2 = p.norm_var[j] * cnt + bvar * bn + delta * delta * cnt * bn / tot;
-          p.norm_mean[j] = p.norm_mean[j] + delta * bn / tot;
-          p.norm_var[j] = m2 / tot;
-        }
+        if (p.merge) chan_merge(s, q, static_cast<double>(p.N), *p.norm_count, p.norm_mean[j], p.norm_var[j]);
       }
-      __syncthreads();
-      if (tid == 0) {
-        if (p.merge) *p.norm_count = *p.norm_count + static_cast<double>(p.N);
-        *p.ticket = 0u;
-      }
+      __syncthreads();   // every thread has read *norm_count
+      if (tid == 0 && p.merge) *p.norm_count = *p.norm_count + static_cast<double>(p.N);
     }
   }
 }

@@ -10,7 +10,7 @@
 // minibatch are moved by ONE launch (grid.y = key).  The row indices themselves are produced
 // by the host with the reference's own NumPy calls (bit-exact replay indexing) and uploaded.
 // HBM-bound: 2 x row_bytes per (row, key).
-#include "common.cuh"
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -70,90 +70,62 @@ __global__ void __launch_bounds__(256) row_copy_kernel(const RowCopyParams p) {
     __syncthreads();
     if (threadIdx.x == 0) {
       __threadfence();
-      const unsigned total = gridDim.x * gridDim.y * gridDim.z;
-      if (atomicAdd(p.ticket, 1u) == total - 1) {
+      if (draw_ticket(p.ticket, gridDim.x * gridDim.y * gridDim.z)) {
         *p.adv_ptr = (*p.adv_ptr + 1) % p.adv_T;
         if (p.adv_size && *p.adv_size < p.adv_T) *p.adv_size += 1;
-        *p.ticket = 0u;
       }
     }
   }
 }
 
-// stats[0..3] = mean, unbiased std, max, min of x[0..n)   (one CTA; fp64 accumulation)
-__global__ void __launch_bounds__(1024) vec_stats_kernel(const float* __restrict__ x, long long n,
-                                                        float* __restrict__ stats) {
-  __shared__ double sh_s[32], sh_q[32];
-  __shared__ float sh_mx[32], sh_mn[32];
-  double s = 0.0, q = 0.0;
-  float mx = -INFINITY, mn = INFINITY;
+// the raw moments (sum, sum of squares, max, min) of x[0..n) over the block (fp64 accumulation); true in thread 0,
+// which holds them
+__device__ __forceinline__ bool vec_block_moments(const float* __restrict__ x, long long n, double& s, double& q,
+                                                  float& mx, float& mn) {
+  s = 0.0; q = 0.0; mx = -INFINITY; mn = INFINITY;
   for (long long i = threadIdx.x; i < n; i += blockDim.x) {
     const float v = x[i];
     s += v; q += static_cast<double>(v) * v;
     mx = fmaxf(mx, v); mn = fminf(mn, v);
   }
-  s = warp_sum(s); q = warp_sum(q); mx = warp_max(mx); mn = warp_min(mn);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (lane == 0) { sh_s[wid] = s; sh_q[wid] = q; sh_mx[wid] = mx; sh_mn[wid] = mn; }
-  __syncthreads();
-  if (wid == 0) {
-    s = lane < nw ? sh_s[lane] : 0.0; q = lane < nw ? sh_q[lane] : 0.0;
-    mx = lane < nw ? sh_mx[lane] : -INFINITY; mn = lane < nw ? sh_mn[lane] : INFINITY;
-    s = warp_sum(s); q = warp_sum(q); mx = warp_max(mx); mn = warp_min(mn);
-    if (lane == 0) {
-      const double dn = static_cast<double>(n);
-      const double mean = s / dn;
-      double var = (q - s * mean) / (dn - 1.0);   // unbiased (torch.std default); n==1 -> nan like torch
-      if (var < 0.0) var = 0.0;
-      stats[0] = static_cast<float>(mean);
-      stats[1] = static_cast<float>(sqrt(var));
-      stats[2] = mx;
-      stats[3] = mn;
-    }
-  }
+  return block_moments(s, q, mx, mn);
+}
+
+// stats[0..3] = mean, unbiased std, max, min of x[0..n)   (one CTA; fp64 accumulation)
+__global__ void __launch_bounds__(1024) vec_stats_kernel(const float* __restrict__ x, long long n,
+                                                        float* __restrict__ stats) {
+  double s, q;
+  float mx, mn;
+  if (vec_block_moments(x, n, s, q, mx, mn)) stats_from_moments(s, q, mx, mn, static_cast<double>(n), stats);
 }
 
 // raw moments of x[0..n): m[0..3] = sum, sum of squares, max, -min (fp64) -- the local half of a
 // cross-rank statistic (K12: advantage normalisation over all ranks' envs, ppo.py:147)
 __global__ void __launch_bounds__(1024) vec_moments_kernel(const float* __restrict__ x, long long n,
                                                           double* __restrict__ m) {
-  __shared__ double sh_s[32], sh_q[32];
-  __shared__ float sh_mx[32], sh_mn[32];
-  double s = 0.0, q = 0.0;
-  float mx = -INFINITY, mn = INFINITY;
-  for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-    const float v = x[i];
-    s += v; q += static_cast<double>(v) * v;
-    mx = fmaxf(mx, v); mn = fminf(mn, v);
+  double s, q;
+  float mx, mn;
+  if (vec_block_moments(x, n, s, q, mx, mn)) { m[0] = s; m[1] = q; m[2] = mx; m[3] = -static_cast<double>(mn); }
+}
+
+// [mean, unbiased std, max, min] from W ranks' raw moments g[r * stride ..][0..3] (sum, sum of squares, max, -min),
+// combined in rank order
+__device__ __forceinline__ void stats_from_rank_moments(const double* __restrict__ g, int W, long long stride,
+                                                        double n_total, float* __restrict__ stats) {
+  double s = 0.0, q = 0.0, mx = -INFINITY, nmn = -INFINITY;
+  for (int r = 0; r < W; ++r) {
+    const double* m = g + r * stride;
+    s += m[0]; q += m[1];
+    mx = fmax(mx, m[2]); nmn = fmax(nmn, m[3]);
   }
-  s = warp_sum(s); q = warp_sum(q); mx = warp_max(mx); mn = warp_min(mn);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (lane == 0) { sh_s[wid] = s; sh_q[wid] = q; sh_mx[wid] = mx; sh_mn[wid] = mn; }
-  __syncthreads();
-  if (wid == 0) {
-    s = lane < nw ? sh_s[lane] : 0.0; q = lane < nw ? sh_q[lane] : 0.0;
-    mx = lane < nw ? sh_mx[lane] : -INFINITY; mn = lane < nw ? sh_mn[lane] : INFINITY;
-    s = warp_sum(s); q = warp_sum(q); mx = warp_max(mx); mn = warp_min(mn);
-    if (lane == 0) { m[0] = s; m[1] = q; m[2] = mx; m[3] = -static_cast<double>(mn); }
-  }
+  stats_from_moments(s, q, mx, -nmn, n_total, stats);
 }
 
 // combine W ranks' raw moments (W x 4 doubles, rank order) into [mean, unbiased std, max, min]
 __global__ void vec_stats_from_moments_kernel(const double* __restrict__ g, int W, double n_total,
                                               float* __restrict__ stats) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  double s = 0.0, q = 0.0, mx = -INFINITY, nmn = -INFINITY;
-  for (int r = 0; r < W; ++r) {
-    s += g[4 * r]; q += g[4 * r + 1];
-    mx = fmax(mx, g[4 * r + 2]); nmn = fmax(nmn, g[4 * r + 3]);
-  }
-  const double mean = s / n_total;
-  double var = (q - s * mean) / (n_total - 1.0);
-  if (var < 0.0) var = 0.0;
-  stats[0] = static_cast<float>(mean);
-  stats[1] = static_cast<float>(sqrt(var));
-  stats[2] = static_cast<float>(mx);
-  stats[3] = static_cast<float>(-nmn);
+  stats_from_rank_moments(g, W, 4, n_total, stats);
 }
 
 // raw moments of every minibatch of an epoch in ONE launch: CTA u reduces the b time rows idx[u*b .. (u+1)*b) of x
@@ -162,8 +134,6 @@ __global__ void vec_stats_from_moments_kernel(const double* __restrict__ g, int 
 // statistics of ppo.py:141-147 need not be recomputed (nor all-reduced) per minibatch
 __global__ void __launch_bounds__(1024) row_group_moments_kernel(const float* __restrict__ x, const long long* __restrict__ idx,
                                                                 int b, long long n, double* __restrict__ out) {
-  __shared__ double sh_s[32], sh_q[32];
-  __shared__ float sh_mx[32], sh_mn[32];
   double s = 0.0, q = 0.0;
   float mx = -INFINITY, mn = INFINITY;
   for (int k = 0; k < b; ++k) {
@@ -174,18 +144,9 @@ __global__ void __launch_bounds__(1024) row_group_moments_kernel(const float* __
       mx = fmaxf(mx, v); mn = fminf(mn, v);
     }
   }
-  s = warp_sum(s); q = warp_sum(q); mx = warp_max(mx); mn = warp_min(mn);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (lane == 0) { sh_s[wid] = s; sh_q[wid] = q; sh_mx[wid] = mx; sh_mn[wid] = mn; }
-  __syncthreads();
-  if (wid == 0) {
-    s = lane < nw ? sh_s[lane] : 0.0; q = lane < nw ? sh_q[lane] : 0.0;
-    mx = lane < nw ? sh_mx[lane] : -INFINITY; mn = lane < nw ? sh_mn[lane] : INFINITY;
-    s = warp_sum(s); q = warp_sum(q); mx = warp_max(mx); mn = warp_min(mn);
-    if (lane == 0) {
-      double* o = out + 4LL * blockIdx.x;
-      o[0] = s; o[1] = q; o[2] = mx; o[3] = -static_cast<double>(mn);
-    }
+  if (block_moments(s, q, mx, mn)) {
+    double* o = out + 4LL * blockIdx.x;
+    o[0] = s; o[1] = q; o[2] = mx; o[3] = -static_cast<double>(mn);
   }
 }
 
@@ -194,19 +155,7 @@ __global__ void group_stats_from_moments_kernel(const double* __restrict__ g, in
                                                 float* __restrict__ stats) {
   const int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= U) return;
-  double s = 0.0, q = 0.0, mx = -INFINITY, nmn = -INFINITY;
-  for (int r = 0; r < W; ++r) {
-    const double* m = g + (static_cast<long long>(r) * U + u) * 4;
-    s += m[0]; q += m[1];
-    mx = fmax(mx, m[2]); nmn = fmax(nmn, m[3]);
-  }
-  const double mean = s / n_total;
-  double var = (q - s * mean) / (n_total - 1.0);
-  if (var < 0.0) var = 0.0;
-  stats[4 * u] = static_cast<float>(mean);
-  stats[4 * u + 1] = static_cast<float>(sqrt(var));
-  stats[4 * u + 2] = static_cast<float>(mx);
-  stats[4 * u + 3] = static_cast<float>(-nmn);
+  stats_from_rank_moments(g + 4LL * u, W, 4LL * U, n_total, stats + 4 * u);
 }
 
 }  // namespace trl

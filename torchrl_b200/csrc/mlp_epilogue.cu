@@ -8,7 +8,7 @@
 // ncu (profiles/launches_ppo_step_r1.md) showed these PyTorch epilogue/elementwise/reduce launches at
 // ~30 % of a minibatch update; both kernels here are HBM-bound: 8 B/element forward, 12 B/element
 // backward (+ H floats of bias gradient).
-#include "common.cuh"
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -59,7 +59,6 @@ __global__ void __launch_bounds__(256) bias_act_bwd_kernel(const float* g, const
                                                           unsigned* __restrict__ tickets, long long M, int H,
                                                           int act) {
   __shared__ float4 sh[8][32];
-  __shared__ unsigned s_last;
   const int lane = threadIdx.x & 31, rg = threadIdx.x >> 5;
   const int col = (blockIdx.x * 32 + lane) * 4;               // first of this thread's 4 columns
   const long long row0 = static_cast<long long>(blockIdx.y) * kBwdRows;
@@ -86,12 +85,7 @@ __global__ void __launch_bounds__(256) bias_act_bwd_kernel(const float* g, const
     for (int k = 1; k < 8; ++k) { s.x += sh[k][lane].x; s.y += sh[k][lane].y; s.z += sh[k][lane].z; s.w += sh[k][lane].w; }
     *reinterpret_cast<float4*>(partial + static_cast<long long>(blockIdx.y) * H + col) = s;
   }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(&tickets[blockIdx.x], 1u) == gridDim.y - 1) ? 1u : 0u;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_cta(&tickets[blockIdx.x], gridDim.y)) return;   // one ticket per column block
   // last CTA of this column block: all 8 row-groups share the partial rows (fixed assignment and fixed
   // combination order -> deterministic), instead of one row-group walking all of them serially
   {
@@ -113,7 +107,6 @@ __global__ void __launch_bounds__(256) bias_act_bwd_kernel(const float* g, const
       *reinterpret_cast<float4*>(db + col) = t;
     }
   }
-  if (threadIdx.x == 0) tickets[blockIdx.x] = 0u;
 }
 
 }  // namespace trl

@@ -9,8 +9,9 @@
 // fp32 `count` would lose integer precision after 2^24 samples.  The batch moments are
 // produced by synth_env_step_kernel (per-CTA partials -> last CTA); trl_obs_norm_moments
 // computes them for an arbitrary (N,o) batch (host-env bridge / tests), trl_obs_norm_merge
-// is the stand-alone merge used when the batch sums were first all-reduced across GPUs.
-#include "common.cuh"
+// is the stand-alone merge used when the batch sums were first all-reduced across GPUs.  Both
+// merges are reduce.cuh's chan_merge.
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -44,16 +45,7 @@ __global__ void obs_merge_kernel(const double* __restrict__ sums, double batch_n
   const int j = threadIdx.x;
   const double cnt = *count;
   __syncthreads();
-  if (j < o) {
-    const double bmean = sums[j] / batch_n;
-    double bvar = sums[o + j] / batch_n - bmean * bmean;
-    if (bvar < 0.0) bvar = 0.0;
-    const double tot = cnt + batch_n;
-    const double delta = bmean - mean[j];
-    const double m2 = var[j] * cnt + bvar * batch_n + delta * delta * cnt * batch_n / tot;
-    mean[j] = mean[j] + delta * batch_n / tot;
-    var[j] = m2 / tot;
-  }
+  if (j < o) chan_merge(sums[j], sums[o + j], batch_n, cnt, mean[j], var[j]);
   if (j == 0) *count = cnt + batch_n;
 }
 

@@ -10,43 +10,13 @@
 //   DQN.update        /root/reference/torchrl/algo/off_policy/dqn.py:38-74
 // Every kernel returns the scalar loss (device), the gradient wrt the network outputs and the
 // logged statistics; network forward/backward stays in PyTorch.  Reductions are two-level and
-// deterministic (per-CTA partials, last CTA reduces in fixed order).  All HBM/latency-bound.
-#include "common.cuh"
+// deterministic (reduce.cuh: block_reduce_* per CTA, then the last CTA's thread 0 folds the partials
+// serially in CTA order).  All HBM/latency-bound.
+#include "reduce.cuh"
 
 namespace trl {
 
 constexpr int kOffThreads = 256;
-
-__device__ __forceinline__ double blk_sum(double v, double* sh) {
-  v = warp_sum(v);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[wid] = v;
-  __syncthreads();
-  double r = 0.0;
-  if (wid == 0) { r = lane < nw ? sh[lane] : 0.0; r = warp_sum(r); }
-  return r;  // valid in warp 0
-}
-__device__ __forceinline__ float blk_max(float v, float* sh) {
-  v = warp_max(v);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[wid] = v;
-  __syncthreads();
-  float r = -INFINITY;
-  if (wid == 0) { r = lane < nw ? sh[lane] : -INFINITY; r = warp_max(r); }
-  return r;
-}
-// true in exactly one CTA: the last one to arrive (partials of all CTAs are visible to it)
-__device__ __forceinline__ bool last_cta(unsigned* ticket) {
-  __shared__ unsigned s_last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (s_last) __threadfence();
-  return s_last != 0u;
-}
 
 // ---------------------------------------------------------------------------------------------
 // y = r + (1-d)*gamma*(min(q1n,q2n) - alpha*logp_next)      (alpha = exp(*log_alpha); SAC)
@@ -81,13 +51,12 @@ __global__ void __launch_bounds__(kOffThreads) td_target_kernel(const TdTargetPa
     const float nd = p.terminals[b] ? 0.f : 1.f;
     p.y[b] = r + nd * p.gamma * v;
   }
-  const double s = blk_sum(static_cast<double>(r), shd);
+  const double s = block_reduce_sum(static_cast<double>(r), shd);
   if (threadIdx.x == 0) p.partial[blockIdx.x] = s;
-  if (last_cta(p.ticket) && threadIdx.x == 0) {
+  if (last_cta(p.ticket, gridDim.x) && threadIdx.x == 0) {
     double acc = 0.0;
     for (unsigned i = 0; i < gridDim.x; ++i) acc += p.partial[i];
     p.info[0] = static_cast<float>(acc / static_cast<double>(p.B));
-    *p.ticket = 0u;
   }
 }
 
@@ -137,9 +106,9 @@ __global__ void __launch_bounds__(kOffThreads) sac_alpha_step_kernel(const Alpha
   __shared__ double shd[32];
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const double v = (b < p.B) ? static_cast<double>(p.logp[b] + p.target_entropy) : 0.0;
-  const double s = blk_sum(v, shd);
+  const double s = block_reduce_sum(v, shd);
   if (threadIdx.x == 0) p.partial[blockIdx.x] = s;
-  if (last_cta(p.ticket) && threadIdx.x == 0) {
+  if (last_cta(p.ticket, gridDim.x) && threadIdx.x == 0) {
     double acc = 0.0;
     for (unsigned i = 0; i < gridDim.x; ++i) acc += p.partial[i];
     const float mean_term = static_cast<float>(acc / static_cast<double>(p.B));
@@ -157,7 +126,6 @@ __global__ void __launch_bounds__(kOffThreads) sac_alpha_step_kernel(const Alpha
     *p.log_alpha = la_new;
     p.info[0] = expf(la_new);
     p.info[1] = loss;
-    *p.ticket = 0u;
   }
 }
 
@@ -198,12 +166,12 @@ __global__ void __launch_bounds__(kOffThreads) sac_policy_loss_kernel(const SacP
   double* pp = p.partial + static_cast<long long>(blockIdx.x) * 5;
   double r;
   float f;
-  r = blk_sum(static_cast<double>(L), shd);                      if (threadIdx.x == 0) pp[0] = r;
-  r = blk_sum(ok ? static_cast<double>(lp) : 0.0, shd);          if (threadIdx.x == 0) pp[1] = r;
-  r = blk_sum(ok ? static_cast<double>(lp) * lp : 0.0, shd);     if (threadIdx.x == 0) pp[2] = r;
-  f = blk_max(ok ? lp : -INFINITY, shf);                         if (threadIdx.x == 0) pp[3] = f;
-  f = blk_max(ok ? -lp : -INFINITY, shf);                        if (threadIdx.x == 0) pp[4] = -f;
-  if (last_cta(p.ticket) && threadIdx.x == 0) {
+  r = block_reduce_sum(static_cast<double>(L), shd);                      if (threadIdx.x == 0) pp[0] = r;
+  r = block_reduce_sum(ok ? static_cast<double>(lp) : 0.0, shd);          if (threadIdx.x == 0) pp[1] = r;
+  r = block_reduce_sum(ok ? static_cast<double>(lp) * lp : 0.0, shd);     if (threadIdx.x == 0) pp[2] = r;
+  f = block_reduce_max(ok ? lp : -INFINITY, shf);                         if (threadIdx.x == 0) pp[3] = f;
+  f = block_reduce_max(ok ? -lp : -INFINITY, shf);                        if (threadIdx.x == 0) pp[4] = -f;
+  if (last_cta(p.ticket, gridDim.x) && threadIdx.x == 0) {
     double t[5] = {0.0, 0.0, 0.0, -INFINITY, INFINITY};
     for (unsigned i = 0; i < gridDim.x; ++i) {
       const double* q = p.partial + static_cast<long long>(i) * 5;
@@ -217,7 +185,6 @@ __global__ void __launch_bounds__(kOffThreads) sac_policy_loss_kernel(const SacP
     p.info[2] = static_cast<float>(sqrt(var > 0.0 ? var : 0.0));
     p.info[3] = static_cast<float>(t[3]);
     p.info[4] = static_cast<float>(t[4]);
-    *p.ticket = 0u;
   }
 }
 
@@ -251,16 +218,15 @@ __global__ void __launch_bounds__(kOffThreads) twin_mse_kernel(const TwinMsePara
       p.g2[b] = 2.f * d2 * invB;
     }
   }
-  double r = blk_sum(static_cast<double>(l1), shd);
+  double r = block_reduce_sum(static_cast<double>(l1), shd);
   if (threadIdx.x == 0) p.partial[2 * blockIdx.x] = r;
-  r = blk_sum(static_cast<double>(l2), shd);
+  r = block_reduce_sum(static_cast<double>(l2), shd);
   if (threadIdx.x == 0) p.partial[2 * blockIdx.x + 1] = r;
-  if (last_cta(p.ticket) && threadIdx.x == 0) {
+  if (last_cta(p.ticket, gridDim.x) && threadIdx.x == 0) {
     double a = 0.0, c = 0.0;
     for (unsigned i = 0; i < gridDim.x; ++i) { a += p.partial[2 * i]; c += p.partial[2 * i + 1]; }
     p.info[0] = static_cast<float>(a / static_cast<double>(p.B));
     p.info[1] = static_cast<float>(c / static_cast<double>(p.B));
-    *p.ticket = 0u;
   }
 }
 
@@ -354,22 +320,21 @@ __global__ void __launch_bounds__(kOffThreads) qr_loss_kernel(const QrParams p) 
     }
     gb[act * Q + i] = g;
   }
-  double v = blk_sum(lsum, shd);
+  double v = block_reduce_sum(lsum, shd);
   if (tid == 0) {
     p.partial[3 * b] = v * wb;
     // un-weighted per-sample loss magnitude: |TD| for DQN, mean quantile-Huber loss for QR-DQN
     if (p.td_out) p.td_out[b] = p.mse ? sqrtf(static_cast<float>(v)) : static_cast<float>(v / (static_cast<double>(Q) * Q));
   }
-  v = blk_sum(qsum, shd);
+  v = block_reduce_sum(qsum, shd);
   if (tid == 0) { p.partial[3 * b + 1] = v; p.partial[3 * b + 2] = r; }
-  if (last_cta(p.ticket) && tid == 0) {
+  if (last_cta(p.ticket, gridDim.x) && tid == 0) {
     double l = 0.0, q = 0.0, rr = 0.0;
     for (int i = 0; i < p.B; ++i) { l += p.partial[3 * i]; q += p.partial[3 * i + 1]; rr += p.partial[3 * i + 2]; }
     const double nB = static_cast<double>(p.B);
     p.info[0] = static_cast<float>(p.mse ? l / nB : l / (nB * Q * Q));
     p.info[1] = static_cast<float>(q / (nB * Q));
     p.info[2] = static_cast<float>(rr / nB);
-    *p.ticket = 0u;
   }
 }
 

@@ -13,7 +13,7 @@
 //   trl_adam_step   : clip coefficient + Adam + zero the gradient, one pass over the buffers
 // The same flat gradient buffer is what NCCL all-reduces in the multi-GPU path (K12).
 // HBM-bound: 4 reads + 4 writes of 4 B per parameter.
-#include "common.cuh"
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -41,7 +41,6 @@ struct SumsqParams {
 // grid = nseg * blocks_per_seg
 __global__ void __launch_bounds__(kOptThreads) grad_sumsq_kernel(const SumsqParams p) {
   __shared__ double sh[32];
-  __shared__ unsigned s_last;
   const int s = blockIdx.x / p.blocks_per_seg, bi = blockIdx.x % p.blocks_per_seg;
   double acc = 0.0;
   if ((p.active_mask >> s) & 1u) {
@@ -52,47 +51,13 @@ __global__ void __launch_bounds__(kOptThreads) grad_sumsq_kernel(const SumsqPara
       acc += static_cast<double>(v) * v;
     }
   }
-  acc = warp_sum(acc);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) sh[wid] = acc;
-  __syncthreads();
-  if (wid == 0) {
-    acc = lane < (blockDim.x >> 5) ? sh[lane] : 0.0;
-    acc = warp_sum(acc);
-    if (lane == 0) p.partial[blockIdx.x] = acc;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  if (threadIdx.x < p.seg.nseg) {
-    const int k = threadIdx.x;
-    if ((p.active_mask >> k) & 1u) {
-      // the partials are requested 16 at a time before they are added (same order as a plain loop, one L2 round
-      // trip instead of one per partial)
-      double t = 0.0;
-      for (int i0 = 0; i0 < p.blocks_per_seg; i0 += 16) {
-        double v[16];
-#pragma unroll
-        for (int u = 0; u < 16; ++u)
-          v[u] = (i0 + u < p.blocks_per_seg) ? __ldcg(p.partial + k * p.blocks_per_seg + i0 + u) : 0.0;
-#pragma unroll
-        for (int u = 0; u < 16; ++u) t += v[u];
-      }
-      p.out[k] = t;
-      if (p.step) {
-        const int st = p.step[k] + 1;
-        p.step[k] = st;
-        // bias corrections in fp64 once per segment (torch computes them in Python floats)
-        p.out[p.seg.nseg + 2 * k] = 1.0 - pow_int(p.beta1, st);
-        p.out[p.seg.nseg + 2 * k + 1] = sqrt(1.0 - pow_int(p.beta2, st));
-      }
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) *p.ticket = 0u;
+  acc = block_reduce_sum</*kReuse=*/false>(acc, sh);
+  if (threadIdx.x == 0) p.partial[blockIdx.x] = acc;
+  if (!last_cta(p.ticket, gridDim.x)) return;
+  const int k = threadIdx.x;
+  if (k < p.seg.nseg && ((p.active_mask >> k) & 1u))
+    sumsq_segment_tail(p.partial + k * p.blocks_per_seg, p.blocks_per_seg, 1, k, p.seg.nseg, p.out, p.step, p.beta1,
+                       p.beta2);
 }
 
 struct AdamParams {

@@ -9,8 +9,9 @@
 // One launch produces the scalar loss, dL/d(mean), dL/d(log_std) and the logged statistics;
 // the caller seeds torch.autograd.backward at the MLP outputs with these gradients, so no
 // intermediate (B,a) tensors ever round-trip through HBM and nothing syncs with the host.
-// Reductions are two-level (per-CTA partials, last CTA reduces in fixed order): deterministic.
-#include "loss_reduce.cuh"
+// Reductions are two-level and deterministic (reduce.cuh: per-CTA partials, then last_cta; each kernel's last CTA folds
+// the partials in its own fixed order).
+#include "reduce.cuh"
 
 namespace trl {
 
@@ -54,7 +55,6 @@ __device__ __forceinline__ float clamped_ls(const ActorParams& p, float raw, boo
 }
 
 __global__ void __launch_bounds__(kLossThreads) ppo_actor_loss_kernel(const ActorParams p) {
-  __shared__ unsigned s_last;
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const bool ok = b < p.B;
   const int a = p.a;
@@ -166,12 +166,7 @@ __global__ void __launch_bounds__(kLossThreads) ppo_actor_loss_kernel(const Acto
       pp[slot] = (q & 1) ? -static_cast<double>(m) : static_cast<double>(m);
     }
   }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_cta(p.ticket, gridDim.x)) return;
   // ---- last CTA: fixed-order reduction of the partials ----------------------------------
   const int K = kActorFixed + a;   // <= 44
   const int nb = gridDim.x;
@@ -254,7 +249,6 @@ __global__ void __launch_bounds__(kLossThreads) ppo_actor_loss_kernel(const Acto
     clamped_ls(p, p.log_std[j], &pass);
     p.g_log_std[j] = pass ? static_cast<float>(t[kActorFixed + j]) - p.ent_coef : 0.f;
   }
-  if (threadIdx.x == 0) *p.ticket = 0u;
 }
 
 // ------------------------------------------------------------------------------------ critic
@@ -273,7 +267,6 @@ struct CriticParams {
 
 __global__ void __launch_bounds__(kLossThreads) ppo_critic_loss_kernel(const CriticParams p) {
   __shared__ double shd[32];
-  __shared__ unsigned s_last;
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const float invB = 1.0f / static_cast<float>(p.B);
   float L = 0.f;
@@ -299,21 +292,13 @@ __global__ void __launch_bounds__(kLossThreads) ppo_critic_loss_kernel(const Cri
   }
   double r = block_reduce_sum(static_cast<double>(L), shd);
   if (threadIdx.x == 0) p.partial[blockIdx.x] = r;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
+  if (!last_cta(p.ticket, gridDim.x)) return;
   if (threadIdx.x < 32) {
     // lane l folds partials l, l+32, ... (independent loads), then a fixed shuffle tree: deterministic
     double acc = 0.0;
     for (unsigned i = threadIdx.x; i < gridDim.x; i += 32) acc += __ldcg(p.partial + i);
     acc = warp_sum(acc);
-    if (threadIdx.x == 0) {
-      p.info[0] = static_cast<float>(acc / static_cast<double>(p.B));
-      *p.ticket = 0u;
-    }
+    if (threadIdx.x == 0) p.info[0] = static_cast<float>(acc / static_cast<double>(p.B));
   }
 }
 
