@@ -50,8 +50,9 @@ __device__ __forceinline__ void st_stream(float4* p, float4 v) { __stcs(p, v); }
 
 // ---- tanh on the MUFU pipe -----------------------------------------------------------
 // tanh(x) = 1 - 2 / (exp(2x) + 1) as FMUL, MUFU.EX2, FADD, MUFU.RCP, FFMA (5 instructions; libdevice tanhf is ~25 with
-// a branch).  ex2.approx is good to 2^-22 relative and rcp.approx to 1 ulp, so |abs err| < 2e-7: the fp32 round-off of
-// the activations themselves.  Saturation needs no clamp: exp -> +inf gives rcp -> +0 -> 1, exp -> 0 gives 1 - 2 = -1.
+// a branch).  ex2.approx is good to 2^-22 relative and rcp.approx to 1 ulp, so |abs err| < 2.5e-7 (2.31e-7 measured on
+// an H100 over 2^20 points in [-20, 20]): a few ulp of the activations.  Saturation needs no clamp: exp -> +inf gives
+// rcp -> +0 -> 1, exp -> 0 gives 1 - 2 = -1.
 __device__ __forceinline__ float tanh_ex2(float x) {
   float e, r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * 2.8853900817779268f));

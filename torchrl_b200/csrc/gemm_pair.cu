@@ -5,7 +5,7 @@
 //     step (csrc/optim.cu writes both planes), TMA loads both planes and only the activation operand A is split;
 //   * B may be N-major (b_nmajor): the dgrad shape dX = G . W reads W (K x 256, row-major) directly -- no per-
 //     minibatch transpose of the weights;
-//   * tanh = 1 - 2/(exp(2x)+1) on the MUFU unit (abs err < 2e-7, same as csrc/skinny.cu);
+//   * tanh = 1 - 2/(exp(2x)+1) on the MUFU unit (abs err < 2.5e-7, same as csrc/skinny.cu);
 //   * split-K slabs are summed by an 8-way balanced tree (pair_splitk_reduce_kernel).
 // Shapes:
 //   nt   : A (M x K) row-major, B (256 x K) row-major      forward  y = act(x W^T + b)
