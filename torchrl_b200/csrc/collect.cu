@@ -283,6 +283,8 @@ TRL_API int trl_tanh_gaussian_sample_bwd(const float* action, const float* eps, 
   TRL_REQUIRE(M >= 0 && act_dim >= 1, "trl_tanh_gaussian_sample_bwd: bad sizes");
   if (M == 0) return TRL_OK;
   TRL_REQUIRE(action && eps && log_std && g_mean && g_log_std, "trl_tanh_gaussian_sample_bwd: null pointer");
+  TRL_REQUIRE(ls_stride == 0 || ls_stride == act_dim,
+              "trl_tanh_gaussian_sample_bwd: ls_stride must be 0 or act_dim");
   SampleBwdParams p{action, eps, log_std, g_action, g_logp, g_mean, g_log_std, M, act_dim, ls_stride, tanh_action};
   tanh_gaussian_sample_bwd_kernel<<<static_cast<unsigned>(ceil_div<long long>(M * act_dim, 256)), 256, 0,
                                     static_cast<cudaStream_t>(stream)>>>(p);

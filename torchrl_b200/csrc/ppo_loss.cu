@@ -156,8 +156,9 @@ __global__ void __launch_bounds__(kLossThreads) ppo_actor_loss_kernel(const Acto
       // partial slots: 0 L, 1 logp, 2 logp^2, 7 ls, 8 ls^2, 11 dkl, 12+j dL/dls_j
       const int slot = k == 0 ? 0 : k == 1 ? 1 : k == 2 ? 2 : k == 3 ? 7 : k == 4 ? 8 : k == 5 ? 11 : kActorFixed + (k - 6);
       pp[slot] = t;
-    } else if (k >= 32 && k < 38) {
-      const int q = k - 32;
+    } else if (k >= 6 + kMaxAct && k < 12 + kMaxAct) {
+      // threads of their own, past the largest nsum: with a shared log-std and a >= 27 the sum slots reach thread 32
+      const int q = k - (6 + kMaxAct);
       float m = -INFINITY;
 #pragma unroll
       for (int w = 0; w < NW; ++w) m = fmaxf(m, sh_max[w][q]);
