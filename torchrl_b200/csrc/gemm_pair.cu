@@ -67,9 +67,9 @@ TRL_API int trl_gemm3_pair(const float* A, const float* b_hi, const float* b_lo,
   TRL_REQUIRE(act >= 0 && act <= 2, "trl_gemm3_pair: unknown activation %d", act);
   CUtensorMap ma, mb, mb2;
   const uint64_t b_rows = b_nmajor ? static_cast<uint64_t>(K) : kN, b_cols = b_nmajor ? kN : static_cast<uint64_t>(K);
-  if (!make_map(&ma, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), false) ||
-      !make_map(&mb, b_hi, b_rows, b_cols, b_nmajor != 0) ||
-      !make_map(&mb2, b_lo ? b_lo : b_hi, b_rows, b_cols, b_nmajor != 0)) {
+  const Box b_box = b_nmajor ? Box::kMNMajor : Box::kKMajor;
+  if (!make_map(&ma, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), Box::kKMajor) ||
+      !make_map(&mb, b_hi, b_rows, b_cols, b_box) || !make_map(&mb2, b_lo ? b_lo : b_hi, b_rows, b_cols, b_box)) {
     set_error("trl_gemm3_pair: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }
@@ -99,8 +99,8 @@ TRL_API int trl_gemm3_pair_tn(const float* A, const float* B, float* C, int64_t 
   TRL_REQUIRE(aligned16(A) && aligned16(B) && aligned16(C) && aligned16(workspace),
               "trl_gemm3_pair_tn: pointers must be 16-byte aligned");
   CUtensorMap ma, mb;
-  if (!make_map(&ma, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), true) ||
-      !make_map(&mb, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), true)) {
+  if (!make_map(&ma, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), Box::kMNMajorA) ||
+      !make_map(&mb, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), Box::kMNMajor)) {
     set_error("trl_gemm3_pair_tn: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }

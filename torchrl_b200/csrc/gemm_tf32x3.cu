@@ -75,8 +75,8 @@ TRL_API int trl_gemm_tf32x3_nt(const float* A, const float* B, float* C, int64_t
   TRL_REQUIRE(act >= 0 && act <= 2, "trl_gemm_tf32x3_nt: unknown activation %d", act);
   using namespace trl::wg;
   CUtensorMap map_a, map_b;
-  if (!make_map(&map_a, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), false) ||
-      !make_map(&map_b, B, static_cast<uint64_t>(kN), static_cast<uint64_t>(K), false)) {
+  if (!make_map(&map_a, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), Box::kKMajor) ||
+      !make_map(&map_b, B, static_cast<uint64_t>(kN), static_cast<uint64_t>(K), Box::kKMajor)) {
     set_error("trl_gemm_tf32x3_nt: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }
@@ -105,8 +105,8 @@ TRL_API int trl_gemm_tf32x3_tn(const float* A, const float* B, float* C, int64_t
   using namespace trl::wg;
   CUtensorMap map_a, map_b;
   // (K rows) x (M | 256 contiguous) matrices, consumed M/N-major
-  if (!make_map(&map_a, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), true) ||
-      !make_map(&map_b, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), true)) {
+  if (!make_map(&map_a, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), Box::kMNMajorA) ||
+      !make_map(&map_b, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), Box::kMNMajor)) {
     set_error("trl_gemm_tf32x3_tn: cuTensorMapEncodeTiled failed");
     return TRL_EUNSUPPORTED;
   }

@@ -9,15 +9,20 @@
 // large sum takes one add per K step instead of three.  Callers keep K / splits <= 256 where accuracy matters (the
 // wgrad shape splits K).
 //
-// One CTA per 128 x 128 output tile and K slab (gridDim = (M tiles, 2 column halves, splits)), 288 threads:
-//   warp 8       TMA producer : cp.async.bulk.tensor 2D loads of the raw fp32 A / B tiles (no swizzle) into a
-//                               2-stage ring, mbarrier complete_tx
-//   warps 0..7   two consumer warpgroups.  Per K block of 32: split raw -> (hi, lo) while re-laying the tile out as the
-//                               K-major SWIZZLE_128B canonical layout wgmma reads (this is also where M/N-major sources --
-//                               the dgrad B and both wgrad operands -- are transposed: wgmma takes tf32 operands from
-//                               shared memory only K-major), release the raw stage, then warpgroup w issues the 12
-//                               wgmma of its 64 rows into two register accumulators (see above).  The hi/lo tiles
-//                               are double-buffered, so the MMAs of block kb run while block kb + 1 is converted.
+// One CTA per 128 x 128 output tile and K slab (gridDim = (M tiles, 2 column halves, splits)), 384 threads:
+//   warps 8..11  producer     : one thread issues cp.async.bulk.tensor 2D loads of one K block (32 deep) per ring stage, mbarrier
+//                               complete_tx.  K-major operands arrive SWIZZLE_128B, i.e. already in the canonical
+//                               layout the wgmma B descriptor reads (16-byte chunk c of row r at chunk c ^ (r & 7)).
+//   warps 0..7   two consumer warpgroups.  Per K block:
+//                  A: each thread loads its m64k8 register fragments straight from the TMA tile, splits them with
+//                     cvt.rna in registers and issues the register-A form of wgmma (no A planes in shared memory);
+//                  B: pre-split K-major planes (the forward) are read by the MMAs where TMA put them.  Every other B
+//                     is converted once by the consumers into the stage's hi / lo planes -- raw K-major: split in
+//                     place; N-major (dgrad, wgrad): transposed, since wgmma takes tf32 operands from shared memory
+//                     only K-major -- and handed to both warpgroups through an mbarrier;
+//                  warpgroup w issues the 12 wgmma of its 64 rows into two register accumulators (see above), waits
+//                  for them and releases the stage to the producer.  The ring is 2-4 stages deep (as many as fit), so
+//                  TMA runs ahead of the MMAs and the two warpgroups drift against each other without a CTA barrier.
 //   epilogue                  accumulator fragments -> bias / activation -> global (float2 per thread, 32-byte rows).
 // Shapes (template flags):
 //   AMN = false: A (M x K) row-major;  AMN = true: A (K x M) row-major (reduction index = row index)
@@ -31,14 +36,23 @@ namespace trl {
 namespace wg {
 
 constexpr int kBM = 128, kBN = 128, kN = 256, kBK = 32;
-constexpr int kRawStages = 2;
 constexpr int kTileBytes = 128 * kBK * 4;                 // 16 KB: one 128 x 32 fp32 tile
-constexpr int kRawStageBytes = 3 * kTileBytes;            // A | B (hi) | B lo (pre-split B only)
-constexpr int kHiLoBytes = 4 * kTileBytes;                // A hi | A lo | B hi | B lo
 constexpr int kConsumers = 256;                           // two warpgroups
-constexpr int kThreads = kConsumers + 32;                 // + TMA warp
-constexpr int kSmemBytes = 2 * kHiLoBytes + kRawStages * kRawStageBytes + 1024 /*align*/ + 64 /*barriers*/;
-static_assert(kSmemBytes <= 227 * 1024, "fits one sm_90 CTA");
+constexpr int kThreads = kConsumers + 128;                // + producer warpgroup (one TMA thread)
+// Registers per thread: 168 at launch (__launch_bounds__(384, 1)); the producer warpgroup drops to 40 and the consumers
+// take 232 (8 x 32 x 232 + 4 x 32 x 40 <= 64 K), which holds both accumulators and the A fragments of a K block.
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
+// Ring stage: A | B hi | B lo [| raw N-major B | raw N-major B lo plane].  The stage count fills ~200 KB.
+template <bool BMN, bool BSPLIT>
+struct Ring {
+  static constexpr int kTiles = 3 + (BMN ? (BSPLIT ? 2 : 1) : 0);
+  static constexpr int kStageBytes = kTiles * kTileBytes;
+  static constexpr int kStages = (200 * 1024) / kStageBytes < 4 ? (200 * 1024) / kStageBytes : 4;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 128 /*barriers*/;
+  static constexpr bool kConvertB = BMN || !BSPLIT;       // the consumers write the B planes
+  static_assert(kStages >= 2 && kSmemBytes <= 227 * 1024, "fits one sm_90 CTA");
+};
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -71,8 +85,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer)
       : "memory");
 }
-// named barrier of the two consumer warpgroups (the TMA warp does not take part)
-__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
 
 // K-major SWIZZLE_128B canonical layout: rows of 32 fp32 (128 B), 16-byte chunk c of row r stored at chunk c ^ (r & 7),
 // 8-row atoms of 1024 B.  Descriptor: start >> 4, LBO unused (1), SBO = 1024 B, layout type 1 (128B swizzle).
@@ -85,18 +97,20 @@ __device__ __forceinline__ uint64_t desc_k_sw128(uint32_t smem_addr) {
   return d;
 }
 
-// d[64] += A(64 x 8) . B(128 x 8)^T, both K-major in shared memory, tf32 inputs, fp32 accumulate (one warpgroup)
-__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
+// d[64] += A(64 x 8) . B(128 x 8)^T, A from registers (this thread's m64k8 tf32 fragment: rows gid, gid + 8 of its
+// warp's 16, k = tid, tid + 4 as a = {(gid, tid), (gid + 8, tid), (gid, tid + 4), (gid + 8, tid + 4)}), B K-major in
+// shared memory, fp32 accumulate (one warpgroup)
+__device__ __forceinline__ void wgmma_m64n128k8_tf32_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
       "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
       "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1;\n\t"
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t"
       "}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
@@ -106,7 +120,7 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t de
         "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
         "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
         "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(desc_a), "l"(desc_b), "r"(1));
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(1));
 }
 
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
@@ -122,29 +136,40 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
 __device__ __forceinline__ void sts128(uint32_t addr, const float4 v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w));
 }
+__device__ __forceinline__ uint32_t tf32_bits(float x) {
+  uint32_t u;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
+  return u;
+}
 __device__ __forceinline__ float4 tf32_hi(const float4 v) {
-  float4 h;
-  unsigned u;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.x)); h.x = __uint_as_float(u);
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.y)); h.y = __uint_as_float(u);
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.z)); h.z = __uint_as_float(u);
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v.w)); h.w = __uint_as_float(u);
-  return h;
+  return make_float4(__uint_as_float(tf32_bits(v.x)), __uint_as_float(tf32_bits(v.y)), __uint_as_float(tf32_bits(v.z)),
+                     __uint_as_float(tf32_bits(v.w)));
+}
+__device__ __forceinline__ float4 sub4(const float4 a, const float4 b) {
+  return make_float4(a.x - b.x, a.y - b.y, a.z - b.z, a.w - b.w);
 }
 
-// float4 unit u (0..1023) of a 128 x 32 tile: its row of the K-major destination and its 16-byte chunk (4 reduction
-// indices), read from the raw tile as TMA delivered it: (128 rows x 32) for K-major sources, (32 x 128) for M/N-major
-__device__ __forceinline__ float4 load_unit(uint32_t raw, int u, bool mn, int& row, int& chunk) {
-  if (!mn) {
-    row = u >> 3; chunk = u & 7;
-    return lds128(raw + static_cast<uint32_t>(u) * 16u);
-  }
+// float4 unit u (0..1023) of a raw M/N-major 128 x 32 tile as TMA delivered it (32 reduction rows x 128): its row of
+// the K-major destination and its 16-byte chunk (4 reduction indices)
+__device__ __forceinline__ float4 load_unit_mn(uint32_t raw, int u, int& row, int& chunk) {
   row = u & 127; chunk = u >> 7;
   const uint32_t a = raw + static_cast<uint32_t>(chunk * 4 * 128 + row) * 4u;
   return make_float4(lds32(a), lds32(a + 512u), lds32(a + 1024u), lds32(a + 1536u));
 }
 __device__ __forceinline__ uint32_t sw128(int row, int chunk) {
   return static_cast<uint32_t>(row * 128 + ((chunk ^ (row & 7)) << 4));
+}
+
+// Byte offset of A element (m, k) of the block in its stage slot.
+//   K-major A: one 32 x 128 box, SWIZZLE_128B.  A warp's fragment load (fixed k chunk, rows gid = 0..7, k & 3 = tid)
+//     hits chunk c ^ gid, word tid: 32 distinct banks.
+//   M-major A: four 32 (m) x 32 (k) boxes, SWIZZLE_128B: row k holds 32 m.  A warp's load (m = 16 w + gid + 8 h, k =
+//     tid + 4 c) hits chunk ((m & 31) >> 2) ^ (k & 7), word m & 3: (gid >> 2, tid) = (0, 1) and (1, 0) share a chunk, so
+//     2 wavefronts, 16 distinct banks.
+template <bool AMN>
+__device__ __forceinline__ uint32_t a_offset(int m, int k) {
+  if (!AMN) return static_cast<uint32_t>(m * 128 + ((((k >> 2) ^ (m & 7))) << 4) + (k & 3) * 4);
+  return static_cast<uint32_t>((m >> 5) * 4096 + k * 128 + ((((m & 31) >> 2) ^ (k & 7)) << 4) + (m & 3) * 4);
 }
 
 struct Params {
@@ -160,13 +185,15 @@ template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                    const __grid_constant__ CUtensorMap map_b2, const Params p) {
+  using R = Ring<BMN, BSPLIT>;
+  constexpr int S = R::kStages;
+  constexpr int kA = 0, kBhi = kTileBytes, kBlo = 2 * kTileBytes, kBraw = 3 * kTileBytes, kBraw2 = 4 * kTileBytes;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* hilo = smem;                                    // [2][A hi | A lo | B hi | B lo]
-  uint8_t* raw = smem + 2 * kHiLoBytes;                    // [kRawStages][A | B | B lo]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(raw + kRawStages * kRawStageBytes);
-  uint64_t* full = bars;                                   // [kRawStages] TMA -> consumers
-  uint64_t* empty = bars + kRawStages;                     // [kRawStages] consumers -> TMA
+  uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + S * R::kStageBytes);
+  uint64_t* full = bars;                                   // [S] TMA -> consumers
+  uint64_t* empty = bars + S;                              // [S] consumers' MMAs done -> TMA
+  uint64_t* conv = bars + 2 * S;                           // [S] B planes written -> both warpgroups (kConvertB)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, n0 = blockIdx.y * kBN, split = blockIdx.z;
@@ -177,31 +204,38 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
     if (BSPLIT) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b2)) : "memory");
-    for (int s = 0; s < kRawStages; ++s) {
+    for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], kConsumers / 32);               // one arrival per consumer warp
+      mbar_init(&conv[s], kConsumers / 32);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  if (warp == kConsumers / 32) {
+  if (warp >= kConsumers / 32) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == kConsumers / 32 && lane == 0) {
       for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % kRawStages;
-        const uint32_t ph = (kb / kRawStages) & 1;
+        const int s = kb % S;
+        const uint32_t ph = (kb / S) & 1;
         mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* st = raw + s * kRawStageBytes;
+        uint8_t* st = ring + s * R::kStageBytes;
         mbar_arrive_expect_tx(&full[s], (BSPLIT ? 3 : 2) * kTileBytes);
         const int k0 = (kb0 + kb) * kBK;
-        if (AMN) tma_load_2d(st, &map_a, &full[s], m_blk * kBM, k0);
-        else tma_load_2d(st, &map_a, &full[s], k0, m_blk * kBM);
-        if (BMN) tma_load_2d(st + kTileBytes, &map_b, &full[s], n0, k0);
-        else tma_load_2d(st + kTileBytes, &map_b, &full[s], k0, n0);
-        if (BSPLIT) {
-          if (BMN) tma_load_2d(st + 2 * kTileBytes, &map_b2, &full[s], n0, k0);
-          else tma_load_2d(st + 2 * kTileBytes, &map_b2, &full[s], k0, n0);
+        if (AMN) {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) tma_load_2d(st + kA + j * 4096, &map_a, &full[s], m_blk * kBM + 32 * j, k0);
+        } else {
+          tma_load_2d(st + kA, &map_a, &full[s], k0, m_blk * kBM);
+        }
+        if (BMN) {
+          tma_load_2d(st + kBraw, &map_b, &full[s], n0, k0);
+          if (BSPLIT) tma_load_2d(st + kBraw2, &map_b2, &full[s], n0, k0);
+        } else {
+          tma_load_2d(st + kBhi, &map_b, &full[s], k0, n0);
+          if (BSPLIT) tma_load_2d(st + kBlo, &map_b2, &full[s], k0, n0);
         }
       }
     }
@@ -209,77 +243,84 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
   }
 
   // -------------------------------------------------------------------- consumers
-  const int ct = threadIdx.x, wgi = warp >> 2;
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+  const int ct = threadIdx.x, wgi = warp >> 2, wl = warp & 3;
+  const int gid = lane >> 2, tid = lane & 3;
+  const int am = wgi * 64 + wl * 16 + gid;                 // this thread's fragment rows: am, am + 8
   float acc[64], cor[64];                                  // hi*hi | lo*hi + hi*lo
 #pragma unroll
   for (int i = 0; i < 64; ++i) { acc[i] = 0.f; cor[i] = 0.f; }
   for (int kb = 0; kb < nkb; ++kb) {
-    const int s = kb % kRawStages;
-    const uint32_t ph = (kb / kRawStages) & 1;
-    const uint32_t rs = smem_u32(raw + s * kRawStageBytes);
-    const uint32_t hs = smem_u32(hilo + (kb & 1) * kHiLoBytes);
+    const int s = kb % S;
+    const uint32_t ph = (kb / S) & 1;
+    const uint32_t st = smem_u32(ring + s * R::kStageBytes);
     mbar_wait(&full[s], ph);
-    // per operand: all loads of this thread first (independent accesses in flight), then split and store
-    {
-      float4 va[4];
-      int ra[4], ca[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) va[i] = load_unit(rs, ct + i * kConsumers, AMN, ra[i], ca[i]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 h = tf32_hi(va[i]);
-        const uint32_t o = sw128(ra[i], ca[i]);
-        sts128(hs + o, h);
-        sts128(hs + kTileBytes + o, make_float4(va[i].x - h.x, va[i].y - h.y, va[i].z - h.z, va[i].w - h.w));
-      }
-    }
-    {
+    if (R::kConvertB) {
+      // all loads of this thread first (independent accesses in flight), then split / re-lay out and store
       float4 vb[4], vl[4];
       int rb[4], cb[4];
+      if (BMN) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) vb[i] = load_unit(rs + kTileBytes, ct + i * kConsumers, BMN, rb[i], cb[i]);
-      if (BSPLIT) {
+        for (int i = 0; i < 4; ++i) vb[i] = load_unit_mn(st + kBraw, ct + i * kConsumers, rb[i], cb[i]);
+        if (BSPLIT) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) vl[i] = load_unit(rs + 2 * kTileBytes, ct + i * kConsumers, BMN, rb[i], cb[i]);
+          for (int i = 0; i < 4; ++i) vl[i] = load_unit_mn(st + kBraw2, ct + i * kConsumers, rb[i], cb[i]);
+        }
+      } else {                                             // raw K-major B, already swizzled: split in place
+#pragma unroll
+        for (int i = 0; i < 4; ++i) vb[i] = lds128(st + kBhi + static_cast<uint32_t>(ct + i * kConsumers) * 16u);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);               // raw stage s may be refilled
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const uint32_t o = sw128(rb[i], cb[i]);
+        const uint32_t o = BMN ? sw128(rb[i], cb[i]) : static_cast<uint32_t>(ct + i * kConsumers) * 16u;
         if (BSPLIT) {
-          sts128(hs + 2 * kTileBytes + o, vb[i]);
-          sts128(hs + 3 * kTileBytes + o, vl[i]);
+          sts128(st + kBhi + o, vb[i]);
+          sts128(st + kBlo + o, vl[i]);
         } else {
           const float4 h = tf32_hi(vb[i]);
-          sts128(hs + 2 * kTileBytes + o, h);
-          sts128(hs + 3 * kTileBytes + o, make_float4(vb[i].x - h.x, vb[i].y - h.y, vb[i].z - h.z, vb[i].w - h.w));
+          sts128(st + kBhi + o, h);
+          sts128(st + kBlo + o, sub4(vb[i], h));
         }
       }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&conv[s]);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
-    consumers_sync();
-    const uint64_t da_hi = desc_k_sw128(hs + wgi * 64 * 128), da_lo = desc_k_sw128(hs + kTileBytes + wgi * 64 * 128);
-    const uint64_t db_hi = desc_k_sw128(hs + 2 * kTileBytes), db_lo = desc_k_sw128(hs + 3 * kTileBytes);
+    // A fragments of the 4 K steps, split in registers
+    uint32_t ahi[kBK / 8][4], alo[kBK / 8][4];
+    {
+      float av[kBK / 8][4];
+#pragma unroll
+      for (int k = 0; k < kBK / 8; ++k)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) av[k][r] = lds32(st + kA + a_offset<AMN>(am + 8 * (r & 1), 8 * k + tid + 4 * (r >> 1)));
+#pragma unroll
+      for (int k = 0; k < kBK / 8; ++k)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          ahi[k][r] = tf32_bits(av[k][r]);
+          alo[k][r] = __float_as_uint(av[k][r] - __uint_as_float(ahi[k][r]));
+        }
+    }
+    if (R::kConvertB) mbar_wait(&conv[s], ph);
+    const uint64_t db_hi = desc_k_sw128(st + kBhi), db_lo = desc_k_sw128(st + kBlo);
     asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
     for (int k = 0; k < kBK / 8; ++k) {
       const uint64_t adv = static_cast<uint64_t>((k * 8 * 4) >> 4);   // +32 B per K step inside the 128 B row
-      wgmma_m64n128k8_tf32(cor, da_lo + adv, db_hi + adv);
-      wgmma_m64n128k8_tf32(cor, da_hi + adv, db_lo + adv);
-      wgmma_m64n128k8_tf32(acc, da_hi + adv, db_hi + adv);
+      wgmma_m64n128k8_tf32_rs(cor, alo[k], db_hi + adv);
+      wgmma_m64n128k8_tf32_rs(cor, ahi[k], db_lo + adv);
+      wgmma_m64n128k8_tf32_rs(acc, ahi[k], db_hi + adv);
     }
     asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
-    consumers_sync();                                      // the MMAs of block kb - 1 (both warpgroups) are complete:
-                                                           // its hi/lo buffer may be rewritten
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);                 // this warp is done with stage s
   }
-  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 
   // -------------------------------------------------------------------- epilogue
   // fragment i of this thread: rows r0 and r0 + 8, columns n0 + 8 (i / 4) + 2 (lane % 4) + {0, 1}
-  const int wl = warp & 3;
-  const long long r0 = static_cast<long long>(m_blk) * kBM + wgi * 64 + wl * 16 + (lane >> 2);
+  const long long r0 = static_cast<long long>(m_blk) * kBM + am;
   float* cbase = p.C + static_cast<long long>(split) * p.M * kN;
   const bool has_bias = p.bias != nullptr;
 #pragma unroll
@@ -321,34 +362,41 @@ inline PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// (rows x cols) fp32 row-major operand, unswizzled boxes of one 128 x 32 tile: K-major (cols = K): 32 contiguous
-// elements x 128 rows; M/N-major (rows = K): 128 contiguous elements x 32 reduction rows.  Out-of-range rows are
-// filled with zeros (ragged M).
-inline bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, bool mn_major) {
+// How an operand's 128 x 32 tile is boxed:
+//   kKMajor  : reduction index = column.  One 32 x 128 box, SWIZZLE_128B (the wgmma K-major layout).
+//   kMNMajor : reduction index = row.  One 128 x 32 box, no swizzle (transposed by the consumers).
+//   kMNMajorA: reduction index = row.  32 x 32 boxes (four per tile), SWIZZLE_128B (the register-A fragment loads).
+enum class Box { kKMajor, kMNMajor, kMNMajorA };
+
+// (rows x cols) fp32 row-major operand.  Out-of-range rows are filled with zeros (ragged M).
+inline bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, Box box_kind) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return false;
   const cuuint64_t gdim[2] = {cols, rows};
   const cuuint64_t gstride[1] = {cols * sizeof(float)};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(mn_major ? 128 : kBK), static_cast<cuuint32_t>(mn_major ? kBK : 128)};
+  const cuuint32_t inner = box_kind == Box::kMNMajor ? 128 : kBK;
+  const cuuint32_t box[2] = {inner, static_cast<cuuint32_t>(box_kind == Box::kKMajor ? 128 : kBK)};
   const cuuint32_t estr[2] = {1, 1};
   return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+             CU_TENSOR_MAP_INTERLEAVE_NONE,
+             box_kind == Box::kMNMajor ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
+             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // grid: (ceil(M / 128), 2, splits); p.C is the split-K workspace when splits > 1
 template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU>
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mb2, const Params& p, unsigned splits,
            cudaStream_t st, const char* what) {
+  constexpr int kSmem = Ring<BMN, BSPLIT>::kSmemBytes;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return static_cast<int>(e); }
     attr_set = true;
   }
   const dim3 grid(static_cast<unsigned>(ceil_div<long long>(p.M, kBM)), kN / kBN, splits);
-  gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU><<<grid, kThreads, kSmemBytes, st>>>(ma, mb, mb2, p);
+  gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU><<<grid, kThreads, kSmem, st>>>(ma, mb, mb2, p);
   return check_launch(what);
 }
 
