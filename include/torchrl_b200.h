@@ -293,6 +293,11 @@ int trl_gemm3_pair(const float* A, const float* b_hi, const float* b_lo, float* 
 /* C (M x 256) = A (K x M)^T . B (K x 256), M % 256 == 0, deterministic split-K (the weight-gradient shape). */
 int trl_gemm3_pair_tn(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
                       float* workspace, void* stream);
+/* The same C bit for bit, with the split-K sum inside one launch (thread-block clusters of splits / 8 CTAs).
+ * 8 <= splits <= 64, splits % 8 == 0; workspace: 8*M*256 floats; tickets: M/8 int32, zero on entry and left zero,
+ * one set per stream. */
+int trl_gemm3_pair_tn_cluster(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
+                              float* workspace, int* tickets, void* stream);
 
 /* ---- "skinny" Linear layers of the small MLPs (first layer K = obs_dim, output layer N = act_dim / 1;
  * networks/base.py:24-44, networks/nets.py:13-52): memory-bound fp32 kernels, bias / activation fused. */

@@ -144,8 +144,9 @@ class A2C(OnRLAlgo):
     def _mb_body(self):
         """One minibatch update reading its row indices at device position `upd`.  Layer gradients go straight into
         the flat gradient buffer (networks.fused.direct_grad): every parameter gets exactly one contribution per
-        minibatch and the optimizer step left the buffer zeroed."""
-        with fused.direct_grad(), fused.deferred_reduces():
+        minibatch and the optimizer step left the buffer zeroed.  The dgrad GEMMs read transposed weight planes,
+        rewritten from the previous optimizer step's planes beside the gather and the forward passes."""
+        with fused.direct_grad(), fused.deferred_reduces(), fused.transposed_planes(self.opt):
             st, rb = self._mb_state, self.replay_buffer
             batch = rb.gather_rows(st["perm"], st["keys"], pos_ptr=st["upd"], rows=st["b"])
             batch["obs"] = self._prep_obs(batch["obs"])

@@ -6,7 +6,8 @@
 //   * B may be N-major (b_nmajor): the dgrad shape dX = G . W reads W (K x 256, row-major) directly -- no per-
 //     minibatch transpose of the weights;
 //   * tanh = 1 - 2/(exp(2x)+1) on the MUFU unit (abs err < 2.5e-7, same as csrc/skinny.cu);
-//   * split-K slabs are summed by an 8-way balanced tree (pair_splitk_reduce_kernel).
+//   * split-K slabs are summed by an 8-way balanced tree (pair_splitk_reduce_kernel), or, in the same order, inside
+//     the GEMM launch through thread-block clusters (trl_gemm3_pair_tn_cluster, the weight gradient's hot path).
 // Shapes:
 //   nt   : A (M x K) row-major, B (256 x K) row-major      forward  y = act(x W^T + b)
 //   nn   : A (M x K) row-major, B (K x 256) row-major      dgrad    dX = G W
@@ -111,4 +112,32 @@ TRL_API int trl_gemm3_pair_tn(const float* A, const float* B, float* C, int64_t 
   const long long mn = M * kN;
   pair::pair_splitk_reduce_kernel<<<static_cast<unsigned>(ceil_div<long long>(mn / 4, 64)), 512, 0, st>>>(workspace, C, mn, splits);
   return check_launch("pair_splitk_reduce_kernel");
+}
+
+// trl_gemm3_pair_tn with the split-K sum inside the one launch, bit for bit the same C: clusters of splits / 8 CTAs
+// add their slabs through distributed shared memory into 8 group partials, and the last CTA of each tile slice adds
+// those in pair_splitk_reduce_kernel's order.  8 <= splits <= 64, splits % 8 == 0; `workspace` holds 8*M*256 floats,
+// `tickets` M/8 int32 that are zero on entry and are left zero (one set per stream: concurrent calls must not share).
+TRL_API int trl_gemm3_pair_tn_cluster(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
+                                      float* workspace, int* tickets, void* stream) {
+  using namespace trl;
+  using namespace trl::wg;
+  TRL_REQUIRE(M >= kN && M % kN == 0 && K >= kBK, "trl_gemm3_pair_tn_cluster: bad sizes M=%lld K=%lld (M must be a multiple of 256)",
+              (long long)M, (long long)K);
+  TRL_REQUIRE(splits >= 8 && splits <= 64 && splits % 8 == 0,
+              "trl_gemm3_pair_tn_cluster: splits=%d must be a multiple of 8 in [8, 64]", splits);
+  TRL_REQUIRE(K % (static_cast<int64_t>(kBK) * splits) == 0,
+              "trl_gemm3_pair_tn_cluster: K=%lld must be a multiple of 32*splits", (long long)K);
+  TRL_REQUIRE(A && B && C && workspace && tickets, "trl_gemm3_pair_tn_cluster: null pointer");
+  TRL_REQUIRE(aligned16(A) && aligned16(B) && aligned16(C) && aligned16(workspace),
+              "trl_gemm3_pair_tn_cluster: pointers must be 16-byte aligned");
+  CUtensorMap ma, mb;
+  if (!make_map(&ma, A, static_cast<uint64_t>(K), static_cast<uint64_t>(M), Box::kMNMajorA) ||
+      !make_map(&mb, B, static_cast<uint64_t>(K), static_cast<uint64_t>(kN), Box::kMNMajor)) {
+    set_error("trl_gemm3_pair_tn_cluster: cuTensorMapEncodeTiled failed");
+    return TRL_EUNSUPPORTED;
+  }
+  Params p{nullptr, 0, C, M, static_cast<int>(K / kBK / splits), workspace, reinterpret_cast<unsigned*>(tickets)};
+  return launch<true, true, false, true, true>(ma, mb, mb, p, static_cast<unsigned>(splits),
+                                               static_cast<cudaStream_t>(stream), "gemm3_wgmma_kernel<tn,cluster>");
 }

@@ -24,12 +24,14 @@
 //                  for them and releases the stage to the producer.  The ring is 2-4 stages deep (as many as fit), so
 //                  TMA runs ahead of the MMAs and the two warpgroups drift against each other without a CTA barrier.
 //   epilogue                  accumulator fragments -> bias / activation -> global (float2 per thread, 32-byte rows).
+//   CLUSTER (split-K wgrad):  the splits are summed inside the launch instead (see the epilogue below).
 // Shapes (template flags):
 //   AMN = false: A (M x K) row-major;  AMN = true: A (K x M) row-major (reduction index = row index)
 //   BMN = false: B (256 x K) row-major; BMN = true: B (K x 256) row-major
 //   BSPLIT: B arrives as two pre-split planes (hi = tf32(w), lo = w - hi) and is only re-laid out, not split.
 #pragma once
 #include "common.cuh"
+#include "reduce.cuh"
 #include <cuda.h>
 
 namespace trl {
@@ -136,6 +138,30 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
 __device__ __forceinline__ void sts128(uint32_t addr, const float4 v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w));
 }
+// Thread-block cluster: this CTA's rank, the cluster's size, the split barrier (arrive releases this thread's shared
+// memory writes, wait acquires every thread's) and a 16-byte load from the same offset of rank r's shared memory.
+__device__ __forceinline__ uint32_t cluster_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_size() {
+  uint32_t n;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+  return n;
+}
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+__device__ __forceinline__ float4 ld_cluster128(uint32_t addr, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(addr), "r"(rank));
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "r"(remote)
+               : "memory");
+  return v;
+}
 __device__ __forceinline__ uint32_t tf32_bits(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
@@ -178,10 +204,22 @@ struct Params {
   float* __restrict__ C;           // (splits, M, 256) when splits > 1 else (M, 256)
   long long M;                     // output rows
   int k_blocks_per_split;          // K blocks (of 32) accumulated by one CTA
+  float* __restrict__ ws;          // CLUSTER: (8, M, 256) group partials
+  unsigned* tickets;               // CLUSTER: M / 8 arrival counters (8 row slices per 128 x 128 tile), zero on entry
 };
 
-// TANH_MUFU: tanh as tanh_ex2 (common.cuh, |abs err| < 2.5e-7) instead of libdevice tanhf
-template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU>
+// CLUSTER epilogue, shared memory: the CTA's 128 x 128 tile (acc + cor), rows padded so that a warp's float2 fragment
+// stores take 2 wavefronts.  It lives in the (then idle) ring.
+constexpr int kTileLd = kBN + 8;
+
+// TANH_MUFU: tanh as tanh_ex2 (common.cuh, |abs err| < 2.5e-7) instead of libdevice tanhf.
+// CLUSTER: split-K (splits = 8 c) summed inside the launch, in the order of pair_splitk_reduce_kernel (csrc/gemm_pair.cu:
+// group g = 0..7 adds splits g, g + 8, ... to 0 in turn, then the 8 group sums are combined as a balanced tree).
+// Launched in clusters of c CTAs along z; rank j of cluster g owns split g + 8 j.  After the main loop every CTA puts
+// its tile into its ring, rank j adds row slice j of the c tiles in rank order through distributed shared memory and
+// stores the group-g partial to p.ws; the last of the 8 CTAs holding slice j of a tile (last_cta) adds the 8 group
+// partials and writes C.  No bias / activation.
+template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU, bool CLUSTER = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                    const __grid_constant__ CUtensorMap map_b2, const Params p) {
@@ -196,7 +234,9 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
   uint64_t* conv = bars + 2 * S;                           // [S] B planes written -> both warpgroups (kConvertB)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_blk = blockIdx.x, n0 = blockIdx.y * kBN, split = blockIdx.z;
+  const int m_blk = blockIdx.x, n0 = blockIdx.y * kBN;
+  const int c_size = CLUSTER ? static_cast<int>(cluster_size()) : 1, c_rank = CLUSTER ? static_cast<int>(cluster_rank()) : 0;
+  const int split = CLUSTER ? static_cast<int>(blockIdx.z) / c_size + 8 * c_rank : static_cast<int>(blockIdx.z);
   const int nkb = p.k_blocks_per_split;
   const int kb0 = split * nkb;
 
@@ -238,6 +278,17 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
           if (BSPLIT) tma_load_2d(st + kBlo, &map_b2, &full[s], k0, n0);
         }
       }
+    }
+    if constexpr (CLUSTER) {
+      // the producer warps pass every CTA and cluster barrier of the consumers' epilogue (same order, see there):
+      // no thread of a cluster exits while a peer may still read its shared memory
+      __syncwarp();
+      __syncthreads();
+      cluster_arrive();
+      cluster_wait();
+      cluster_arrive();
+      last_cta(p.tickets + (m_blk * 2 + blockIdx.y) * 8 + c_rank, 8u);
+      cluster_wait();
     }
     return;
   }
@@ -320,6 +371,50 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
 
   // -------------------------------------------------------------------- epilogue
   // fragment i of this thread: rows r0 and r0 + 8, columns n0 + 8 (i / 4) + 2 (lane % 4) + {0, 1}
+  if constexpr (CLUSTER) {
+    __syncthreads();                                        // every warp is past its last MMA: the ring is idle
+    float* tile = reinterpret_cast<float*>(ring);
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(tile + (am + 8 * h) * kTileLd + j * 8 + 2 * tid) =
+            make_float2(acc[4 * j + 2 * h] + cor[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + cor[4 * j + 2 * h + 1]);
+    cluster_arrive();
+    cluster_wait();                                         // every tile of the cluster is in shared memory
+    // row slice c_rank (of c_size, as even as 128 rows allow), 32 float4 per row
+    const int r_lo = c_rank * kBM / c_size, n_vec = ((c_rank + 1) * kBM / c_size - r_lo) * (kBN / 4);
+    const long long slab = p.M * kN;
+    const uint32_t tile_u32 = smem_u32(tile);
+    for (int v = ct; v < n_vec; v += kConsumers) {
+      const int r = r_lo + v / (kBN / 4), q4 = v % (kBN / 4);
+      const uint32_t a = tile_u32 + static_cast<uint32_t>(r * kTileLd + 4 * q4) * 4u;
+      float4 x[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q)
+        if (q < c_size) x[q] = ld_cluster128(a, static_cast<uint32_t>(q));
+      float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int q = 0; q < 8; ++q)
+        if (q < c_size) { s.x += x[q].x; s.y += x[q].y; s.z += x[q].z; s.w += x[q].w; }
+      const long long o = (static_cast<long long>(m_blk) * kBM + r) * kN + n0 + 4 * q4;
+      *reinterpret_cast<float4*>(p.ws + (static_cast<long long>(blockIdx.z) / c_size) * slab + o) = s;
+    }
+    cluster_arrive();                                       // done with the peers' shared memory
+    if (last_cta(p.tickets + (m_blk * 2 + blockIdx.y) * 8 + c_rank, 8u)) {
+      for (int v = ct; v < n_vec; v += kConsumers) {
+        const long long o = (static_cast<long long>(m_blk) * kBM + r_lo + v / (kBN / 4)) * kN + n0 + 4 * (v % (kBN / 4));
+        float4 t[8];
+#pragma unroll
+        for (int g = 0; g < 8; ++g) t[g] = __ldcg(reinterpret_cast<const float4*>(p.ws + g * slab + o));
+#define TRL_T3(c) (((t[0].c + t[1].c) + (t[2].c + t[3].c)) + ((t[4].c + t[5].c) + (t[6].c + t[7].c)))
+        *reinterpret_cast<float4*>(p.C + o) = make_float4(TRL_T3(x), TRL_T3(y), TRL_T3(z), TRL_T3(w));
+#undef TRL_T3
+      }
+    }
+    cluster_wait();                                         // nobody in the cluster reads this CTA's tile any more
+    return;
+  }
   const long long r0 = static_cast<long long>(m_blk) * kBM + am;
   float* cbase = p.C + static_cast<long long>(split) * p.M * kN;
   const bool has_bias = p.bias != nullptr;
@@ -383,20 +478,38 @@ inline bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_
              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// grid: (ceil(M / 128), 2, splits); p.C is the split-K workspace when splits > 1
-template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU>
+// grid: (ceil(M / 128), 2, splits); p.C is the split-K workspace when splits > 1 (CLUSTER: clusters of splits / 8
+// CTAs along z, p.C the sum)
+template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU, bool CLUSTER = false>
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mb2, const Params& p, unsigned splits,
            cudaStream_t st, const char* what) {
   constexpr int kSmem = Ring<BMN, BSPLIT>::kSmemBytes;
+  auto kernel = gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU, CLUSTER>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return static_cast<int>(e); }
     attr_set = true;
   }
   const dim3 grid(static_cast<unsigned>(ceil_div<long long>(p.M, kBM)), kN / kBN, splits);
-  gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU><<<grid, kThreads, kSmem, st>>>(ma, mb, mb2, p);
+  if constexpr (CLUSTER) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = kSmem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 1;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = splits / 8;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, ma, mb, mb2, p);
+    if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return static_cast<int>(e); }
+  } else {
+    kernel<<<grid, kThreads, kSmem, st>>>(ma, mb, mb2, p);
+  }
   return check_launch(what);
 }
 

@@ -53,6 +53,11 @@ class FlatParams:
         # to a `networks.fused.presplit()` scope, looked up by the weight's address inside such a scope only.
         self.hi = torch.zeros(self.total, dtype=F32, device=self.device)
         self.lo = torch.zeros(self.total, dtype=F32, device=self.device)
+        # the same planes transposed, for the square 256 x 256 weights only: the dgrad GEMM reads them K-major, like the
+        # forward (written by refresh_transposed on entry to a `networks.fused.transposed_planes(flat)` scope)
+        self._square = [(p, o) for p, o in zip(self.params, self.offsets) if tuple(p.shape) == (256, 256)]
+        self.hi_t = torch.zeros(len(self._square), 256, 256, dtype=F32, device=self.device)
+        self.lo_t = torch.zeros(len(self._square), 256, 256, dtype=F32, device=self.device)
         if self.device.type == "cuda":
             from .networks import fused
             fused.register_flat(self)
@@ -65,6 +70,16 @@ class FlatParams:
                 n = p.numel()
                 out[p.data_ptr()] = (self.hi[o:o + n].view(p.shape), self.lo[o:o + n].view(p.shape))
         return out
+
+    def transposed_views(self):
+        """{weight address: (hi^T, lo^T)} for the square 256 x 256 weights."""
+        return {p.data_ptr(): (self.hi_t[i], self.lo_t[i]) for i, (p, _) in enumerate(self._square)}
+
+    def refresh_transposed(self):
+        """hi_t / lo_t <- the transposes of the current hi / lo planes of the square weights."""
+        for i, (_, o) in enumerate(self._square):
+            ops.transpose_f32(self.hi[o:o + 65536].view(256, 256), out=self.hi_t[i])
+            ops.transpose_f32(self.lo[o:o + 65536].view(256, 256), out=self.lo_t[i])
 
     def refresh_split(self):
         """Recompute both planes from `data` (one launch)."""

@@ -54,6 +54,8 @@ def set_gemm_impl(impl):
 _FLATS = weakref.WeakSet()       # live flat.FlatParams objects
 _PLANES = {}                     # weight address -> (hi, lo) views into the owning FlatParams' planes
 _PRESPLIT_DEPTH = 0
+_TRANSPOSED = None               # the open transposed_planes scope
+_T_STREAMS = {}
 
 
 def _drop_planes(ptrs):
@@ -104,6 +106,53 @@ def _planes_of(weight):
     return _PLANES.get(weight.data_ptr()) if _PRESPLIT_DEPTH > 0 else None
 
 
+class transposed_planes:
+    """Scope inside `presplit()` in which the dgrad GEMMs of the square 256 x 256 weights of the given flat parameter
+    buffers read transposed pre-split planes, i.e. K-major like the forward, instead of transposing the N-major weight
+    tile in shared memory on every K block (same products, same bits).  On entry the buffers rewrite their transposed
+    planes from their current hi / lo planes on a companion stream (under graph capture: a parallel branch); the first
+    dgrad on each stream waits for them, and the exit joins the companion stream.  These weights must not change inside
+    the scope before the last dgrad (the PPO / A2C minibatch body steps the optimizer after its backward passes)."""
+
+    def __init__(self, *flats):
+        self.flats = flats
+
+    def __enter__(self):
+        global _TRANSPOSED
+        self.prev, self.event, self.joined, self.table = _TRANSPOSED, None, set(), {}
+        if _PRESPLIT_DEPTH > 0 and _MATMUL_MODE == "tc3" and _GEMM_IMPL == "pair":
+            self.main = torch.cuda.current_stream()
+            key = self.main.cuda_stream
+            if key not in _T_STREAMS:
+                _T_STREAMS[key] = torch.cuda.Stream(device=self.main.device)
+            self.side = _T_STREAMS[key]
+            self.side.wait_stream(self.main)
+            with torch.cuda.stream(self.side):
+                for f in self.flats:
+                    f.refresh_transposed()
+                    self.table.update(f.transposed_views())
+            self.event = torch.cuda.Event()
+            self.event.record(self.side)
+        _TRANSPOSED = self
+        return self
+
+    def __exit__(self, *a):
+        global _TRANSPOSED
+        _TRANSPOSED = self.prev
+        if self.event is not None:
+            self.main.wait_stream(self.side)
+
+    def planes(self, weight):
+        """(hi^T, lo^T) of `weight`, ready on the current stream, or None."""
+        pl = self.table.get(weight.data_ptr()) if _PRESPLIT_DEPTH > 0 else None
+        if pl is not None:
+            st = torch.cuda.current_stream()
+            if st.cuda_stream not in self.joined:
+                st.wait_event(self.event)
+                self.joined.add(st.cuda_stream)
+        return pl
+
+
 def mm_fwd(x, weight, bias=None, act=0):
     """act(x (M,K) @ weight (256,K)^T + bias) on the tensor cores."""
     if _GEMM_IMPL == "pair":
@@ -112,8 +161,12 @@ def mm_fwd(x, weight, bias=None, act=0):
 
 
 def mm_dgrad(gz, weight):
-    """gz (M,256) @ weight (256,256): the weights are read N-major by the pair kernel (no transpose)."""
+    """gz (M,256) @ weight (256,256): inside `transposed_planes()` from the weight's transposed pre-split planes
+    (K-major, the forward's route), elsewhere the pair kernel reads the weights N-major (no transpose)."""
     if _GEMM_IMPL == "pair":
+        planes_t = _TRANSPOSED.planes(weight) if _TRANSPOSED is not None else None
+        if planes_t is not None:
+            return ops.gemm3_pair(gz, weight, planes=planes_t)
         return ops.gemm3_pair(gz, weight, planes=_planes_of(weight), b_nmajor=True)
     return ops.gemm_tf32x3_nt(gz, ops.transpose_f32(weight))
 
@@ -155,12 +208,17 @@ def wgrad(gz, x, out=None):
     K = x.shape[1]
     if _tc3_ok(M, K, M) and H % 128 == 0 and M % (32 * 64) == 0:
         # wgmma 3xTF32, operands consumed M/N-major from their row-major storage, deterministic split-K
-        key = (H, str(gz.device), _stream_key())
+        pair = _GEMM_IMPL == "pair" and H % 256 == 0
+        key = (H, pair, str(gz.device), _stream_key())
         ws = _WGRAD_WS.get(key)
+        if pair:
+            # split-K summed inside the launch (8 group partials + arrival tickets instead of 64 slabs)
+            if ws is None:
+                ws = _WGRAD_WS[key] = (torch.empty(8 * H * 256, dtype=torch.float32, device=gz.device),
+                                       torch.zeros(H // 8, dtype=torch.int32, device=gz.device))
+            return ops.gemm3_pair_tn_cluster(gz, x, *ws, out=out, splits=64)
         if ws is None:
             ws = _WGRAD_WS[key] = torch.empty(64 * H * 256, dtype=torch.float32, device=gz.device)
-        if _GEMM_IMPL == "pair" and H % 256 == 0:
-            return ops.gemm3_pair_tn(gz, x, out=out, splits=64, workspace=ws)
         return ops.gemm_tf32x3_tn(gz, x, out=out, splits=64, workspace=ws)
     if (_MATMUL_MODE != "fp32" and K <= 24 and H % 32 == 0 and H <= 256 and _skinny_ok(gz)
             and (out is None or out.is_contiguous())):

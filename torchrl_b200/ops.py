@@ -550,6 +550,19 @@ def gemm3_pair_tn(a, b, out=None, splits=1, workspace=None):
     return out
 
 
+def gemm3_pair_tn_cluster(a, b, workspace, tickets, out=None, splits=64):
+    """gemm3_pair_tn's result bit for bit in one launch: the split-K sum runs through thread-block clusters.
+    workspace: 8*M*256 floats; tickets: M // 8 zeroed int32 (left zero), one set per stream."""
+    K, M = a.shape
+    assert b.shape == (K, 256), "B must be (K, 256)"
+    assert workspace.numel() >= 8 * M * 256 and tickets.numel() >= M // 8, "workspace / tickets too small"
+    if out is None:
+        out = torch.empty(M, 256, dtype=F32, device=a.device)
+    _lib.call("trl_gemm3_pair_tn_cluster", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K,
+              int(splits), _chk(workspace, F32, "workspace"), _chk(tickets, torch.int32, "tickets"), _stream())
+    return out
+
+
 def transpose_f32(x, out=None):
     """out (C,R) = x (R,C)^T (contiguous)."""
     R, C = x.shape
