@@ -298,6 +298,13 @@ int trl_gemm3_pair_tn(const float* A, const float* B, float* C, int64_t M, int64
  * one set per stream. */
 int trl_gemm3_pair_tn_cluster(const float* A, const float* B, float* C, int64_t M, int64_t K, int splits,
                               float* workspace, int* tickets, void* stream);
+/* The dgrad dH1 = G (M x 256) . W2 of an MLP's second hidden layer with the first layer's backward as its epilogue:
+ * writes the slab partials of trl_skinny_act_wgrad_partial(dH1, Y, X, M, 256, K, act, scratch) bit for bit, dH1 itself
+ * is never stored.  (w_hi_t, w_lo_t): the transposed pre-split planes of W2 (256 x 256, hi^T and lo^T); Y: h1 (M x 256);
+ * X: the first layer's input (M x K).  scratch: trl_skinny_tn_scratch_floats(M, 256, K) floats, summed by
+ * trl_skinny_reduce_jobs (kind 1).  1 <= M <= 16896, 1 <= K <= 24; G, W, Y and scratch 16-byte aligned. */
+int trl_gemm3_pair_dgrad_act_wgrad(const float* G, const float* w_hi_t, const float* w_lo_t, const float* Y,
+                                   const float* X, int64_t M, int K, int act, float* scratch, void* stream);
 
 /* ---- "skinny" Linear layers of the small MLPs (first layer K = obs_dim, output layer N = act_dim / 1;
  * networks/base.py:24-44, networks/nets.py:13-52): memory-bound fp32 kernels, bias / activation fused. */

@@ -12,7 +12,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CASES = ("nt", "nt_split", "nn", "nn_split", "tn", "time")
+CASES = ("nt", "nt_split", "nn", "nn_split", "tn", "time", "dgrad_first")
 
 
 def timeit(fn, n=50):
@@ -96,6 +96,38 @@ def run_case(name):
         t2 = timeit(lambda: ops.gemm_tf32x3_tn(g, x, splits=64, workspace=ws))
         t3 = timeit(lambda: torch.mm(g.t(), x))
         print("wgrad 256x256, K=16384, 64 splits (incl. reduce): pair %.1f us  single %.1f us  cublas %.1f us" % (t1, t2, t3),
+              flush=True)
+    elif name == "dgrad_first":
+        # the dgrad dH1 = gz2 W2 with the first layer's backward in its epilogue, against the dgrad (transposed
+        # pre-split planes) followed by trl_skinny_act_wgrad_partial: same slab partials, one launch instead of two
+        from torchrl_b200 import _lib
+        M, K = 16384, 17
+        gz = torch.randn(M, 256, device=dev)
+        w = torch.randn(256, 256, device=dev) / 16
+        hi, lo = planes(w)
+        plt = (hi.t().contiguous(), lo.t().contiguous())
+        h1 = torch.tanh(torch.randn(M, 256, device=dev))
+        x = torch.randn(M, K, device=dev)
+        n = int(_lib.load().trl_skinny_tn_scratch_floats(M, 256, K))
+        ws_f, ws_u = torch.empty(n, device=dev), torch.empty(n, device=dev)
+        dh1 = torch.empty(M, 256, device=dev)
+
+        def unfused():
+            ops.gemm3_pair(gz, w, out=dh1, planes=plt)
+            _lib.call("trl_skinny_act_wgrad_partial", dh1.data_ptr(), h1.data_ptr(), x.data_ptr(), M, 256, K, 1,
+                      ws_u.data_ptr(), ops._stream())
+
+        def fused_():
+            ops.gemm3_pair_dgrad_act_wgrad(gz, plt, h1, x, 1, ws_f)
+
+        unfused()
+        fused_()
+        torch.cuda.synchronize()
+        assert torch.equal(ws_f.view(torch.int32), ws_u.view(torch.int32)), "slab partials differ"
+        t_d = timeit(lambda: ops.gemm3_pair(gz, w, out=dh1, planes=plt))
+        t_u = timeit(unfused)
+        t_f = timeit(fused_)
+        print("M=%d K=%d: dgrad %.1f us, dgrad + act_wgrad %.1f us, fused %.1f us (50 calls each)" % (M, K, t_d, t_u, t_f),
               flush=True)
     else:
         raise SystemExit("unknown case " + name)

@@ -90,6 +90,7 @@ SIGNATURES = {
     "trl_gemm3_pair": [vp, vp, vp, vp, i64, i64, i32, vp, i32, vp],
     "trl_gemm3_pair_tn": [vp, vp, vp, i64, i64, i32, vp, vp],
     "trl_gemm3_pair_tn_cluster": [vp, vp, vp, i64, i64, i32, vp, vp, vp],
+    "trl_gemm3_pair_dgrad_act_wgrad": [vp, vp, vp, vp, vp, i64, i32, i32, vp, vp],
     "trl_skinny_k_fwd": [vp, vp, vp, vp, i64, i32, i32, i32, vp],
     "trl_skinny_tn_scratch_floats": [i64, i32, i32],
     "trl_skinny_tn": [vp, vp, vp, vp, i64, i32, i32, i32, vp, vp],

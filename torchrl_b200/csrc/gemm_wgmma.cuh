@@ -25,6 +25,8 @@
 //                  TMA runs ahead of the MMAs and the two warpgroups drift against each other without a CTA barrier.
 //   epilogue                  accumulator fragments -> bias / activation -> global (float2 per thread, 32-byte rows).
 //   CLUSTER (split-K wgrad):  the splits are summed inside the launch instead (see the epilogue below).
+//   XK > 0 (dgrad dH1 = gz2 W2 of a first layer with XK inputs): dH1 is never stored; the epilogue reduces it to the
+//                             first layer's weight / bias gradient slab partials (see there).
 // Shapes (template flags):
 //   AMN = false: A (M x K) row-major;  AMN = true: A (K x M) row-major (reduction index = row index)
 //   BMN = false: B (256 x K) row-major; BMN = true: B (K x 256) row-major
@@ -32,6 +34,7 @@
 #pragma once
 #include "common.cuh"
 #include "reduce.cuh"
+#include "skinny_common.cuh"
 #include <cuda.h>
 
 namespace trl {
@@ -46,12 +49,16 @@ constexpr int kThreads = kConsumers + 128;                // + producer warpgrou
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 
 // Ring stage: A | B hi | B lo [| raw N-major B | raw N-major B lo plane].  The stage count fills ~200 KB.
-template <bool BMN, bool BSPLIT>
+// XK > 0: a 128 x 128 tile of the first layer's activations h1 and the CTA's rows of its input x ([128][KP]) follow the
+// ring, and the ring gives up its fourth stage for them (227 KB in all; the dgrad has only 8 K blocks).
+template <bool BMN, bool BSPLIT, int XK = 0>
 struct Ring {
   static constexpr int kTiles = 3 + (BMN ? (BSPLIT ? 2 : 1) : 0);
   static constexpr int kStageBytes = kTiles * kTileBytes;
-  static constexpr int kStages = (200 * 1024) / kStageBytes < 4 ? (200 * 1024) / kStageBytes : 4;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 128 /*barriers*/;
+  static constexpr int kYBytes = XK ? kBM * kBN * 4 : 0;
+  static constexpr int kXBytes = XK ? kBM * ((XK + 3) & ~3) * 4 : 0;
+  static constexpr int kStages = XK ? 3 : ((200 * 1024) / kStageBytes < 4 ? (200 * 1024) / kStageBytes : 4);
+  static constexpr int kSmemBytes = kStages * kStageBytes + kYBytes + kXBytes + 1024 /*align*/ + 128 /*barriers*/;
   static constexpr bool kConvertB = BMN || !BSPLIT;       // the consumers write the B planes
   static_assert(kStages >= 2 && kSmemBytes <= 227 * 1024, "fits one sm_90 CTA");
 };
@@ -206,11 +213,17 @@ struct Params {
   int k_blocks_per_split;          // K blocks (of 32) accumulated by one CTA
   float* __restrict__ ws;          // CLUSTER: (8, M, 256) group partials
   unsigned* tickets;               // CLUSTER: M / 8 arrival counters (8 row slices per 128 x 128 tile), zero on entry
+  const float* __restrict__ X;     // XK: the first layer's input (M, XK)
+  int wg_rows;                     // XK: rows per consumer warpgroup, a whole number of slabs (<= 64)
+  int slab_rows;                   // XK: rows per slab, sk_rows_per_cta(M)
 };
 
 // CLUSTER epilogue, shared memory: the CTA's 128 x 128 tile (acc + cor), rows padded so that a warp's float2 fragment
 // stores take 2 wavefronts.  It lives in the (then idle) ring.
 constexpr int kTileLd = kBN + 8;
+
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // TANH_MUFU: tanh as tanh_ex2 (common.cuh, |abs err| < 2.5e-7) instead of libdevice tanhf.
 // CLUSTER: split-K (splits = 8 c) summed inside the launch, in the order of pair_splitk_reduce_kernel (csrc/gemm_pair.cu:
@@ -219,19 +232,31 @@ constexpr int kTileLd = kBN + 8;
 // its tile into its ring, rank j adds row slice j of the c tiles in rank order through distributed shared memory and
 // stores the group-g partial to p.ws; the last of the 8 CTAs holding slice j of a tile (last_cta) adds the 8 group
 // partials and writes C.  No bias / activation.
-template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU, bool CLUSTER = false>
+// XK > 0: the dgrad dH1 = gz2 W2 (K-major pre-split planes) of an MLP whose first layer h1 = act(x W1^T + b1) has XK
+// inputs; instead of dH1 the launch writes the slab partials of skinny_tn_kernel<XK, true> (csrc/skinny.cu) for
+// dW1 = (dH1 * act'(h1))^T x and db1, bit for bit.  The tile rows follow the slabs (sk_rows_per_cta rows each): each
+// warpgroup owns p.wg_rows rows, a whole number of slabs, so a CTA covers 2 p.wg_rows <= 128 rows (the rows of its
+// m64 MMAs past p.wg_rows are computed and dropped).  The producer warpgroup TMA-loads the tile's h1 rows (map_y) and
+// stages the tile's x rows while the main loop runs; after the last MMA the tile goes into the idle ring and each
+// warpgroup re-reads it in the skinny kernel's row-lane order (skinny_common.cuh).  No bias / activation.
+template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU, bool CLUSTER = false, int XK = 0>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                   const __grid_constant__ CUtensorMap map_b2, const Params p) {
-  using R = Ring<BMN, BSPLIT>;
+                   const __grid_constant__ CUtensorMap map_b2, const __grid_constant__ CUtensorMap map_y, const Params p) {
+  static_assert(XK == 0 || (!AMN && !BMN && BSPLIT && !CLUSTER), "the first-layer epilogue is a K-major pre-split dgrad");
+  using R = Ring<BMN, BSPLIT, XK>;
+  constexpr int XKP = (XK + 3) & ~3;
   constexpr int S = R::kStages;
   constexpr int kA = 0, kBhi = kTileBytes, kBlo = 2 * kTileBytes, kBraw = 3 * kTileBytes, kBraw2 = 4 * kTileBytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + S * R::kStageBytes);
+  float* ytile = reinterpret_cast<float*>(ring + S * R::kStageBytes);   // XK: [128][128] h1 rows
+  float* xs = reinterpret_cast<float*>(ring + S * R::kStageBytes + R::kYBytes);   // XK: [128][XKP] x rows
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + S * R::kStageBytes + R::kYBytes + R::kXBytes);
   uint64_t* full = bars;                                   // [S] TMA -> consumers
   uint64_t* empty = bars + S;                              // [S] consumers' MMAs done -> TMA
   uint64_t* conv = bars + 2 * S;                           // [S] B planes written -> both warpgroups (kConvertB)
+  uint64_t* ybar = bars + 3 * S;                           // XK: h1 tile landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blk = blockIdx.x, n0 = blockIdx.y * kBN;
@@ -239,6 +264,7 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
   const int split = CLUSTER ? static_cast<int>(blockIdx.z) / c_size + 8 * c_rank : static_cast<int>(blockIdx.z);
   const int nkb = p.k_blocks_per_split;
   const int kb0 = split * nkb;
+  const int m_row0 = XK ? m_blk * 2 * p.wg_rows : m_blk * kBM;   // first row of the A box
 
   if (threadIdx.x == kConsumers) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
@@ -249,6 +275,7 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
       mbar_init(&empty[s], kConsumers / 32);               // one arrival per consumer warp
       mbar_init(&conv[s], kConsumers / 32);
     }
+    if (XK) mbar_init(ybar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -268,7 +295,7 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
 #pragma unroll
           for (int j = 0; j < 4; ++j) tma_load_2d(st + kA + j * 4096, &map_a, &full[s], m_blk * kBM + 32 * j, k0);
         } else {
-          tma_load_2d(st + kA, &map_a, &full[s], k0, m_blk * kBM);
+          tma_load_2d(st + kA, &map_a, &full[s], k0, m_row0);
         }
         if (BMN) {
           tma_load_2d(st + kBraw, &map_b, &full[s], n0, k0);
@@ -277,6 +304,19 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
           tma_load_2d(st + kBhi, &map_b, &full[s], k0, n0);
           if (BSPLIT) tma_load_2d(st + kBlo, &map_b2, &full[s], k0, n0);
         }
+        if (XK && kb == (nkb < S ? nkb : S) - 1) {       // behind the ring's first fill: the h1 rows of the tile
+          mbar_arrive_expect_tx(ybar, R::kYBytes);
+          tma_load_2d(ytile, &map_y, ybar, n0, m_row0);
+        }
+      }
+    }
+    if constexpr (XK > 0) {
+      // warps 9..11 stage the tile's x rows for the epilogue, then signal the consumers (named barrier 1)
+      if (warp > kConsumers / 32) {
+        const long long nx = p.M - m_row0;
+        stage_rows<XK>(xs, p.X, m_row0, static_cast<int>(nx < 2 * p.wg_rows ? nx : 2 * p.wg_rows),
+                       threadIdx.x - kConsumers - 32, 96);
+        named_arrive(1, kConsumers + 96);
       }
     }
     if constexpr (CLUSTER) {
@@ -297,7 +337,7 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
   const int ct = threadIdx.x, wgi = warp >> 2, wl = warp & 3;
   const int gid = lane >> 2, tid = lane & 3;
-  const int am = wgi * 64 + wl * 16 + gid;                 // this thread's fragment rows: am, am + 8
+  const int am = (XK ? wgi * p.wg_rows : wgi * 64) + wl * 16 + gid;   // this thread's fragment rows: am, am + 8
   float acc[64], cor[64];                                  // hi*hi | lo*hi + hi*lo
 #pragma unroll
   for (int i = 0; i < 64; ++i) { acc[i] = 0.f; cor[i] = 0.f; }
@@ -371,6 +411,45 @@ gemm3_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_const
 
   // -------------------------------------------------------------------- epilogue
   // fragment i of this thread: rows r0 and r0 + 8, columns n0 + 8 (i / 4) + 2 (lane % 4) + {0, 1}
+  if constexpr (XK > 0) {
+    named_sync(2, kConsumers);                              // every consumer warp is past its last MMA: the ring is idle
+    // the warpgroup's 64 fragment rows (acc + cor: the value the plain dgrad stores) at rows 64 wgi + 0..63
+    float* tile = reinterpret_cast<float*>(ring);
+    const int lr = wgi * 64 + wl * 16 + gid;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        *reinterpret_cast<float2*>(tile + (lr + 8 * h) * kTileLd + j * 8 + 2 * tid) =
+            make_float2(acc[4 * j + 2 * h] + cor[4 * j + 2 * h], acc[4 * j + 2 * h + 1] + cor[4 * j + 2 * h + 1]);
+    named_sync(1, kConsumers + 96);                         // the tile and the x rows are in shared memory
+    mbar_wait(ybar, 0);                                     // so are the h1 rows
+    // skinny_tn_kernel's layout over the warpgroup's 128 columns: warp wl owns 32, lane = (row lane, column quad)
+    const int rl = lane >> 3, cc = wl * 32 + (lane & 7) * 4;
+    const int spw = p.wg_rows / p.slab_rows;
+    const uint32_t g_u32 = smem_u32(tile + (wgi * 64) * kTileLd + cc), y_u32 = smem_u32(ytile + cc);
+    for (int sl = 0; sl < spw; ++sl) {
+      const long long slab = static_cast<long long>(m_blk * 2 + wgi) * spw + sl;
+      const long long row0 = slab * p.slab_rows;
+      if (row0 >= p.M) break;
+      const int nrows = static_cast<int>(p.M - row0 < p.slab_rows ? p.M - row0 : p.slab_rows);
+      const int gr0 = sl * p.slab_rows, br0 = wgi * p.wg_rows + sl * p.slab_rows;   // slab row 0 in the tile / box
+      float wacc[XKP][4];
+#pragma unroll
+      for (int k = 0; k < XKP; ++k)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) wacc[k][j] = 0.f;
+      float4 asum = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 2
+      for (int r = rl; r < nrows; r += 4) {
+        const float4 g = lds128(g_u32 + static_cast<uint32_t>((gr0 + r) * kTileLd) * 4u);
+        const float4 y = lds128(y_u32 + static_cast<uint32_t>((br0 + r) * kBN) * 4u);
+        act_wgrad_row<XK>(wacc, asum, g, y, xs + (br0 + r) * XKP, p.act);
+      }
+      act_wgrad_store<XK>(p.ws + slab * (XK + 1) * kN, wacc, asum, kN, n0 + cc, rl);
+    }
+    return;
+  }
   if constexpr (CLUSTER) {
     __syncthreads();                                        // every warp is past its last MMA: the ring is idle
     float* tile = reinterpret_cast<float*>(ring);
@@ -461,7 +540,8 @@ inline PFN_encodeTiled get_encode() {
 //   kKMajor  : reduction index = column.  One 32 x 128 box, SWIZZLE_128B (the wgmma K-major layout).
 //   kMNMajor : reduction index = row.  One 128 x 32 box, no swizzle (transposed by the consumers).
 //   kMNMajorA: reduction index = row.  32 x 32 boxes (four per tile), SWIZZLE_128B (the register-A fragment loads).
-enum class Box { kKMajor, kMNMajor, kMNMajorA };
+//   kTile    : a whole 128 x 128 output tile, no swizzle (XK: the h1 rows read by the epilogue).
+enum class Box { kKMajor, kMNMajor, kMNMajorA, kTile };
 
 // (rows x cols) fp32 row-major operand.  Out-of-range rows are filled with zeros (ragged M).
 inline bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_t cols, Box box_kind) {
@@ -469,29 +549,31 @@ inline bool make_map(CUtensorMap* map, const float* base, uint64_t rows, uint64_
   if (!enc) return false;
   const cuuint64_t gdim[2] = {cols, rows};
   const cuuint64_t gstride[1] = {cols * sizeof(float)};
-  const cuuint32_t inner = box_kind == Box::kMNMajor ? 128 : kBK;
-  const cuuint32_t box[2] = {inner, static_cast<cuuint32_t>(box_kind == Box::kKMajor ? 128 : kBK)};
+  const bool plain = box_kind == Box::kMNMajor || box_kind == Box::kTile;
+  const cuuint32_t inner = plain ? 128 : kBK;
+  const cuuint32_t box[2] = {inner, static_cast<cuuint32_t>(box_kind == Box::kKMajor || box_kind == Box::kTile ? 128 : kBK)};
   const cuuint32_t estr[2] = {1, 1};
   return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE,
-             box_kind == Box::kMNMajor ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
+             plain ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B,
              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// grid: (ceil(M / 128), 2, splits); p.C is the split-K workspace when splits > 1 (CLUSTER: clusters of splits / 8
+// grid: (ceil(M / 128), 2, splits) (XK: ceil(M / (2 p.wg_rows)) row blocks); p.C is the split-K workspace when splits > 1 (CLUSTER: clusters of splits / 8
 // CTAs along z, p.C the sum)
-template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU, bool CLUSTER = false>
+template <bool AMN, bool BMN, bool BSPLIT, bool TANH_MUFU, bool CLUSTER = false, int XK = 0>
 int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mb2, const Params& p, unsigned splits,
-           cudaStream_t st, const char* what) {
-  constexpr int kSmem = Ring<BMN, BSPLIT>::kSmemBytes;
-  auto kernel = gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU, CLUSTER>;
+           cudaStream_t st, const char* what, const CUtensorMap* my = nullptr) {
+  constexpr int kSmem = Ring<BMN, BSPLIT, XK>::kSmemBytes;
+  auto kernel = gemm3_wgmma_kernel<AMN, BMN, BSPLIT, TANH_MUFU, CLUSTER, XK>;
+  const CUtensorMap& mys = my ? *my : mb2;                  // map_y is read by the XK instances only
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return static_cast<int>(e); }
     attr_set = true;
   }
-  const dim3 grid(static_cast<unsigned>(ceil_div<long long>(p.M, kBM)), kN / kBN, splits);
+  const dim3 grid(static_cast<unsigned>(ceil_div<long long>(p.M, XK ? 2 * p.wg_rows : kBM)), kN / kBN, splits);
   if constexpr (CLUSTER) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
@@ -505,10 +587,10 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mb2,
     attr[0].val.clusterDim.z = splits / 8;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, ma, mb, mb2, p);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, ma, mb, mb2, mys, p);
     if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return static_cast<int>(e); }
   } else {
-    kernel<<<grid, kThreads, kSmem, st>>>(ma, mb, mb2, p);
+    kernel<<<grid, kThreads, kSmem, st>>>(ma, mb, mb2, mys, p);
   }
   return check_launch(what);
 }

@@ -16,12 +16,9 @@
 //   skinny_act_wgrad   : dW1 = (G * act'(Y))^T X,  db1 = colsum(G * act'(Y))    (first layer: gz never stored)
 //   skinny_n_dgrad_act : gz = (G . W) * act'(Y),  db = colsum(gz)               (output-layer dgrad + act backward)
 // Reductions have a fixed combination order (deterministic, run-to-run bit-identical).
-#include "common.cuh"
+#include "skinny_common.cuh"
 
 namespace trl {
-
-constexpr int kSkMaxRows = 128;      // rows of the skinny operand staged per CTA (<= 12 KB of shared memory)
-constexpr int kSkCtas = 2 * kNumSM;  // target grid: two resident CTAs per SM
 
 __device__ __forceinline__ float sk_tanh(float x) { return tanh_ex2(x); }   // common.cuh: 2 MUFU ops, abs err < 2.5e-7
 
@@ -30,43 +27,6 @@ __device__ __forceinline__ float4 sk_act4(float4 v, int act) {
   if (act == 1) return make_float4(sk_tanh(v.x), sk_tanh(v.y), sk_tanh(v.z), sk_tanh(v.w));
   if (act == 2) return make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f));
   return v;
-}
-
-// g * act'(.) with the derivative expressed through the activation's OUTPUT y (same convention as mlp_epilogue.cu)
-__device__ __forceinline__ float4 sk_dact4(float4 g, float4 y, int act) {
-  if (act == 1)
-    return make_float4(g.x * fmaf(-y.x, y.x, 1.f), g.y * fmaf(-y.y, y.y, 1.f), g.z * fmaf(-y.z, y.z, 1.f),
-                       g.w * fmaf(-y.w, y.w, 1.f));
-  if (act == 2) return make_float4(y.x > 0.f ? g.x : 0.f, y.y > 0.f ? g.y : 0.f, y.z > 0.f ? g.z : 0.f, y.w > 0.f ? g.w : 0.f);
-  return g;
-}
-
-static inline int sk_rows_per_cta(long long M) {
-  long long r = ceil_div<long long>(M, kSkCtas);
-  if (r < 8) r = 8;
-  if (r > kSkMaxRows) r = kSkMaxRows;
-  return static_cast<int>(r);
-}
-
-// stage rows [row0, row0+nrows) of a row-major (M x K) matrix into shared memory as [nrows][KP], zero padded.  The slab
-// is one contiguous run of nrows*K floats: it is read as such (fully coalesced); K is a compile-time constant, so the
-// (row, column) split is a multiply-shift, not a division.
-template <int K>
-__device__ __forceinline__ void stage_rows(float* __restrict__ dst, const float* __restrict__ src, long long row0,
-                                           int nrows, int tid, int nthr) {
-  constexpr int KP = (K + 3) & ~3;
-  const float* base = src + row0 * K;
-  for (int j = tid; j < nrows * K; j += nthr) {
-    const int r = j / K, k = j - r * K;
-    dst[r * KP + k] = __ldg(base + j);
-  }
-  if (KP != K) {
-    constexpr int PAD = KP - K > 0 ? KP - K : 1;
-    for (int j = tid; j < nrows * PAD; j += nthr) {
-      const int r = j / PAD, k = K + (j - r * PAD);
-      dst[r * KP + k] = 0.f;
-    }
-  }
 }
 
 // run-time K (the <= 8 wide output-layer gradient): [nrows][KP], zero padded
@@ -151,23 +111,6 @@ __global__ void __launch_bounds__(256, 2) skinny_k_fwd_kernel(const float* __res
 // before the first is used (U 16-byte loads in flight per thread, 2U with the fused activation gradient).  After the
 // slab: butterfly over the 4 row lanes, then the CTA writes its partial k-major ([K+1][H], row K = column sums of B);
 // skinny_tn_reduce sums the CTAs in a fixed order.
-template <int K>
-__device__ __forceinline__ void tn_fma_row(float (&acc)[(K + 3) & ~3][4], const float4 a, const float* __restrict__ brow) {
-  constexpr int KP = (K + 3) & ~3;
-  const float av[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-  for (int q = 0; q < KP / 4; ++q) {
-    const float4 b = reinterpret_cast<const float4*>(brow)[q];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (4 * q < K) acc[4 * q][j] = fmaf(av[j], b.x, acc[4 * q][j]);
-      if (4 * q + 1 < K) acc[4 * q + 1][j] = fmaf(av[j], b.y, acc[4 * q + 1][j]);
-      if (4 * q + 2 < K) acc[4 * q + 2][j] = fmaf(av[j], b.z, acc[4 * q + 2][j]);
-      if (4 * q + 3 < K) acc[4 * q + 3][j] = fmaf(av[j], b.w, acc[4 * q + 3][j]);
-    }
-  }
-}
-
 // ACT = true: A is not read but formed on the fly as G * act'(Yact) (first-layer backward: the activation
 // gradient is never written to memory) and row K of the partial receives the column sums of A (the bias gradient).
 template <int K, bool ACT>
@@ -205,47 +148,25 @@ __global__ void __launch_bounds__(256, 2) skinny_tn_kernel(const float* __restri
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      float4 a0 = g[u];
-      if (ACT) {
-        a0 = sk_dact4(a0, y[u], act);
-        asum.x += a0.x; asum.y += a0.y; asum.z += a0.z; asum.w += a0.w;
-      }
-      tn_fma_row<K>(acc, a0, sk_smem + (r + 4 * u) * KP);
+      if (ACT) act_wgrad_row<K>(acc, asum, g[u], y[u], sk_smem + (r + 4 * u) * KP, act);
+      else tn_fma_row<K>(acc, g[u], sk_smem + (r + 4 * u) * KP);
     }
   }
   for (; r < nrows; r += 4) {
-    float4 a0 = __ldg(reinterpret_cast<const float4*>(ap + static_cast<long long>(r) * H));
-    if (ACT) {
-      a0 = sk_dact4(a0, __ldg(reinterpret_cast<const float4*>(yp + static_cast<long long>(r) * H)), act);
-      asum.x += a0.x; asum.y += a0.y; asum.z += a0.z; asum.w += a0.w;
-    }
-    tn_fma_row<K>(acc, a0, sk_smem + r * KP);
+    const float4 a0 = __ldg(reinterpret_cast<const float4*>(ap + static_cast<long long>(r) * H));
+    if (ACT) act_wgrad_row<K>(acc, asum, a0, __ldg(reinterpret_cast<const float4*>(yp + static_cast<long long>(r) * H)),
+                              sk_smem + r * KP, act);
+    else tn_fma_row<K>(acc, a0, sk_smem + r * KP);
   }
-  // combine the 4 row lanes (lanes l, l^8, l^16, l^24 hold the same columns): fixed order
-#pragma unroll
-  for (int k = 0; k < K; ++k)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float v = acc[k][j];
-      v += __shfl_xor_sync(0xffffffffu, v, 8);
-      v += __shfl_xor_sync(0xffffffffu, v, 16);
-      acc[k][j] = v;
-    }
-  // partial layout per CTA: [K + 1][H] (k-major); row lane (k & 3) stores column-quad k
+  // partial layout per CTA: [K + 1][H] (k-major), after the fixed-order combine of the 4 row lanes (skinny_common.cuh)
   float* pp = partial + static_cast<long long>(blockIdx.x) * (K + 1) * H;
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    if ((k & 3) == rl)
-      *reinterpret_cast<float4*>(pp + static_cast<long long>(k) * H + c0) =
-          make_float4(acc[k][0], acc[k][1], acc[k][2], acc[k][3]);
-  }
   if (ACT) {
-    asum.x += __shfl_xor_sync(0xffffffffu, asum.x, 8); asum.x += __shfl_xor_sync(0xffffffffu, asum.x, 16);
-    asum.y += __shfl_xor_sync(0xffffffffu, asum.y, 8); asum.y += __shfl_xor_sync(0xffffffffu, asum.y, 16);
-    asum.z += __shfl_xor_sync(0xffffffffu, asum.z, 8); asum.z += __shfl_xor_sync(0xffffffffu, asum.z, 16);
-    asum.w += __shfl_xor_sync(0xffffffffu, asum.w, 8); asum.w += __shfl_xor_sync(0xffffffffu, asum.w, 16);
-    if (rl == (K & 3)) *reinterpret_cast<float4*>(pp + static_cast<long long>(K) * H + c0) = asum;
-  } else if (tid < K) {
+    act_wgrad_store<K>(pp, acc, asum, H, c0, rl);
+  } else {
+    tn_combine_lanes<K>(acc);
+    tn_store_rows<K>(pp, acc, H, c0, rl);
+  }
+  if (!ACT && tid < K) {
     float s = 0.f;
     if (want_colsum)
       for (int rr = 0; rr < nrows; ++rr) s += sk_smem[rr * KP + tid];

@@ -67,6 +67,12 @@ class MLPBase(nn.Module):
         shapes allow (fused._MLPTail); None when they do not (the caller then takes the plain route)."""
         if not (self._pairs and fused.fused_enabled() and x.is_cuda):
             return None
+        if len(self._pairs) == 2:
+            (fc1, act1), (fc, act) = self._pairs
+            if fused.first_ok(x, fc1, act1) and fused.tail_ok(x, fc, act, head):
+                # the whole MLP as one node: the backward reduces dH1 to the first layer's gradients in place
+                return fused.mlp_tail(x, fc, fused.ACT_CODES[type(act)], head,
+                                      first=(fc1, fused.ACT_CODES[type(act1)]))
         for fc, act in self._pairs[:-1]:
             x = self._pair(x, fc, act)
         fc, act = self._pairs[-1]

@@ -400,22 +400,26 @@ def _defer_scratch(kind, M, H, K, device):
 def flush_reduces():
     """Second stages of every job recorded since the scope opened, on the current stream (which must already be ordered
     after the streams the first stages ran on)."""
-    import ctypes
     global _DEFER
     jobs = _DEFER
     if not jobs:
         return
     for i in range(0, len(jobs), 8):
-        part = jobs[i:i + 8]
-        n = len(part)
-        vp = ctypes.c_void_p
-        _lib.call("trl_skinny_reduce_jobs", n, (ctypes.c_int * n)(*[j[0] for j in part]),
-                  (vp * n)(*[j[1].data_ptr() for j in part]),
-                  (vp * n)(*[0 if j[2] is None else j[2].data_ptr() for j in part]),
-                  (vp * n)(*[0 if j[3] is None else j[3].data_ptr() for j in part]),
-                  (ctypes.c_int64 * n)(*[j[4] for j in part]), (ctypes.c_int * n)(*[j[5] for j in part]),
-                  (ctypes.c_int * n)(*[j[6] for j in part]), (ctypes.c_int * n)(*[j[7] for j in part]), ops._stream())
+        _reduce_jobs(jobs[i:i + 8])
     _DEFER = []
+
+
+def _reduce_jobs(part):
+    """One trl_skinny_reduce_jobs launch for up to 8 jobs (kind, scratch, out, colsum, M, H, K, out_transposed)."""
+    import ctypes
+    n = len(part)
+    vp = ctypes.c_void_p
+    _lib.call("trl_skinny_reduce_jobs", n, (ctypes.c_int * n)(*[j[0] for j in part]),
+              (vp * n)(*[j[1].data_ptr() for j in part]),
+              (vp * n)(*[0 if j[2] is None else j[2].data_ptr() for j in part]),
+              (vp * n)(*[0 if j[3] is None else j[3].data_ptr() for j in part]),
+              (ctypes.c_int64 * n)(*[j[4] for j in part]), (ctypes.c_int * n)(*[j[5] for j in part]),
+              (ctypes.c_int * n)(*[j[6] for j in part]), (ctypes.c_int * n)(*[j[7] for j in part]), ops._stream())
 
 
 def _can_defer(*outs):
@@ -448,12 +452,9 @@ class _LinearAct(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, act):
         tc = (_MATMUL_MODE == "tf32x3" and min(x.shape[0], x.shape[1], weight.shape[0]) >= _TF32X3_MIN_DIM)
-        if (_MATMUL_MODE != "fp32" and _skinny_ok(x) and x.shape[1] <= 24 and weight.shape[0] % 4 == 0
-                and weight.shape[0] <= 1024 and weight.is_contiguous() and bias.is_contiguous()):
+        if _first_skinny_ok(x, weight, bias):
             # skinny first layer: GEMM + bias + activation in one memory-bound launch
-            z = torch.empty(x.shape[0], weight.shape[0], dtype=torch.float32, device=x.device)
-            _lib.call("trl_skinny_k_fwd", x.data_ptr(), weight.data_ptr(), bias.data_ptr(), z.data_ptr(), x.shape[0],
-                      x.shape[1], weight.shape[0], act, ops._stream())
+            z = _skinny_first_fwd(x, weight, bias, act)
             ctx.save_for_backward(x, weight, z)
             ctx.act, ctx.tc, ctx.params = act, False, (weight, bias)
             return z
@@ -483,40 +484,64 @@ class _LinearAct(torch.autograd.Function):
         if ctx.tc:
             return _LinearAct._backward_tc(ctx, g)
         x, weight, y = ctx.saved_tensors
-        g = g if g.is_contiguous() else g.contiguous()
-        M, H = y.shape
-        w_param, b_param = ctx.params
-        db_out, dw_out = _grad_out(b_param), _grad_out(w_param)
-        db = db_out if db_out is not None else torch.empty(H, dtype=torch.float32, device=y.device)
-        K = x.shape[1]
-        if (not ctx.needs_input_grad[0] and _MATMUL_MODE != "fp32" and _skinny_ok(y) and K <= 24 and H % 32 == 0
-                and H <= 256 and x.is_contiguous() and (dw_out is None or dw_out.is_contiguous())):
-            # first layer (its input needs no gradient): dW and db straight from g and y in ONE pass over the
-            # (M, H) matrices; the activation gradient gz is never written to memory
-            dw = dw_out if dw_out is not None else torch.empty(H, K, dtype=torch.float32, device=y.device)
-            if _can_defer(dw_out, db_out):
-                ws = _defer_scratch(1, M, H, K, y.device)
-                _lib.call("trl_skinny_act_wgrad_partial", g.data_ptr(), y.data_ptr(), x.data_ptr(), M, H, K, ctx.act,
-                          ws.data_ptr(), ops._stream())
-                _DEFER.append((1, ws, dw, db, M, H, K, 0))
-                return None, None, None, None
-            _lib.call("trl_skinny_act_wgrad", g.data_ptr(), y.data_ptr(), x.data_ptr(), dw.data_ptr(), db.data_ptr(),
-                      M, H, K, ctx.act, _tn_scratch(M, H, K, y.device).data_ptr(), ops._stream())
-            _lib.add_launches(1)
-            return None, None if dw_out is not None else dw, None if db_out is not None else db, None
-        gz = torch.empty_like(y)
-        scratch, tickets = _Workspace.get(M, H, y.device)
-        _lib.call("trl_bias_act_bwd", g.data_ptr(), y.data_ptr(), gz.data_ptr(), db.data_ptr(), M, H, ctx.act,
-                  scratch.data_ptr(), tickets.data_ptr(), ops._stream())
-        dx = None
-        if ctx.needs_input_grad[0]:
-            if _tc3_ok(M, weight.shape[1], H) and weight.is_contiguous():
-                dx = mm_dgrad(gz, weight)
-            else:
-                dx = torch.mm(gz, weight)
-        dw = wgrad(gz, x, out=dw_out) if ctx.needs_input_grad[1] else None
-        return (dx, None if dw_out is not None else dw,
-                None if db_out is not None else (db if ctx.needs_input_grad[2] else None), None)
+        return _linear_act_bwd(g, x, weight, y, ctx.act, ctx.params, ctx.needs_input_grad) + (None,)
+
+
+def _first_skinny_ok(x, weight, bias):
+    """The skinny first-layer forward (csrc/skinny.cu k_fwd) serves x (M, K <= 24) . weight^T."""
+    return (_MATMUL_MODE != "fp32" and _skinny_ok(x) and x.shape[1] <= 24 and weight.shape[0] % 4 == 0
+            and weight.shape[0] <= 1024 and weight.is_contiguous() and bias.is_contiguous())
+
+
+def _skinny_first_fwd(x, weight, bias, act):
+    z = torch.empty(x.shape[0], weight.shape[0], dtype=torch.float32, device=x.device)
+    _lib.call("trl_skinny_k_fwd", x.data_ptr(), weight.data_ptr(), bias.data_ptr(), z.data_ptr(), x.shape[0],
+              x.shape[1], weight.shape[0], act, ops._stream())
+    return z
+
+
+def _act_wgrad_ok(x, y, dw_out):
+    """The first layer's weight / bias gradient (its input needs no gradient) runs as ONE skinny pass over g and y."""
+    H = y.shape[1]
+    return (_MATMUL_MODE != "fp32" and _skinny_ok(y) and x.shape[1] <= 24 and H % 32 == 0 and H <= 256
+            and x.is_contiguous() and (dw_out is None or dw_out.is_contiguous()))
+
+
+def _linear_act_bwd(g, x, weight, y, act, params, needs_input_grad):
+    """(dx, dW, db) of y = act(x W^T + b) for the upstream gradient g (None where not needed / written directly)."""
+    g = g if g.is_contiguous() else g.contiguous()
+    M, H = y.shape
+    w_param, b_param = params
+    db_out, dw_out = _grad_out(b_param), _grad_out(w_param)
+    db = db_out if db_out is not None else torch.empty(H, dtype=torch.float32, device=y.device)
+    K = x.shape[1]
+    if not needs_input_grad[0] and _act_wgrad_ok(x, y, dw_out):
+        # first layer (its input needs no gradient): dW and db straight from g and y in ONE pass over the
+        # (M, H) matrices; the activation gradient gz is never written to memory
+        dw = dw_out if dw_out is not None else torch.empty(H, K, dtype=torch.float32, device=y.device)
+        if _can_defer(dw_out, db_out):
+            ws = _defer_scratch(1, M, H, K, y.device)
+            _lib.call("trl_skinny_act_wgrad_partial", g.data_ptr(), y.data_ptr(), x.data_ptr(), M, H, K, act,
+                      ws.data_ptr(), ops._stream())
+            _DEFER.append((1, ws, dw, db, M, H, K, 0))
+            return None, None, None
+        _lib.call("trl_skinny_act_wgrad", g.data_ptr(), y.data_ptr(), x.data_ptr(), dw.data_ptr(), db.data_ptr(),
+                  M, H, K, act, _tn_scratch(M, H, K, y.device).data_ptr(), ops._stream())
+        _lib.add_launches(1)
+        return None, None if dw_out is not None else dw, None if db_out is not None else db
+    gz = torch.empty_like(y)
+    scratch, tickets = _Workspace.get(M, H, y.device)
+    _lib.call("trl_bias_act_bwd", g.data_ptr(), y.data_ptr(), gz.data_ptr(), db.data_ptr(), M, H, act,
+              scratch.data_ptr(), tickets.data_ptr(), ops._stream())
+    dx = None
+    if needs_input_grad[0]:
+        if _tc3_ok(M, weight.shape[1], H) and weight.is_contiguous():
+            dx = mm_dgrad(gz, weight)
+        else:
+            dx = torch.mm(gz, weight)
+    dw = wgrad(gz, x, out=dw_out) if needs_input_grad[1] else None
+    return (dx, None if dw_out is not None else dw,
+            None if db_out is not None else (db if needs_input_grad[2] else None))
 
 
 def _backward_tc(ctx, g):
@@ -579,33 +604,38 @@ class _LinearPlain(torch.autograd.Function):
 
 
 class _MLPTail(torch.autograd.Function):
-    """Last hidden layer + output layer of an MLP head as ONE autograd node:
-        y2 = act(x W2^T + b2)   (wgmma 3xTF32, bias + activation in the epilogue)
+    """Last hidden layer + output layer of an MLP head as ONE autograd node, optionally with a skinny first layer:
+        h1 = act1(x W1^T + b1)  (csrc/skinny.cu k_fwd; only when w1 is given, x then needs no gradient)
+        y2 = act(h1 W2^T + b2)  (wgmma 3xTF32, bias + activation in the epilogue)
         out = y2 W3^T + b3      (csrc/skinny.cu n_fwd)
     so that the backward can fuse the output-layer dgrad with the activation backward of the hidden layer
-    (trl_skinny_n_dgrad_act: gz2 and db2 in one pass, the (M, 256) dgrad matrix is never stored un-activated)."""
+    (trl_skinny_n_dgrad_act: gz2 and db2 in one pass, the (M, 256) dgrad matrix is never stored un-activated), and,
+    with the first layer, the dgrad dH1 = gz2 W2 with the first layer's weight / bias gradient: inside
+    `transposed_planes()` trl_gemm3_pair_dgrad_act_wgrad reduces dH1 to dW1 / db1 slab partials in its epilogue, so
+    dH1 is never stored (elsewhere: mm_dgrad, then the skinny first-layer backward, the same bits)."""
 
     @staticmethod
-    def forward(ctx, x, w2, b2, w3, b3, act):
-        y2 = mm_fwd(x, w2, bias=b2, act=act)
+    def forward(ctx, x, w1, b1, act1, w2, b2, w3, b3, act):
+        h1 = _skinny_first_fwd(x, w1, b1, act1) if w1 is not None else x
+        y2 = mm_fwd(h1, w2, bias=b2, act=act)
         M, H = y2.shape
         N = w3.shape[0]
         out = torch.empty(M, N, dtype=torch.float32, device=x.device)
         _lib.call("trl_skinny_n_fwd", y2.data_ptr(), w3.data_ptr(), b3.data_ptr(), out.data_ptr(), M, H, N,
                   ops._stream())
-        ctx.save_for_backward(x, w2, y2, w3)
-        ctx.act = act
-        ctx.params = (w2, b2, w3, b3)
+        ctx.save_for_backward(x, w1, h1, w2, y2, w3)
+        ctx.act, ctx.act1 = act, act1
+        ctx.params = (w1, b1, w2, b2, w3, b3)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        x, w2, y2, w3 = ctx.saved_tensors
+        x0, w1, x, w2, y2, w3 = ctx.saved_tensors
         g = g if g.is_contiguous() else g.contiguous()
         M, H = y2.shape
         N = w3.shape[0]
         dev = y2.device
-        w2p, b2p, w3p, b3p = ctx.params
+        w1p, b1p, w2p, b2p, w3p, b3p = ctx.params
         dw2_out, db2_out, dw3_out, db3_out = _grad_out(w2p), _grad_out(b2p), _grad_out(w3p), _grad_out(b3p)
         db2 = db2_out if db2_out is not None else torch.empty(H, dtype=torch.float32, device=dev)
         db3 = db3_out if db3_out is not None else torch.empty(N, dtype=torch.float32, device=dev)
@@ -624,6 +654,8 @@ class _MLPTail(torch.autograd.Function):
             _lib.call("trl_skinny_n_dgrad_act", g.data_ptr(), w3.data_ptr(), y2.data_ptr(), gz.data_ptr(), db2.data_ptr(),
                       M, H, N, ctx.act, ws.data_ptr(), ops._stream())
             _lib.add_launches(1)
+        first = w1 is not None
+        want_dx = ctx.needs_input_grad[0] and not first
         fk = _fork_here()
         if fk is not None and dw2_out is not None and dw3_out is not None:
             # the two weight gradients feed nothing but the optimizer: companion stream (see backward_fork)
@@ -633,14 +665,48 @@ class _MLPTail(torch.autograd.Function):
                 dw2 = wgrad(gz, x, out=dw2_out)
             fk.keep += [gz, g, y2, x]
             fk.used = True
-            dx = mm_dgrad(gz, w2) if ctx.needs_input_grad[0] else None
+            first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
+            dx = mm_dgrad(gz, w2) if want_dx else None
         else:
             dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True,   # dW3 (N,H) = g^T y2, db3 = sum g
                             may_defer=dw3_out is not None and db3_out is not None)
-            dx = mm_dgrad(gz, w2) if ctx.needs_input_grad[0] else None
+            first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
+            dx = mm_dgrad(gz, w2) if want_dx else None
             dw2 = wgrad(gz, x, out=dw2_out)
-        return (dx, None if dw2_out is not None else dw2, None if db2_out is not None else db2,
+        tail = (None if dw2_out is not None else dw2, None if db2_out is not None else db2,
                 None if dw3_out is not None else dw3, None if db3_out is not None else db3, None)
+        if first:
+            return (None,) + first_grads + (None,) + tail
+        return (dx, None, None, None) + tail
+
+
+def _first_layer_bwd(ctx, gz, x0, w1, h1, w2):
+    """(dW1, db1) from gz2: dH1 = gz2 W2 feeds nothing else (x0 needs no gradient).  Inside `transposed_planes()`
+    the dgrad's epilogue forms the first layer's slab partials (dH1 never stored); elsewhere mm_dgrad, then the
+    skinny first-layer backward.  The slab sums are the same kernels either way: deferred inside deferred_reduces()."""
+    M, H = h1.shape
+    K = x0.shape[1]
+    w1p, b1p = ctx.params[0], ctx.params[1]
+    dw_out, db_out = _grad_out(w1p), _grad_out(b1p)
+    planes_t = (_TRANSPOSED.planes(w2) if _TRANSPOSED is not None and _GEMM_IMPL == "pair" and H == 256
+                and tuple(w2.shape) == (256, 256) else None)
+    if planes_t is None or M > _DGRAD_FIRST_MAX_ROWS or not _act_wgrad_ok(x0, h1, dw_out):
+        return _linear_act_bwd(mm_dgrad(gz, w2), x0, w1, h1, ctx.act1, (w1p, b1p), (False, True, True))[1:]
+    dw = dw_out if dw_out is not None else torch.empty(H, K, dtype=torch.float32, device=h1.device)
+    db = db_out if db_out is not None else torch.empty(H, dtype=torch.float32, device=h1.device)
+    if _can_defer(dw_out, db_out):
+        ws = _defer_scratch(1, M, H, K, h1.device)
+        ops.gemm3_pair_dgrad_act_wgrad(gz, planes_t, h1, x0, ctx.act1, ws)
+        _DEFER.append((1, ws, dw, db, M, H, K, 0))
+        return None, None
+    ws = _tn_scratch(M, H, K, h1.device)
+    ops.gemm3_pair_dgrad_act_wgrad(gz, planes_t, h1, x0, ctx.act1, ws)
+    _reduce_jobs([(1, ws, dw, db, M, H, K, 0)])
+    _lib.add_launches(1)
+    return None if dw_out is not None else dw, None if db_out is not None else db
+
+
+_DGRAD_FIRST_MAX_ROWS = 16896    # trl_gemm3_pair_dgrad_act_wgrad: slabs of at most 64 rows (sk_rows_per_cta)
 
 
 def tail_ok(h, fc, act_module, head):
@@ -655,12 +721,22 @@ def tail_ok(h, fc, act_module, head):
             and fc.weight.is_contiguous() and head.weight.is_contiguous())
 
 
-def mlp_tail(h, fc, act_code, head):
+def first_ok(x, fc, act_module):
+    """True when act(fc(x)) can open an _MLPTail node as its skinny first layer: x needs no gradient and the layer
+    takes the skinny forward of _LinearAct."""
+    if not (can_fuse(x, fc, act_module) and not x.requires_grad and x.dim() >= 1):
+        return False
+    return _first_skinny_ok(x.reshape(-1, x.shape[-1]), fc.weight, fc.bias)
+
+
+def mlp_tail(h, fc, act_code, head, first=None):
+    """head(act(fc(h))) as one _MLPTail node; first = (fc1, act1_code): h is the input of that skinny first layer."""
     lead = h.shape[:-1]
     h2 = h.reshape(-1, h.shape[-1])
     if not h2.is_contiguous():
         h2 = h2.contiguous()
-    out = _MLPTail.apply(h2, fc.weight, fc.bias, head.weight, head.bias, act_code)
+    w1, b1, act1 = (first[0].weight, first[0].bias, first[1]) if first is not None else (None, None, 0)
+    out = _MLPTail.apply(h2, w1, b1, act1, fc.weight, fc.bias, head.weight, head.bias, act_code)
     return out.reshape(tuple(lead) + (out.shape[-1],))
 
 

@@ -563,6 +563,19 @@ def gemm3_pair_tn_cluster(a, b, workspace, tickets, out=None, splits=64):
     return out
 
 
+def gemm3_pair_dgrad_act_wgrad(g, planes_t, h1, x, act, scratch):
+    """The first layer's weight / bias gradient slab partials of dH1 = g (M,256) @ W2, dH1 never stored: the
+    partials trl_skinny_act_wgrad_partial(dH1, h1, x) writes, bit for bit, into `scratch`
+    (trl_skinny_tn_scratch_floats(M, 256, K) floats; summed by trl_skinny_reduce_jobs, kind 1).
+    planes_t = (hi^T, lo^T): the transposed pre-split planes of W2.  M <= 16896, x (M,K) with K <= 24."""
+    M, K = x.shape
+    hi, lo = planes_t
+    assert g.shape == (M, 256) and h1.shape == (M, 256) and hi.shape == (256, 256) and lo.shape == (256, 256)
+    _lib.call("trl_gemm3_pair_dgrad_act_wgrad", _chk(g, F32, "g"), _chk(hi, F32, "w_hi_t"), _chk(lo, F32, "w_lo_t"),
+              _chk(h1, F32, "h1"), _chk(x, F32, "x"), M, K, int(act), _chk(scratch, F32, "scratch"), _stream())
+    return scratch
+
+
 def transpose_f32(x, out=None):
     """out (C,R) = x (R,C)^T (contiguous)."""
     R, C = x.shape
