@@ -336,6 +336,17 @@ int trl_skinny_n_dgrad_act_partial(const float* G, const float* W, const float* 
 int trl_skinny_reduce_jobs(int njobs, const int* kind, const float* const* scratch, float* const* out,
                            float* const* colsum, const int64_t* M, const int* H, const int* K, const int* out_transposed,
                            void* stream);
+/* The output layer's whole backward in one pass over Y (H == 256, 1 <= N <= 8): trl_skinny_n_dgrad_act_partial(G, W, Y,
+ * gz, M, 256, N, act, db_scratch) and trl_skinny_tn_partial(Y, G, M, 256, N, 1, w_scratch) in one launch, bit for bit.
+ * db_scratch (trl_skinny_dgrad_act_scratch_floats(M, 256) floats) is summed by reduce kind 2, w_scratch
+ * (trl_skinny_tn_scratch_floats(M, 256, N) floats) by kind 0 with out_transposed = 1.  W, Y, gz, w_scratch 16-byte
+ * aligned.  The second form also runs both reduces in one launch: db (256) = colsum(gz), dW (N x 256) = G^T Y,
+ * dbias (N) = colsum(G). */
+int trl_skinny_n_dgrad_act_wgrad_partial(const float* G, const float* W, const float* Y, float* gz, int64_t M, int H,
+                                         int N, int act, float* db_scratch, float* w_scratch, void* stream);
+int trl_skinny_n_dgrad_act_wgrad(const float* G, const float* W, const float* Y, float* gz, float* db, float* dW,
+                                 float* dbias, int64_t M, int H, int N, int act, float* db_scratch, float* w_scratch,
+                                 void* stream);
 
 /* ---- K1 for BASELINE config 4: synthetic Atari-shaped pixel env, obs (N,4,84,84) uint8, 6 actions (defined in
  * oracle/synth_atari.py; the reference only wraps real ALE games, env/atari_wrapper.py).  latent: (N,5) int32. */

@@ -103,6 +103,8 @@ SIGNATURES = {
     "trl_skinny_act_wgrad_partial": [vp, vp, vp, i64, i32, i32, i32, vp, vp],
     "trl_skinny_n_dgrad_act_partial": [vp, vp, vp, vp, i64, i32, i32, i32, vp, vp],
     "trl_skinny_reduce_jobs": [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp],
+    "trl_skinny_n_dgrad_act_wgrad_partial": [vp, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp],
+    "trl_skinny_n_dgrad_act_wgrad": [vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp],
     "trl_synth_atari_step": [vp, vp, vp, vp, vp, vp, vp, i64, i32, vp],
     "trl_synth_atari_reset": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i64, vp],
     "trl_u8_to_f32": [vp, vp, i64, f32, vp],

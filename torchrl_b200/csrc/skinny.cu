@@ -12,9 +12,11 @@
 //   skinny_tn      : Out (H,K) = A (M,H)^T . B (M,K)  [+ column sums of B]       K <= 24, H % 32 == 0, H <= 256
 //   skinny_n_fwd   : Y (M,N)  = X (M,H) . W (N,H)^T + b                          N <= 8, H in {128, 256}
 //   skinny_n_dgrad : dX (M,H) = G (M,N) . W (N,H)                                N <= 8, H % 4 == 0, H <= 1024
-// and two backward fusions that remove a whole pass over the (M x H) matrix each:
+// and three backward fusions that remove a whole pass over the (M x H) matrix each:
 //   skinny_act_wgrad   : dW1 = (G * act'(Y))^T X,  db1 = colsum(G * act'(Y))    (first layer: gz never stored)
 //   skinny_n_dgrad_act : gz = (G . W) * act'(Y),  db = colsum(gz)               (output-layer dgrad + act backward)
+//   skinny_n_dgrad_act_wgrad : the above and dW = G^T Y, db_out = colsum(G)     (H = 256: the output layer's whole
+//                        backward in one pass over Y; skinny_tn's slab partials bit for bit)
 // Reductions have a fixed combination order (deterministic, run-to-run bit-identical).
 #include "skinny_common.cuh"
 
@@ -330,26 +332,56 @@ __global__ void __launch_bounds__(256, 2) skinny_n_fwd_kernel(const float* __res
 // ([rows][8], zero padded) broadcast from shared memory: 2 LDS.128 + 32 FMA + one 16-byte store per row.
 // ACT = true: the result is multiplied by act'(Yact) before it is stored (gz of the last hidden layer) and the
 // per-column sums of the stored values (that layer's bias gradient) go to colpart[cta][H].
-template <bool ACT>
+// NW > 0 (with ACT, H = 256, N = NW): the same pass also forms the output layer's weight / bias gradient slab partial
+// of skinny_tn_kernel<NW, false>(Yact, G, want_colsum = 1), bit for bit, in wpart[cta][NW + 1][H].  At H = 256 both
+// kernels give a thread 4 columns and a row lane rl in 0..3 that runs rows rl, rl + 4, ... in increasing order; each
+// thread feeds the Yact float4 it loaded for act'() and the staged G row to tn_fma_row<NW> (skinny_common.cuh), the
+// 4 row lanes (here in different warps) are added through shared memory as (v0 + v1) + (v2 + v3), tn_combine_lanes'
+// value, and row NW is the sequential sum of the slab's staged G rows.
+template <bool ACT, int NW>
 __global__ void __launch_bounds__(256, 2) skinny_n_dgrad_kernel(const float* __restrict__ G, const float* __restrict__ W,
                                                                const float* __restrict__ Yact, int act,
                                                                float* __restrict__ dX, float* __restrict__ colpart,
-                                                               long long M, int H, int N, int rows_per_cta) {
-  extern __shared__ __align__(16) float sk_smem[];
+                                                               float* __restrict__ wpart, long long M, int H, int N,
+                                                               int rows_per_cta) {
+  static_assert(NW == 0 || (ACT && NW <= 8), "the output-layer weight gradient rides on the activation backward");
+  extern __shared__ __align__(16) float sk_smem[];       // G slab [rows_per_cta][8]; NW > 0: then [3][NW][H]
   __shared__ __align__(16) float colred[1024];           // [RL][H], RL * H <= 1024
   const int tid = threadIdx.x;
   const long long row0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
   const int nrows = static_cast<int>(min(static_cast<long long>(rows_per_cta), M - row0));   // grid never overshoots
-  stage_rows_rt<8>(sk_smem, G, row0, nrows, N, tid, 256);
+  if (NW > 0) N = NW;
   const int cpg = H >> 2;
   const int RL = 256 / cpg;
   const bool active = tid < RL * cpg;
   const int cg = tid % cpg, rl = tid / cpg;
+  // NW in 1..6 (registers to spare): the Yact rows go through a two-batch pipeline, the next four rows requested
+  // before the current four are used, and the first four are requested before the G slab is staged, so that only
+  // one load latency per CTA is exposed (a slab is 16 rows per row lane at M = 16384).  Same rows, same order.
+  constexpr bool kPipe = NW > 0 && NW <= 6;
+  const float* yp = ACT ? Yact + row0 * H + 4 * cg : nullptr;
+  float4 ya[4], yn[4];
+  auto load4 = [&](float4 (&d)[4], int r) {
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+      d[u] = (r + u * RL < nrows) ? __ldg(reinterpret_cast<const float4*>(yp + static_cast<long long>(r + u * RL) * H))
+                                  : make_float4(0.f, 0.f, 0.f, 0.f);
+  };
+  if (kPipe) load4(ya, rl);
+  stage_rows_rt<8>(sk_smem, G, row0, nrows, N, tid, 256);
   float4 w[8];
 #pragma unroll
   for (int n = 0; n < 8; ++n)
     w[n] = (active && n < N) ? *reinterpret_cast<const float4*>(W + static_cast<long long>(n) * H + 4 * cg)
                              : make_float4(0.f, 0.f, 0.f, 0.f);
+  constexpr int NWA = NW > 0 ? NW : 1;
+  float wacc[(NWA + 3) & ~3][4];                         // this thread's 4 columns of the NW rows of G^T Yact
+  if (NW > 0) {
+#pragma unroll
+    for (int k = 0; k < NWA; ++k)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) wacc[k][j] = 0.f;
+  }
   __syncthreads();
   float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
   auto row_out = [&](int r, float4 yv) {
@@ -365,6 +397,7 @@ __global__ void __launch_bounds__(256, 2) skinny_n_dgrad_kernel(const float* __r
     acc.x = fmaf(g1.z, w[6].x, acc.x); acc.y = fmaf(g1.z, w[6].y, acc.y); acc.z = fmaf(g1.z, w[6].z, acc.z); acc.w = fmaf(g1.z, w[6].w, acc.w);
     acc.x = fmaf(g1.w, w[7].x, acc.x); acc.y = fmaf(g1.w, w[7].y, acc.y); acc.z = fmaf(g1.w, w[7].z, acc.z); acc.w = fmaf(g1.w, w[7].w, acc.w);
     if (ACT) {
+      if (NW > 0) tn_fma_row<NWA>(wacc, yv, sk_smem + r * 8);
       acc = sk_dact4(acc, yv, act);
       cs.x += acc.x; cs.y += acc.y; cs.z += acc.z; cs.w += acc.w;
     }
@@ -373,10 +406,18 @@ __global__ void __launch_bounds__(256, 2) skinny_n_dgrad_kernel(const float* __r
   if (active) {
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     int r = rl;
-    if (ACT) {
+    if (kPipe) {
+      for (; r < nrows; r += 4 * RL) {
+        load4(yn, r + 4 * RL);
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+          if (r + u * RL < nrows) row_out(r + u * RL, ya[u]);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) ya[u] = yn[u];
+      }
+    } else if (ACT) {
       // the activations of four rows are requested before the first one is used: four 16-byte loads in flight per
       // thread instead of one dependent load per row
-      const float* yp = Yact + row0 * H + 4 * cg;
       for (; r + 3 * RL < nrows; r += 4 * RL) {
         const float4 y0 = __ldg(reinterpret_cast<const float4*>(yp + static_cast<long long>(r) * H));
         const float4 y1 = __ldg(reinterpret_cast<const float4*>(yp + static_cast<long long>(r + RL) * H));
@@ -390,12 +431,40 @@ __global__ void __launch_bounds__(256, 2) skinny_n_dgrad_kernel(const float* __r
     }
   }
   if (ACT) {
+    float* cb = sk_smem + rows_per_cta * 8;              // NW > 0: row lanes 1..3 of wacc, [3][NW][H]
+    float gs = 0.f;
     if (active) *reinterpret_cast<float4*>(colred + rl * H + 4 * cg) = cs;
+    if (NW > 0) {
+      if (rl > 0) {
+#pragma unroll
+        for (int k = 0; k < NW; ++k)
+          *reinterpret_cast<float4*>(cb + ((rl - 1) * NW + k) * H + 4 * cg) =
+              make_float4(wacc[k][0], wacc[k][1], wacc[k][2], wacc[k][3]);
+      }
+      if (tid < NW)
+        for (int rr = 0; rr < nrows; ++rr) gs += sk_smem[rr * 8 + tid];
+    }
     __syncthreads();
     for (int c = tid; c < H; c += blockDim.x) {          // H may exceed the 256 threads (H <= 1024)
       float s = colred[c];
       for (int i = 1; i < RL; ++i) s += colred[i * H + c];
       colpart[static_cast<long long>(blockIdx.x) * H + c] = s;
+    }
+    if (NW > 0) {
+      // skinny_tn_kernel's partial layout, [NW + 1][H] per CTA; only the first NW entries of row NW are meaningful
+      float* pp = wpart + static_cast<long long>(blockIdx.x) * (NW + 1) * H;
+      if (rl == 0) {
+#pragma unroll
+        for (int k = 0; k < NW; ++k) {
+          const float4 v1 = *reinterpret_cast<const float4*>(cb + k * H + 4 * cg);
+          const float4 v2 = *reinterpret_cast<const float4*>(cb + (NW + k) * H + 4 * cg);
+          const float4 v3 = *reinterpret_cast<const float4*>(cb + (2 * NW + k) * H + 4 * cg);
+          *reinterpret_cast<float4*>(pp + k * H + 4 * cg) =
+              make_float4((wacc[k][0] + v1.x) + (v2.x + v3.x), (wacc[k][1] + v1.y) + (v2.y + v3.y),
+                          (wacc[k][2] + v1.z) + (v2.z + v3.z), (wacc[k][3] + v1.w) + (v2.w + v3.w));
+        }
+      }
+      if (tid < NW) pp[NW * H + tid] = gs;
     }
   }
 }
@@ -524,8 +593,8 @@ TRL_API int trl_skinny_n_dgrad(const float* G, const float* W, float* dX, int64_
   TRL_REQUIRE(aligned16(W) && aligned16(dX), "trl_skinny_n_dgrad: W/dX must be 16-byte aligned");
   const int rows = sk_rows_per_cta(M);
   const unsigned grid = static_cast<unsigned>(ceil_div<long long>(M, rows));
-  skinny_n_dgrad_kernel<false><<<grid, 256, sizeof(float) * rows * 8, static_cast<cudaStream_t>(stream)>>>(
-      G, W, nullptr, 0, dX, nullptr, M, H, N, rows);
+  skinny_n_dgrad_kernel<false, 0><<<grid, 256, sizeof(float) * rows * 8, static_cast<cudaStream_t>(stream)>>>(
+      G, W, nullptr, 0, dX, nullptr, nullptr, M, H, N, rows);
   return check_launch("skinny_n_dgrad_kernel");
 }
 
@@ -546,7 +615,8 @@ static int launch_n_dgrad_act(const float* G, const float* W, const float* Y, fl
   const int rows = sk_rows_per_cta(M);
   const int nslab = static_cast<int>(ceil_div<long long>(M, rows));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  skinny_n_dgrad_kernel<true><<<nslab, 256, sizeof(float) * rows * 8, st>>>(G, W, Y, act, gz, scratch, M, H, N, rows);
+  skinny_n_dgrad_kernel<true, 0><<<nslab, 256, sizeof(float) * rows * 8, st>>>(G, W, Y, act, gz, scratch, nullptr, M, H,
+                                                                               N, rows);
   int rc = check_launch("skinny_n_dgrad_kernel");
   if (rc != TRL_OK || defer) return rc;
   // column sums: partial [nslab][H] viewed as a K = 0 "tn" partial (stride H, all H entries are colsum entries)
@@ -616,4 +686,51 @@ TRL_API int trl_skinny_reduce_jobs(int njobs, const int* kind, const float* cons
   q.njobs = njobs;
   skinny_reduce_jobs_kernel<<<ctas, kRedElems * kRedGroups, 0, static_cast<cudaStream_t>(stream)>>>(q);
   return check_launch("skinny_reduce_jobs_kernel");
+}
+
+// ---- the output layer's whole backward in one pass over Y (H = 256) ------------------------------------------------
+// trl_skinny_n_dgrad_act_partial(G, W, Y, gz, M, 256, N, act, db_scratch) and trl_skinny_tn_partial(Y, G, M, 256, N, 1,
+// w_scratch) in one launch, the same bits: gz, the db slabs (reduce kind 2) and the dW (N,H) / dbias (N) slabs (kind 0,
+// out_transposed = 1).  db_scratch: trl_skinny_dgrad_act_scratch_floats(M, 256); w_scratch:
+// trl_skinny_tn_scratch_floats(M, 256, N).
+TRL_API int trl_skinny_n_dgrad_act_wgrad_partial(const float* G, const float* W, const float* Y, float* gz, int64_t M,
+                                                 int H, int N, int act, float* db_scratch, float* w_scratch,
+                                                 void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(M >= 1 && N >= 1 && N <= 8 && H == 256,
+              "trl_skinny_n_dgrad_act_wgrad: need M>=1, 1<=N<=8, H==256 (M=%lld N=%d H=%d)", static_cast<long long>(M),
+              N, H);
+  TRL_REQUIRE(G && W && Y && gz && db_scratch && w_scratch, "trl_skinny_n_dgrad_act_wgrad: null pointer");
+  TRL_REQUIRE(act >= 0 && act <= 2, "trl_skinny_n_dgrad_act_wgrad: unknown activation %d", act);
+  TRL_REQUIRE(aligned16(W) && aligned16(Y) && aligned16(gz) && aligned16(w_scratch),
+              "trl_skinny_n_dgrad_act_wgrad: W/Y/gz/w_scratch must be 16-byte aligned");
+  const int rows = sk_rows_per_cta(M);
+  const int nslab = static_cast<int>(ceil_div<long long>(M, rows));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t smem = sizeof(float) * (static_cast<size_t>(rows) * 8 + 3 * static_cast<size_t>(N) * H);   // <= 28 KB
+#define TRL_NDW(NN)                                                                                              \
+  case NN:                                                                                                       \
+    skinny_n_dgrad_kernel<true, NN><<<nslab, 256, smem, st>>>(G, W, Y, act, gz, db_scratch, w_scratch, M, H, N, rows); \
+    break
+  switch (N) {
+    TRL_NDW(1); TRL_NDW(2); TRL_NDW(3); TRL_NDW(4); TRL_NDW(5); TRL_NDW(6); TRL_NDW(7); TRL_NDW(8);
+  }
+#undef TRL_NDW
+  return check_launch("skinny_n_dgrad_kernel");
+}
+
+// ... and both second stages in one trl_skinny_reduce_jobs launch: db (H) = colsum(gz), dW (N,H) = G^T Y, dbias (N) =
+// colsum(G).
+TRL_API int trl_skinny_n_dgrad_act_wgrad(const float* G, const float* W, const float* Y, float* gz, float* db, float* dW,
+                                         float* dbias, int64_t M, int H, int N, int act, float* db_scratch,
+                                         float* w_scratch, void* stream) {
+  TRL_REQUIRE(db && dW && dbias, "trl_skinny_n_dgrad_act_wgrad: null pointer");
+  const int rc = trl_skinny_n_dgrad_act_wgrad_partial(G, W, Y, gz, M, H, N, act, db_scratch, w_scratch, stream);
+  if (rc != TRL_OK) return rc;
+  const int kind[2] = {2, 0}, Hs[2] = {H, H}, Ks[2] = {0, N}, out_t[2] = {0, 1};
+  const float* scratch[2] = {db_scratch, w_scratch};
+  float* out[2] = {nullptr, dW};
+  float* colsum[2] = {db, dbias};
+  const int64_t Ms[2] = {M, M};
+  return trl_skinny_reduce_jobs(2, kind, scratch, out, colsum, Ms, Hs, Ks, out_t, stream);
 }

@@ -255,7 +255,8 @@ _FORK_STREAMS = {}
 
 class backward_fork:
     """Scope around ONE `torch.autograd.backward` call of an MLP with a fused tail: the weight-gradient work that nothing
-    downstream in that backward pass depends on (output-layer dW / db and the 256 x 256 wgrad GEMM) is issued on a
+    downstream in that backward pass depends on (the 256 x 256 wgrad GEMM, and the output layer's dW / db where they
+    are not formed in the dgrad-act pass) is issued on a
     companion stream while the dgrad GEMM and the first-layer backward continue on the calling stream; the scope's
     exit joins the two (under graph capture: a parallel branch).  Tensors the companion stream reads are kept alive
     until the join.  Outside such a scope the backward is strictly sequential."""
@@ -358,6 +359,15 @@ def _tn_scratch(M, H, K, device):
     ws = _TN_WS.get(key)
     if ws is None:
         n = int(_lib.load().trl_skinny_tn_scratch_floats(M, H, K))
+        ws = _TN_WS[key] = torch.empty(n, dtype=torch.float32, device=device)
+    return ws
+
+
+def _dgrad_act_scratch(M, H, device):
+    key = ("dgrad_act", M, H, str(device), _stream_key())
+    ws = _TN_WS.get(key)
+    if ws is None:
+        n = int(_lib.load().trl_skinny_dgrad_act_scratch_floats(M, H))
         ws = _TN_WS[key] = torch.empty(n, dtype=torch.float32, device=device)
     return ws
 
@@ -609,7 +619,9 @@ class _MLPTail(torch.autograd.Function):
         y2 = act(h1 W2^T + b2)  (wgmma 3xTF32, bias + activation in the epilogue)
         out = y2 W3^T + b3      (csrc/skinny.cu n_fwd)
     so that the backward can fuse the output-layer dgrad with the activation backward of the hidden layer
-    (trl_skinny_n_dgrad_act: gz2 and db2 in one pass, the (M, 256) dgrad matrix is never stored un-activated), and,
+    (trl_skinny_n_dgrad_act: gz2 and db2 in one pass, the (M, 256) dgrad matrix is never stored un-activated; at
+    H = 256 trl_skinny_n_dgrad_act_wgrad also forms the output layer's dW3 / db3 slab partials in that pass over y2,
+    bit for bit those of skinny_tn, so y2 is read once and the companion stream carries the wgrad alone), and,
     with the first layer, the dgrad dH1 = gz2 W2 with the first layer's weight / bias gradient: inside
     `transposed_planes()` trl_gemm3_pair_dgrad_act_wgrad reduces dH1 to dW1 / db1 slab partials in its epilogue, so
     dH1 is never stored (elsewhere: mm_dgrad, then the skinny first-layer backward, the same bits)."""
@@ -640,36 +652,46 @@ class _MLPTail(torch.autograd.Function):
         db2 = db2_out if db2_out is not None else torch.empty(H, dtype=torch.float32, device=dev)
         db3 = db3_out if db3_out is not None else torch.empty(N, dtype=torch.float32, device=dev)
         gz = torch.empty_like(y2)
-        if _can_defer(db2_out):
+        # H = 256: dW3 (N,H) = g^T y2 and db3 = sum g come out of the same pass over y2 (skinny_tn's slab partials)
+        w3_fused = H == 256
+        if w3_fused:
+            dw3 = dw3_out if dw3_out is not None else torch.empty(N, H, dtype=torch.float32, device=dev)
+        if w3_fused and _can_defer(db2_out, dw3_out, db3_out) and len(_DEFER) < 63:     # skinny_tn's bound on jobs
+            ws = _defer_scratch(2, M, H, 0, dev)
+            _DEFER.append((2, ws, None, db2, M, H, 0, 0))
+            ws3 = _defer_scratch(0, M, H, N, dev)
+            _DEFER.append((0, ws3, dw3, db3, M, H, N, 1))
+            ops.skinny_n_dgrad_act_wgrad_partial(g, w3, y2, ctx.act, gz, ws, ws3)
+        elif w3_fused:
+            ops.skinny_n_dgrad_act_wgrad(g, w3, y2, ctx.act, gz, db2, dw3, db3, _dgrad_act_scratch(M, H, dev),
+                                         _tn_scratch(M, H, N, dev))
+        elif _can_defer(db2_out):
             ws = _defer_scratch(2, M, H, 0, dev)
             _lib.call("trl_skinny_n_dgrad_act_partial", g.data_ptr(), w3.data_ptr(), y2.data_ptr(), gz.data_ptr(), M, H, N,
                       ctx.act, ws.data_ptr(), ops._stream())
             _DEFER.append((2, ws, None, db2, M, H, 0, 0))
         else:
-            key = ("dgrad_act", M, H, str(dev), _stream_key())
-            ws = _TN_WS.get(key)
-            if ws is None:
-                n = int(_lib.load().trl_skinny_dgrad_act_scratch_floats(M, H))
-                ws = _TN_WS[key] = torch.empty(n, dtype=torch.float32, device=dev)
             _lib.call("trl_skinny_n_dgrad_act", g.data_ptr(), w3.data_ptr(), y2.data_ptr(), gz.data_ptr(), db2.data_ptr(),
-                      M, H, N, ctx.act, ws.data_ptr(), ops._stream())
+                      M, H, N, ctx.act, _dgrad_act_scratch(M, H, dev).data_ptr(), ops._stream())
             _lib.add_launches(1)
         first = w1 is not None
         want_dx = ctx.needs_input_grad[0] and not first
         fk = _fork_here()
         if fk is not None and dw2_out is not None and dw3_out is not None:
-            # the two weight gradients feed nothing but the optimizer: companion stream (see backward_fork)
+            # the weight gradients that feed nothing but the optimizer: companion stream (see backward_fork)
             fk.side.wait_stream(fk.main)
             with torch.cuda.stream(fk.side):
-                dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True, may_defer=db3_out is not None)
+                if not w3_fused:
+                    dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True, may_defer=db3_out is not None)
                 dw2 = wgrad(gz, x, out=dw2_out)
-            fk.keep += [gz, g, y2, x]
+            fk.keep += [gz, x] if w3_fused else [gz, g, y2, x]
             fk.used = True
             first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
             dx = mm_dgrad(gz, w2) if want_dx else None
         else:
-            dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True,   # dW3 (N,H) = g^T y2, db3 = sum g
-                            may_defer=dw3_out is not None and db3_out is not None)
+            if not w3_fused:
+                dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True,   # dW3 (N,H) = g^T y2, db3 = sum g
+                                may_defer=dw3_out is not None and db3_out is not None)
             first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
             dx = mm_dgrad(gz, w2) if want_dx else None
             dw2 = wgrad(gz, x, out=dw2_out)

@@ -576,6 +576,31 @@ def gemm3_pair_dgrad_act_wgrad(g, planes_t, h1, x, act, scratch):
     return scratch
 
 
+def skinny_n_dgrad_act_wgrad_partial(g, w, y, act, gz, db_scratch, w_scratch):
+    """The output layer's backward in one pass over y (M,256): gz = (g (M,N) @ w (N,256)) * act'(y) into `gz`, and
+    the slab partials of db = colsum(gz) into `db_scratch` (trl_skinny_dgrad_act_scratch_floats(M, 256) floats;
+    reduce kind 2) and of dW = g^T y, dbias = colsum(g) into `w_scratch` (trl_skinny_tn_scratch_floats(M, 256, N)
+    floats; kind 0, out_transposed = 1): trl_skinny_n_dgrad_act_partial's and trl_skinny_tn_partial's bits."""
+    M, H = y.shape
+    N = w.shape[0]
+    assert g.shape == (M, N) and w.shape == (N, H) and gz.shape == (M, H)
+    _lib.call("trl_skinny_n_dgrad_act_wgrad_partial", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
+              _chk(gz, F32, "gz"), M, H, N, int(act), _chk(db_scratch, F32, "db_scratch"),
+              _chk(w_scratch, F32, "w_scratch"), _stream())
+
+
+def skinny_n_dgrad_act_wgrad(g, w, y, act, gz, db, dw, dbias, db_scratch, w_scratch):
+    """skinny_n_dgrad_act_wgrad_partial, then both slab sums in one launch: db (256), dw (N,256), dbias (N)."""
+    M, H = y.shape
+    N = w.shape[0]
+    assert g.shape == (M, N) and w.shape == (N, H) and gz.shape == (M, H)
+    assert db.shape == (H,) and dw.shape == (N, H) and dbias.shape == (N,)
+    _lib.call("trl_skinny_n_dgrad_act_wgrad", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
+              _chk(gz, F32, "gz"), _chk(db, F32, "db"), _chk(dw, F32, "dw"), _chk(dbias, F32, "dbias"), M, H, N,
+              int(act), _chk(db_scratch, F32, "db_scratch"), _chk(w_scratch, F32, "w_scratch"), _stream())
+    _lib.add_launches(1)
+
+
 def transpose_f32(x, out=None):
     """out (C,R) = x (R,C)^T (contiguous)."""
     R, C = x.shape
