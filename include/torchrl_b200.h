@@ -198,6 +198,13 @@ int trl_sac_alpha_step(const float* logp, float target_entropy, float* log_alpha
 int trl_sac_policy_loss(const float* logp, const float* q1, const float* q2, const float* log_alpha,
                         float fixed_alpha, int64_t B, float* g_logp, float* g_q1, float* g_q2, float* info5,
                         double* scratch, unsigned* ticket, void* stream);
+/* SAC / TwinSAC with a V network (sac.py:128-144, twin_sac.py:138-156): value target min(qn1,qn2) - alpha*logpi
+ * (qn2 NULL -> one critic), value MSE and the policy loss (reparameterised: mean(alpha*logpi - min q); otherwise
+ * mean(logpi * (alpha*logpi - (min q - v)).detach()), g_qn = 0) with their gradients;
+ * info6 = [policy_loss, vf_loss, logp mean/std/max/min] */
+int trl_sac_v_loss(const float* logp, const float* qn1, const float* qn2, const float* v_pred, const float* log_alpha,
+                   float fixed_alpha, int reparameterization, int64_t B, float* g_logp, float* g_qn1, float* g_qn2,
+                   float* g_v, float* info6, double* scratch, unsigned* ticket, void* stream);
 /* MSE of one or two critics against the same target (twin_sac_q.py:142-143, td3.py:96-97) */
 int trl_twin_mse_loss(const float* q1, const float* q2, const float* y, int64_t B, float* g1, float* g2,
                       float* info2, double* scratch, unsigned* ticket, void* stream);

@@ -113,6 +113,7 @@ SIGNATURES = {
     "trl_td3_smooth_action": [vp, vp, f32, f32, u64, vp, i64, vp, vp],
     "trl_sac_alpha_step": [vp, f32, vp, vp, f32, f32, f32, f32, i64, vp, vp, vp, vp],
     "trl_sac_policy_loss": [vp, vp, vp, vp, f32, i64, vp, vp, vp, vp, vp, vp, vp],
+    "trl_sac_v_loss": [vp, vp, vp, vp, vp, f32, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp],
     "trl_twin_mse_loss": [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp],
     "trl_qr_dqn_loss": [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
 }

@@ -3,6 +3,8 @@
 // Replaces the op-by-op torch graphs (and .item() syncs) of
 //   TwinSACQ.update   /root/reference/torchrl/algo/off_policy/twin_sac_q.py:84-219
 //       alpha loss :111-123, target :125-139, critic MSE :142-143, policy loss :145-160
+//   SAC.update / TwinSAC.update   /root/reference/torchrl/algo/off_policy/sac.py:74-208, twin_sac.py:82-229
+//       value target + value MSE + policy loss :128-144 / :138-156 (the rest reuses the kernels above)
 //   TD3.update        /root/reference/torchrl/algo/off_policy/td3.py:57-154
 //       target smoothing :75-84, target :86-90, actor loss :128-130
 //   QRDQN.update      /root/reference/torchrl/algo/off_policy/qrdqn.py:22-74
@@ -185,6 +187,96 @@ __global__ void __launch_bounds__(kOffThreads) sac_policy_loss_kernel(const SacP
     p.info[2] = static_cast<float>(sqrt(var > 0.0 ? var : 0.0));
     p.info[3] = static_cast<float>(t[3]);
     p.info[4] = static_cast<float>(t[4]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// SAC / TwinSAC with a state-value network (sac.py:128-144, twin_sac.py:138-156):
+//   m = min(qn1, qn2) (or qn1),  t = m - alpha*logp  (detached)
+//   vf_loss = mean((v - t)^2),                 g_v    = 2(v - t)/B
+//   reparameterised: L = mean(alpha*logp - m),  g_logp = alpha/B, g_qn per torch.min's backward (tie: split)
+//   otherwise:       c = alpha*logp - (m - v) (detached), L = mean(logp*c), g_logp = c/B, g_qn = 0
+// plus the log_probs mean/std/max/min the reference logs.
+struct SacVParams {
+  const float* __restrict__ logp;      // (B)
+  const float* __restrict__ qn1;       // (B)
+  const float* __restrict__ qn2;       // (B) or nullptr (single critic)
+  const float* __restrict__ v;         // (B) V(s)
+  const float* __restrict__ log_alpha; // (1) or nullptr (alpha = fixed_alpha)
+  float* __restrict__ g_logp;          // (B)
+  float* __restrict__ g_qn1;           // (B)
+  float* __restrict__ g_qn2;           // (B) or nullptr (with qn2)
+  float* __restrict__ g_v;             // (B)
+  float* __restrict__ info;            // [0] policy_loss [1] vf_loss [2..5] logp mean/std/max/min
+  double* __restrict__ partial;        // (grid, 5): 4 sums, then max/min packed as two floats
+  unsigned* __restrict__ ticket;
+  long long B;
+  float fixed_alpha;
+  int reparam;
+};
+
+__global__ void __launch_bounds__(kOffThreads) sac_v_loss_kernel(const SacVParams p) {
+  __shared__ double shd[32];
+  __shared__ float shf[32];
+  const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const bool ok = b < p.B;
+  const float alpha = p.log_alpha ? expf(*p.log_alpha) : p.fixed_alpha;
+  const float invB = 1.0f / static_cast<float>(p.B);
+  float L = 0.f, Lv = 0.f, lp = 0.f;
+  if (ok) {
+    lp = p.logp[b];
+    const float a = p.qn1[b];
+    const float c = p.qn2 ? p.qn2[b] : a;
+    const float m = p.qn2 ? fminf(a, c) : a;
+    const float v = p.v[b];
+    const float dv = v - (m - alpha * lp);
+    Lv = dv * dv;
+    p.g_v[b] = 2.f * dv * invB;
+    if (p.reparam) {
+      L = alpha * lp - m;
+      p.g_logp[b] = alpha * invB;
+      if (p.qn2) {
+        p.g_qn1[b] = (a < c) ? -invB : (a > c ? 0.f : -0.5f * invB);
+        p.g_qn2[b] = (c < a) ? -invB : (c > a ? 0.f : -0.5f * invB);
+      } else {
+        p.g_qn1[b] = -invB;
+      }
+    } else {
+      const float cc = alpha * lp - (m - v);
+      L = lp * cc;
+      p.g_logp[b] = cc * invB;
+      p.g_qn1[b] = 0.f;
+      if (p.qn2) p.g_qn2[b] = 0.f;
+    }
+  }
+  double* pp = p.partial + static_cast<long long>(blockIdx.x) * 5;
+  double r;
+  float f;
+  r = block_reduce_sum(static_cast<double>(L), shd);                      if (threadIdx.x == 0) pp[0] = r;
+  r = block_reduce_sum(static_cast<double>(Lv), shd);                     if (threadIdx.x == 0) pp[1] = r;
+  r = block_reduce_sum(ok ? static_cast<double>(lp) : 0.0, shd);          if (threadIdx.x == 0) pp[2] = r;
+  r = block_reduce_sum(ok ? static_cast<double>(lp) * lp : 0.0, shd);     if (threadIdx.x == 0) pp[3] = r;
+  float2* mm = reinterpret_cast<float2*>(pp + 4);
+  f = block_reduce_max(ok ? lp : -INFINITY, shf);                         if (threadIdx.x == 0) mm->x = f;
+  f = block_reduce_max(ok ? -lp : -INFINITY, shf);                        if (threadIdx.x == 0) mm->y = -f;
+  if (last_cta(p.ticket, gridDim.x) && threadIdx.x == 0) {
+    double t[4] = {0.0, 0.0, 0.0, 0.0};
+    float mx = -INFINITY, mn = INFINITY;
+    for (unsigned i = 0; i < gridDim.x; ++i) {
+      const double* q = p.partial + static_cast<long long>(i) * 5;
+      t[0] += q[0]; t[1] += q[1]; t[2] += q[2]; t[3] += q[3];
+      const float2 e = *reinterpret_cast<const float2*>(q + 4);
+      mx = fmaxf(mx, e.x); mn = fminf(mn, e.y);
+    }
+    const double Bn = static_cast<double>(p.B);
+    const double mean = t[2] / Bn;
+    const double var = (t[3] - t[2] * mean) / (Bn - 1.0);   // B == 1: 0/0 = NaN, torch's std of one element
+    p.info[0] = static_cast<float>(t[0] / Bn);
+    p.info[1] = static_cast<float>(t[1] / Bn);
+    p.info[2] = static_cast<float>(mean);
+    p.info[3] = static_cast<float>(p.B > 1 ? sqrt(var > 0.0 ? var : 0.0) : NAN);
+    p.info[4] = mx;
+    p.info[5] = mn;
   }
 }
 
@@ -394,6 +486,21 @@ TRL_API int trl_sac_policy_loss(const float* logp, const float* q1, const float*
   SacPolicyParams p{logp, q1, q2, log_alpha, g_logp, g_q1, g_q2, info5, scratch, ticket, B, fixed_alpha};
   sac_policy_loss_kernel<<<off_blocks(B), kOffThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("sac_policy_loss_kernel");
+}
+
+TRL_API int trl_sac_v_loss(const float* logp, const float* qn1, const float* qn2, const float* v_pred,
+                           const float* log_alpha, float fixed_alpha, int reparameterization, int64_t B, float* g_logp,
+                           float* g_qn1, float* g_qn2, float* g_v, float* info6, double* scratch, unsigned* ticket,
+                           void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(B >= 1, "trl_sac_v_loss: empty batch");
+  TRL_REQUIRE(logp && qn1 && v_pred && g_logp && g_qn1 && g_v && info6 && scratch && ticket,
+              "trl_sac_v_loss: null pointer");
+  TRL_REQUIRE(!qn2 || g_qn2, "trl_sac_v_loss: qn2 given without g_qn2");
+  SacVParams p{logp, qn1, qn2, v_pred, log_alpha, g_logp, g_qn1, qn2 ? g_qn2 : nullptr, g_v, info6, scratch, ticket,
+               B, fixed_alpha, reparameterization ? 1 : 0};
+  sac_v_loss_kernel<<<off_blocks(B), kOffThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("sac_v_loss_kernel");
 }
 
 TRL_API int trl_twin_mse_loss(const float* q1, const float* q2, const float* y, int64_t B, float* g1, float* g2,

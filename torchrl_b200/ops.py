@@ -428,6 +428,23 @@ def sac_policy_loss(logp, q1, q2, log_alpha, scratch, info=None, fixed_alpha=1.0
     return g_lp, g1, g2, info
 
 
+def sac_v_loss(logp, qn1, qn2, v_pred, log_alpha, scratch, reparameterization=True, info=None, fixed_alpha=1.0):
+    """SAC / TwinSAC with a V network (sac.py:128-144, twin_sac.py:138-156) in one launch: value target
+    min(qn1, qn2) - alpha*logpi (qn2 None: one critic), mean squared value error and the policy loss, with the
+    gradients wrt logp, qn1, qn2 and v_pred.  info = [policy_loss, vf_loss, logp mean/std/max/min]."""
+    B = logp.numel()
+    g_lp, g1, g_v = torch.empty_like(logp), torch.empty_like(qn1), torch.empty_like(v_pred)
+    g2 = torch.empty_like(qn2) if qn2 is not None else None
+    if info is None:
+        info = torch.zeros(6, dtype=F32, device=logp.device)
+    _lib.call("trl_sac_v_loss", _chk(logp, F32, "logp"), _chk(qn1, F32, "qn1"), _opt(qn2, F32, "qn2"),
+              _chk(v_pred, F32, "v_pred"), _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha),
+              int(bool(reparameterization)), B, _chk(g_lp, F32, "g_logp"), _chk(g1, F32, "g_qn1"),
+              _opt(g2, F32, "g_qn2"), _chk(g_v, F32, "g_v"), _chk(info, F32, "info"), scratch.buf[2].data_ptr(),
+              scratch.t(5), _stream())
+    return g_lp, g1, g2, g_v, info
+
+
 def twin_mse_loss(q1, q2, y, scratch, info=None):
     """MSE of one or two critics against y: losses in info[0:2], gradients returned (twin_sac_q.py:142-143)."""
     B = q1.numel()
