@@ -260,7 +260,8 @@ def per_sample(prio, size, u, beta):
     is the PUBLISHED algorithm -- Schaul, Quan, Antonoglou, Silver, "Prioritized Experience Replay", ICLR 2016
     (arXiv:1511.05952), proportional variant -- at this buffer's sampling granularity (one priority per time row):
       * eq. (1): P(i) = p_i^alpha / sum_k p_k^alpha            (`prio` already holds p_i^alpha, see per_update)
-      * sec. 3.4: w_i = (N * P(i))^-beta, normalised by max_i w_i = (N * min_k P(k))^-beta
+      * sec. 3.4: w_i = (N * P(i))^-beta, normalised by max_i w_i = (N * min_k P(k))^-beta (over the rows with
+        P(k) > 0, the only ones that can be drawn)
       * appendix B.2.1: "to sample a minibatch of size k, the range [0, p_total] is divided equally into k ranges;
         next, a value is uniformly sampled from each range": target_k = (k + u_k) / b * p_total, and the row whose
         cumulative priority interval contains the target is retrieved (their sum-tree walk == searchsorted on the
@@ -274,8 +275,12 @@ def per_sample(prio, size, u, beta):
     b = len(u)
     target = (np.arange(b, dtype=np.float64) + np.asarray(u, dtype=np.float64)) / b * total
     idx = np.searchsorted(pre, target, side="right")
-    idx = np.minimum(idx, size - 1)
-    max_w = (size * p.min() / total) ** (-beta)
+    # a target that rounds up to the total ((b-1+u)/b == 1 for u within 2^-53 of 1) finds no row: it draws the last
+    # row with a positive priority (a zero-priority row has probability 0 and is never drawn)
+    positive = np.flatnonzero(p > 0)
+    assert positive.size, "per_sample needs at least one row with a positive priority (all %d are zero)" % size
+    idx = np.minimum(idx, positive[-1])
+    max_w = (size * p[positive].min() / total) ** (-beta)
     w = (size * p[idx] / total) ** (-beta) / max_w
     return idx.astype(np.int64), w
 

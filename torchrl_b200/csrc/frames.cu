@@ -35,23 +35,44 @@ struct FrameWriteParams {
   int C, T, frame;                     // frame = which of the C frames to store (C-1: the newest)
 };
 
-// grid = (chunks, N): a CTA copies a 16-byte-aligned slice of one env's frame
+// hist slot of the frame m steps older than the oldest ring row, after `hc` history pushes (the gather's indexing)
+__device__ __forceinline__ long long frame_hist_slot(int hc, int m, int C) {
+  return ((static_cast<long long>(hc) - m) % (C - 1) + (C - 1)) % (C - 1);
+}
+
+// grid = (chunks, min(N, 65535)): a CTA copies a 16-byte-aligned slice of the frames of envs y, y + gridDim.y, ...
 __global__ void __launch_bounds__(kFrameThreads) frame_ring_write_kernel(const FrameWriteParams p) {
-  const long long n = blockIdx.y;
   const int row = *p.top;
-  const bool full = p.hist && (*p.size >= p.T);
-  const uint8_t* src = p.stack + (n * p.C + p.frame) * p.F;
-  uint8_t* dst = p.ring + (static_cast<long long>(row) * p.N + n) * p.F;
-  uint8_t* old = full ? p.hist + ((static_cast<long long>(*p.hist_count) % (p.C - 1)) * p.N + n) * p.F : nullptr;
+  const int size = p.hist ? *p.size : 0;
+  const bool full = p.hist && size >= p.T;
+  // the first write into an empty ring: the row's older frames precede the ring, and the gather reads them from the
+  // history (row 0 of a mid-episode stack), so the frames older than `frame` in this stack are seeded into the slots
+  // the gather reads them from -- the frame d steps back at frame_hist_slot(hc, d)
+  const bool seed = p.hist && size == 0;
+  const int hc = p.hist ? *p.hist_count : 0;
   const long long v16 = p.F / 16;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < v16;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    if (full) reinterpret_cast<uint4*>(old)[i] = reinterpret_cast<const uint4*>(dst)[i];
-    reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && p.age_ring) {
-    const int e = p.elapsed[n];
-    p.age_ring[static_cast<long long>(row) * p.N + n] = static_cast<uint8_t>(e < p.C - 1 ? e : p.C - 1);
+  for (long long n = blockIdx.y; n < p.N; n += gridDim.y) {
+    const uint8_t* src = p.stack + (n * p.C + p.frame) * p.F;
+    uint8_t* dst = p.ring + (static_cast<long long>(row) * p.N + n) * p.F;
+    uint8_t* old = full ? p.hist + ((static_cast<long long>(hc) % (p.C - 1)) * p.N + n) * p.F : nullptr;
+    for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < v16;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+      if (full) reinterpret_cast<uint4*>(old)[i] = reinterpret_cast<const uint4*>(dst)[i];
+      reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
+    }
+    if (seed) {
+      for (int d = 1; d <= p.frame && d < p.C; ++d) {
+        const uint4* s = reinterpret_cast<const uint4*>(p.stack + (n * p.C + p.frame - d) * p.F);
+        uint4* h = reinterpret_cast<uint4*>(p.hist + (frame_hist_slot(hc, d, p.C) * p.N + n) * p.F);
+        for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < v16;
+             i += static_cast<long long>(gridDim.x) * blockDim.x)
+          h[i] = s[i];
+      }
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0 && p.age_ring) {
+      const int e = p.elapsed[n];
+      p.age_ring[static_cast<long long>(row) * p.N + n] = static_cast<uint8_t>(e < p.C - 1 ? e : p.C - 1);
+    }
   }
 }
 
@@ -76,9 +97,8 @@ struct FrameGatherParams {
   float scale;
 };
 
-// grid = (chunks, rows*N): CTA (c, s) rebuilds a slice of both stacks of sample s = k*N + n
-__global__ void __launch_bounds__(kFrameThreads) frame_stack_gather_kernel(const FrameGatherParams p) {
-  const long long s = blockIdx.y;
+// CTA x's slice of both stacks of sample s = k*N + n
+__device__ __forceinline__ void frame_stack_gather_one(const FrameGatherParams& p, const long long s) {
   const int k = static_cast<int>(s / p.N);
   const long long n = s % p.N;
   const int r = static_cast<int>(p.idx[(p.pos ? static_cast<long long>(*p.pos) * p.rows : 0) + k]);
@@ -100,7 +120,7 @@ __global__ void __launch_bounds__(kFrameThreads) frame_stack_gather_kernel(const
         src = p.obs_last + (static_cast<long long>((r - d + p.T) % p.T) * p.N + n) * p.F;
       } else {                               // overwritten by the ring: the (d - back)-th newest history entry
         const int m = d - back;
-        src = p.hist + ((static_cast<long long>(hc - m) % (p.C - 1) + (p.C - 1)) % (p.C - 1) * p.N + n) * p.F;
+        src = p.hist + (frame_hist_slot(hc, m, p.C) * p.N + n) * p.F;
       }
     }
     float* o1 = j < p.C ? p.out_obs + (s * p.C + j) * p.F : nullptr;
@@ -116,12 +136,21 @@ __global__ void __launch_bounds__(kFrameThreads) frame_stack_gather_kernel(const
   }
 }
 
+// grid = (chunks, min(rows*N, 65535)): CTA (x, y) rebuilds its slice of the samples y, y + gridDim.y, ... (grid y is
+// limited to 65535, a batch of samples is not)
+__global__ void __launch_bounds__(kFrameThreads) frame_stack_gather_kernel(const FrameGatherParams p) {
+  const long long samples = static_cast<long long>(p.rows) * p.N;
+  for (long long s = blockIdx.y; s < samples; s += gridDim.y) frame_stack_gather_one(p, s);
+}
+
 }  // namespace trl
 
 // Store frame `frame` (0-based; C-1 = newest) of every env's (N, C, F) uint8 stack at ring row *top.  age_ring /
 // elapsed (both or neither): also record min(elapsed, C-1).  hist / hist_count / size (all or none): when the ring is
 // full the overwritten frame is pushed into the (C-1)-deep history first; call trl_frame_hist_advance once per step
-// after all writes of that step.  F % 16 == 0, 16-byte aligned buffers.
+// after all writes of that step.  When the ring is empty (*size == 0) the stack's frames older than `frame` are
+// seeded into the history, so a first row recorded mid-episode (age > 0) rebuilds its real older frames.  F % 16 == 0,
+// 16-byte aligned buffers.
 TRL_API int trl_frame_ring_write(const uint8_t* stack, uint8_t* ring, uint8_t* age_ring, const int* elapsed, uint8_t* hist,
                                  int* hist_count, const int* top, const int* size, int64_t N, int C, int64_t F, int T,
                                  int frame, void* stream) {
@@ -135,7 +164,8 @@ TRL_API int trl_frame_ring_write(const uint8_t* stack, uint8_t* ring, uint8_t* a
   TRL_REQUIRE(aligned16(stack) && aligned16(ring) && aligned16(hist), "trl_frame_ring_write: buffers must be 16-byte aligned");
   FrameWriteParams p{stack, ring, age_ring, elapsed, hist, hist_count, top, size, N, F, C, T, frame};
   const unsigned chunks = static_cast<unsigned>(ceil_div<long long>(F / 16, kFrameThreads) < 4 ? ceil_div<long long>(F / 16, kFrameThreads) : 4);
-  frame_ring_write_kernel<<<dim3(chunks, static_cast<unsigned>(N)), kFrameThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  frame_ring_write_kernel<<<dim3(chunks, static_cast<unsigned>(N < 65535 ? N : 65535)), kFrameThreads, 0,
+                            static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("frame_ring_write_kernel");
 }
 
@@ -163,7 +193,9 @@ TRL_API int trl_frame_stack_gather(const uint8_t* obs_last, const uint8_t* next_
                       out_obs, out_next, N, F, C, T, rows, scale};
   long long chunks = ceil_div<long long>(F / 4, 4LL * kFrameThreads);
   if (chunks < 1) chunks = 1;
-  frame_stack_gather_kernel<<<dim3(static_cast<unsigned>(chunks), static_cast<unsigned>(rows * N)), kFrameThreads, 0,
+  const long long samples = static_cast<long long>(rows) * N;
+  const unsigned grid_samples = samples < 65535 ? static_cast<unsigned>(samples) : 65535u;
+  frame_stack_gather_kernel<<<dim3(static_cast<unsigned>(chunks), grid_samples), kFrameThreads, 0,
                               static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("frame_stack_gather_kernel");
 }

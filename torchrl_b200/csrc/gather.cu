@@ -42,28 +42,30 @@ __device__ __forceinline__ void copy_units(const char* s, char* d, long long nby
   for (long long i = tid; i < n; i += nthr) dv[i] = sv[i];
 }
 
-// grid = (chunks_per_row, rows, nkeys); each CTA copies one chunk of one row of one key
+// grid = (chunks_per_row, min(rows, 65535), nkeys); each CTA copies one chunk of rows blockIdx.y, blockIdx.y +
+// gridDim.y, ... of one key (grid y is limited to 65535, a batch of rows is not)
 __global__ void __launch_bounds__(256) row_copy_kernel(const RowCopyParams p) {
-  const int key = blockIdx.z, k = blockIdx.y;
-  long long r;
-  if (p.row_ptr) r = *p.row_ptr;
-  else if (p.idx) r = p.idx[(p.pos_ptr ? static_cast<long long>(*p.pos_ptr) * p.rows : 0) + k];
-  else r = k;
+  const int key = blockIdx.z;
   const long long rb = p.row_bytes[key];
-  const long long srow = p.scatter ? k : r, drow = p.scatter ? r : k;
-  const char* s = p.src[key] + srow * rb;
-  char* d = p.dst[key] + drow * rb;
   // chunking: split the row over gridDim.x CTAs in 16B-aligned pieces
   long long per = ceil_div<long long>(rb, gridDim.x);
   per = (per + 15) & ~15LL;
   const long long lo = per * blockIdx.x;
-  if (lo < rb) {
-    const long long len = min(per, rb - lo);
-    s += lo; d += lo;
-    const uintptr_t al = reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(d) | static_cast<uintptr_t>(len);
-    if ((al & 15) == 0) copy_units<uint4>(s, d, len, threadIdx.x, blockDim.x);
-    else if ((al & 3) == 0) copy_units<unsigned>(s, d, len, threadIdx.x, blockDim.x);
-    else copy_units<unsigned char>(s, d, len, threadIdx.x, blockDim.x);
+  for (long long k = blockIdx.y; k < p.rows; k += gridDim.y) {
+    long long r;
+    if (p.row_ptr) r = *p.row_ptr;
+    else if (p.idx) r = p.idx[(p.pos_ptr ? static_cast<long long>(*p.pos_ptr) * p.rows : 0) + k];
+    else r = k;
+    const long long srow = p.scatter ? k : r, drow = p.scatter ? r : k;
+    if (lo < rb) {
+      const long long len = min(per, rb - lo);
+      const char* s = p.src[key] + srow * rb + lo;
+      char* d = p.dst[key] + drow * rb + lo;
+      const uintptr_t al = reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(d) | static_cast<uintptr_t>(len);
+      if ((al & 15) == 0) copy_units<uint4>(s, d, len, threadIdx.x, blockDim.x);
+      else if ((al & 3) == 0) copy_units<unsigned>(s, d, len, threadIdx.x, blockDim.x);
+      else copy_units<unsigned char>(s, d, len, threadIdx.x, blockDim.x);
+    }
   }
   if (p.adv_ptr) {
     // every CTA has read *row_ptr by now; the last one to arrive advances it (one launch instead of copy + advance)
@@ -190,7 +192,8 @@ static int launch_row_copy(int nkeys, const void* const* src, void* const* dst, 
   long long chunks = ceil_div<long long>(max_rb, 16384);
   const long long cap = ceil_div<long long>(8LL * kNumSM, static_cast<long long>(rows) * nkeys);
   if (chunks > cap) chunks = cap < 1 ? 1 : cap;
-  row_copy_kernel<<<dim3(static_cast<unsigned>(chunks), rows, nkeys), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  const unsigned grid_rows = rows < 65535 ? static_cast<unsigned>(rows) : 65535u;
+  row_copy_kernel<<<dim3(static_cast<unsigned>(chunks), grid_rows, nkeys), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("row_copy_kernel");
 }
 

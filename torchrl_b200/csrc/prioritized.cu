@@ -7,11 +7,19 @@
 //     (/root/reference/torchrl/replay_buffers/base.py:39-51): one priority per stored row,
 //     p_row = (mean_n |TD_{row,n}| + eps)^alpha, new rows enter with the running maximum priority;
 //   * stratified proportional sampling (Schaul et al. 2016): segment k of b draws
-//     target = (k + u_k)/b * sum(p), u_k ~ U[0,1) supplied by the caller (host np.random for parity,
-//     so indices are bit-exact vs the oracle), idx_k = first row whose inclusive prefix sum > target;
-//   * importance weights w_k = (size * p_idx/sum)^-beta / max_w, max_w from the minimum priority.
-// One CTA: block-wide inclusive scan of <= 4096 priorities in shared memory (fp64 accumulation so the
-// prefix is exactly reproducible by the NumPy oracle), then one binary search per drawn row.
+//     target = (k + u_k)/b * sum(p), u_k ~ U[0,1) supplied by the caller (host np.random),
+//     idx_k = first row whose inclusive prefix sum > target; a target that rounds up to the total (k = b-1, u_k
+//     within 2^-53 of 1) draws the last row with a positive priority -- a zero-priority row is never drawn;
+//   * importance weights w_k = (size * p_idx/sum)^-beta / max_w, max_w from the minimum positive priority;
+//   * at least one of the `size` priorities must be positive (all zero: the sum is 0 and the weights are NaN;
+//     the oracle refuses the case).
+// One CTA: block-wide inclusive scan of <= 4096 priorities in shared memory (fp64 accumulation), then one
+// binary search per drawn row.  The scan adds in its own order (per-thread runs, a warp scan, a scan across
+// warps), not np.cumsum's sequential one.  The two prefixes are equal -- and the indices bit-exact vs the
+// oracle -- whenever every partial sum is exact in fp64, e.g. when all priorities are integer multiples
+// of one 2^-q and their total is below 2^(53-q).  Otherwise (priorities over a wide exponent range) the
+// prefixes may differ in the last bits, and a drawn row may differ from the oracle's when its target lies
+// within that rounding of a row boundary.
 #include "common.cuh"
 
 namespace trl {
@@ -41,7 +49,7 @@ __global__ void __launch_bounds__(kPerThreads) per_sample_kernel(const PerSample
     const float v = p.prio[i];
     local += static_cast<double>(v);
     pre[i] = local;                                            // thread-local inclusive prefix
-    mn = fminf(mn, v);
+    if (v > 0.f) mn = fminf(mn, v);                            // zero rows are never drawn: no weight to normalise
   }
   // exclusive scan of the per-thread totals: warp shuffle, then across warps
   double incl = local;
@@ -81,6 +89,11 @@ __global__ void __launch_bounds__(kPerThreads) per_sample_kernel(const PerSample
       const int m = (a + c) >> 1;
       if (pre[m] > target) c = m; else a = m + 1;
     }
+    // a zero-priority row here is a target at (or rounded past) a boundary: the search fell through to size-1
+    // (target == total), or the scan's rounding stepped up at a zero row starting a thread's run.  Take the next
+    // row with a positive priority, else the last one before it.
+    while (a < p.size - 1 && !(p.prio[a] > 0.f)) ++a;
+    while (a > 0 && !(p.prio[a] > 0.f)) --a;
     p.idx[k] = a;
     const double prob = static_cast<double>(p.prio[a]) / total;
     p.weights[k] = static_cast<float>(pow(static_cast<double>(p.size) * prob, -static_cast<double>(p.beta)) / max_w);
