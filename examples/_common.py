@@ -28,7 +28,8 @@ class Run:
         name = args.id if args.id is not None else osp.splitext(osp.basename(args.config))[0]
         self.logger = Logger(name, params["env_name"], args.seed, params, args.log_dir, args.overwrite)
         self.obs_dim = self.env.observation_space.shape[0]
-        self.act_dim = self.env.action_space.shape[0]
+        space = self.env.action_space
+        self.act_dim = space.n if hasattr(space, "n") else space.shape[0]     # discrete: the number of actions
 
     def seed_everything(self, seed):
         self.env.seed(seed)

@@ -214,6 +214,25 @@ int trl_qr_dqn_loss(const float* pred, const float* next, const float* actions, 
                     float gamma, float kappa, int mse, float* grad, float* td_out, float* info3, double* scratch,
                     unsigned* ticket, void* stream);   /* weights / td_out: prioritised replay (may be NULL) */
 
+/* ---- Bootstrapped DQN (csrc/bootstrapped.cu): BootstrappedDQN.update (algo/off_policy/bootstrapped_dqn.py:66-113).
+ * pred / next (H, B, A): all heads of the network and of its target; actions (B) as float; masks (B, H) uint8.
+ * Per head y_h = r + gamma*(1-d)*max_a' next[h, b, a'];  loss = sum_{b,h} m_bh (pred[h, b, a_b] - y_h)^2 / (H B).
+ * grad (H, B, A) is written completely: 2 m_bh (pred - y_h) / (H B) at the taken action, 0 elsewhere.
+ * info3 = [loss, mean over (b, h) of pred[h, b, a_b], mean reward].  scratch: trl_offpolicy_scratch_doubles(B). */
+int trl_bootstrapped_dqn_loss(const float* pred, const float* next, const float* actions, const float* rewards,
+                              const uint8_t* terminals, const uint8_t* masks, int64_t B, int num_heads,
+                              int num_actions, float gamma, float* grad, float* info3, double* scratch,
+                              unsigned* ticket, void* stream);
+/* The collector's per-step decision for N envs (bootstrapped_dqn.py:22-62, policies/discrete_policies.py:92-115):
+ * where current_step[n] == 0 a new head[n] = min(floor(u * H), H - 1); action[n] = the first argmax_a of
+ * q_all[head[n], n, a] (q_all (H, N, A)); masks_ring[*top, n, j] = (u_j < bernoulli_p) -- no other ring row is touched.
+ * Uniforms: u_head (N) and u_mask (N, H), or (both NULL) Philox4x32-10 keyed by (seed, *rng_counter, n); then the call
+ * itself advances *rng_counter by one (ticket: a zero-initialised uint32 the caller owns). */
+int trl_bootstrapped_act(const float* q_all, const int* current_step, int* head, float* action, uint8_t* masks_ring,
+                         const int* top, const float* u_head, const float* u_mask, uint64_t seed,
+                         uint64_t* rng_counter, unsigned* ticket, int64_t N, int num_heads, int num_actions,
+                         float bernoulli_p, void* stream);
+
 /* ---- MLP epilogues around the cuBLAS GEMMs of MLPBase (networks/base.py:24-44): z <- act(z + b) in place
  * (act: 0 none, 1 tanh, 2 relu) and its backward g_pre = g * act'(out), dbias = column sums (one launch each). */
 int64_t trl_bias_act_bwd_scratch_floats(int64_t M, int H);

@@ -116,6 +116,8 @@ SIGNATURES = {
     "trl_sac_v_loss": [vp, vp, vp, vp, vp, f32, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp],
     "trl_twin_mse_loss": [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp],
     "trl_qr_dqn_loss": [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
+    "trl_bootstrapped_dqn_loss": [vp, vp, vp, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp],
+    "trl_bootstrapped_act": [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, vp, i64, i32, i32, f32, vp],
 }
 _RESTYPES = {"trl_last_error": ctypes.c_char_p, "trl_ppo_actor_scratch_doubles": ctypes.c_int64,
              "trl_ppo_categorical_actor_scratch_doubles": ctypes.c_int64,

@@ -170,7 +170,7 @@ class OffRLAlgo(RLAlgo):
         for k in self.sample_key:
             v = batch[k]
             v = torch.as_tensor(np.asarray(v)) if not torch.is_tensor(v) else v
-            dt = torch.uint8 if k == "terminals" else torch.float32
+            dt = torch.uint8 if k in ("terminals", "masks") else torch.float32   # masks: Bootstrapped DQN
             conv[k] = v.to(device=dev, dtype=dt).contiguous()
         self.training_update_num += 1
         variant = self._variant()

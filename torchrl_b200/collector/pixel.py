@@ -4,7 +4,10 @@
 Off-policy step (one captured CUDA graph): ring write obs[t] <- frames | u8->f32 scale | epsilon-greedy Q policy |
 env step (frame-stack shift + render, in place) | ring write next_obs[t] <- frames | scalar finalize
 (acts / rewards / terminals / time_limits rows, episode returns, timeout + done -> reset mask) | re-render
-the reset envs | ring advance.  `epsilon` lives in a device scalar refreshed from the host schedule.
+the reset envs | ring advance.  `epsilon` lives in a device scalar refreshed from the host schedule.  With a
+BootstrappedDQNDiscretePolicy the epsilon-greedy stage is the all-heads forward plus one trl_bootstrapped_act launch
+(per-env heads redrawn at episode starts, greedy actions, the transition's bootstrap mask row in the `masks` ring key)
+and there is no epsilon schedule.
 
 On-policy step (PixelVecOnPolicyCollector, the VecOnPolicyCollector of a pixel env,
 /root/reference/torchrl/collector/on_policy.py:94-153): the same graph with V(obs) on a side stream, the policy's
@@ -17,6 +20,7 @@ import torch
 
 from .. import _lib, ops
 from ..policies import distribution as D
+from ..policies.discrete_policies import BootstrappedDQNDiscretePolicy
 from .base import VecCollector
 
 F32, F64, U8, I32 = torch.float32, torch.float64, torch.uint8, torch.int32
@@ -37,6 +41,10 @@ class PixelVecCollector(VecCollector):
         keys = [("acts", (N,), F32), ("rewards", (N, 1), F32), ("terminals", (N, 1), U8), ("time_limits", (N, 1), U8)]
         if self.on_policy:
             keys.append(("values", (N, 1), F32))
+        # Bootstrapped DQN: one Bernoulli mask over the heads per transition, written by the policy's act launch
+        self._boot = isinstance(self.pf, BootstrappedDQNDiscretePolicy)
+        if self._boot:
+            keys.append(("masks", (N, self.pf.head_num), U8))
         assert not (self.on_policy and self._dedup), "the on-policy pixel collector stores full frame stacks"
         if self._dedup:
             # frame-de-duplicated ring (replay_buffers/memory_efficient.py): one frame of obs and one of next_obs per
@@ -61,6 +69,8 @@ class PixelVecCollector(VecCollector):
         if not self._dedup:
             self._plan_obs = ops.RowCopyPlan([self.env.obs.view(1, -1)], [rb._obs], [ops.row_bytes_of(rb._obs)])
             self._plan_next = ops.RowCopyPlan([self.env.obs.view(1, -1)], [rb._next_obs], [ops.row_bytes_of(rb._next_obs)])
+        if self._boot:
+            self.pf.ensure_heads(N, dev)
         self._eps_dev = torch.zeros(1, dtype=F32, device=dev)
         self._eps_host = torch.zeros(1, dtype=F32).pin_memory()
 
@@ -84,6 +94,8 @@ class PixelVecCollector(VecCollector):
                 with torch.cuda.stream(side):
                     self._value.copy_(self.vf(self._obs_f).reshape(-1))
                 self.pf.act_only(self._obs_f, action_out=self._act, nan_flag=self._nan_flag)
+            elif self._boot:
+                self.pf.act(self._obs_f, self.current_step, self._act, rb._masks, rb._top_dev)
             else:
                 out = self.pf.explore(self._obs_f.unsqueeze(0), epsilon=self._eps_dev)
                 self._act.copy_(out["action"].reshape(self._act.shape).to(F32))
@@ -121,7 +133,7 @@ class PixelVecCollector(VecCollector):
 
     def _step(self):
         boot = self.on_policy
-        if not self.on_policy:
+        if not (self.on_policy or self._boot):
             self.pf.tick()                               # host-side epsilon schedule -> device scalar
             self._eps_host[0] = float(self.pf.epsilon)
             self._eps_dev.copy_(self._eps_host, non_blocking=True)

@@ -90,6 +90,11 @@ class BootstrappedNet(nn.Module):
         feature = self.base(x)
         return [self.bootstrapped_heads[i](feature) for i in head_idxs]
 
+    def all_heads(self, x):
+        """Every head on one trunk pass, as one contiguous (head_num, M, output_shape) tensor."""
+        feature = self.base(x)
+        return torch.stack([head(feature) for head in self.bootstrapped_heads])
+
 
 class FlattenBootstrappedNet(BootstrappedNet):
     def forward(self, input, head_idxs):

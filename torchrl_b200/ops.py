@@ -474,6 +474,41 @@ def qr_dqn_loss(pred, nxt, actions, rewards, terminals, gamma, scratch, n_action
     return grad, info
 
 
+def bootstrapped_dqn_loss(pred, nxt, actions, rewards, terminals, masks, gamma, scratch, info=None, grad=None):
+    """Masked multi-head TD loss of Bootstrapped DQN (bootstrapped_dqn.py:66-113) in one launch: pred / nxt (H, B, A),
+    masks (B, H) uint8.  Returns d loss / d pred (H, B, A) and info = [loss, mean q_s_a over (b, h), mean reward]."""
+    H, B, A = pred.shape
+    assert nxt.shape == pred.shape and masks.shape == (B, H) and rewards.numel() == B and scratch.B >= B
+    if grad is None:
+        grad = torch.empty_like(pred)
+    if info is None:
+        info = torch.zeros(3, dtype=F32, device=pred.device)
+    _lib.call("trl_bootstrapped_dqn_loss", _chk(pred, F32, "pred"), _chk(nxt, F32, "next"),
+              _chk(actions, F32, "actions"), _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"),
+              _chk(masks, U8, "masks"), B, H, A, float(gamma), _chk(grad, F32, "grad"), _chk(info, F32, "info"),
+              scratch.buf[4].data_ptr(), scratch.t(4), _stream())
+    return grad, info
+
+
+def bootstrapped_act(q_all, current_step, head, action, masks_ring, top, bernoulli_p, u_head=None, u_mask=None,
+                     rng=None, ticket=None):
+    """Per-env head / greedy action / bootstrap mask row of one collector step (csrc/bootstrapped.cu): q_all (H, N, A);
+    new heads where current_step == 0; masks_ring (T, N, H) row *top written.  Uniforms u_head (N) and u_mask (N, H),
+    or Philox keyed by (rng.seed, rng.counter), which the launch advances (ticket: zeroed int32[1])."""
+    H, N, A = q_all.shape
+    assert masks_ring.shape[1:] == (N, H)
+    seed, ctr = 0, None
+    if u_head is None:
+        if rng is None or rng.counter is None or ticket is None:
+            raise ValueError("bootstrapped_act needs u_head / u_mask or an rng state and a ticket")
+        seed, ctr = rng.seed, rng.counter
+    _lib.call("trl_bootstrapped_act", _chk(q_all, F32, "q_all"), _chk(current_step, I32, "current_step"),
+              _chk(head, I32, "head"), _chk(action, F32, "action"), _chk(masks_ring, U8, "masks_ring"),
+              _chk(top, I32, "top"), _opt(u_head, F32, "u_head"), _opt(u_mask, F32, "u_mask"), ctypes.c_uint64(seed),
+              _opt(ctr, I64, "rng_counter"), _opt(ticket, I32, "ticket"), N, H, A, float(bernoulli_p), _stream())
+    return action
+
+
 # ------------------------------------------------------------------------------------------ K9 prioritised
 def per_sample(prio, size, u, beta, idx=None, weights=None):
     """Stratified proportional row sampling + importance weights (csrc/prioritized.cu; parity unpinned)."""

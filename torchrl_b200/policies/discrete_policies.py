@@ -103,6 +103,77 @@ class EpsilonGreedyQRDQNDiscretePolicy(EpsilonGreedyDQNDiscretePolicy):
         return q.mean(dim=-1).max(dim=-1, keepdim=True)[1].detach()
 
 
+class BootstrappedDQNDiscretePolicy:
+    """Greedy actions of one bootstrapped head per env (discrete_policies.py:92-121), batched over envs.  `head` is the
+    (N,) int32 device vector of the envs' current heads (the reference's scalar `idx`, one per env).  The collector's
+    captured step calls `act`: all heads in one forward, then one launch (csrc/bootstrapped.cu) that redraws the heads
+    of envs starting an episode, picks the greedy actions and writes the transition's Bernoulli(`bernoulli_p`) mask
+    row.  Not an nn.Module, like in the reference: `to` / `parameters` forward to the wrapped network."""
+
+    def __init__(self, qf, head_num, action_shape):
+        self.qf = qf
+        self.head_num = head_num
+        self.action_shape = action_shape
+        self.bernoulli_p = 0.5                 # BootstrappedDQN hands its own value over
+        self.head = None
+        self.continuous = False
+        self._rng = _DeviceRng()
+        self._ticket = None
+
+    def ensure_heads(self, n, device):
+        """Allocate the (n,) head vector (all head 0) if it does not exist yet; returns it."""
+        if self.head is None or self.head.numel() != n or self.head.device != torch.device(device):
+            self.head = torch.zeros(n, dtype=torch.int32, device=device)
+        return self.head
+
+    def sample_head(self):
+        """A new uniform head for every env (the collector redraws them per env at each episode start)."""
+        if self.head is not None:
+            self.head.copy_(torch.randint(0, self.head_num, self.head.shape, device=self.head.device))
+
+    def set_head(self, idx):
+        """Every env to head `idx` (an int), or per env (an (N,) tensor)."""
+        if self.head is None:
+            raise RuntimeError("no per-env heads yet: the collector allocates them (ensure_heads)")
+        if torch.is_tensor(idx):
+            self.head.copy_(idx.to(self.head.device, torch.int32))
+        else:
+            self.head.fill_(int(idx))
+
+    def explore(self, x):
+        """The greedy action of each env's head for x (N, ...)."""
+        q = self.qf.all_heads(x)
+        head = self.ensure_heads(q.shape[1], q.device).long()
+        q_value = q[head, torch.arange(q.shape[1], device=q.device)]
+        return {"q_value": q_value, "action": q_value.max(dim=-1)[1].detach()}
+
+    def act(self, x, current_step, action_out, masks_ring, top, u_head=None, u_mask=None):
+        """The collector's per-step decision (capturable): see trl_bootstrapped_act.  u_head (N) and u_mask (N, H)
+        replace the Philox stream."""
+        q = self.qf.all_heads(x)
+        q = q if q.is_contiguous() else q.contiguous()
+        self.ensure_heads(q.shape[1], q.device)
+        rng = None
+        if u_head is None:
+            rng = self._rng.ensure(q.device)
+            if self._ticket is None:
+                self._ticket = torch.zeros(1, dtype=torch.int32, device=q.device)
+        return ops.bootstrapped_act(q.detach(), current_step, self.head, action_out.reshape(-1), masks_ring, top,
+                                    self.bernoulli_p, u_head=u_head, u_mask=u_mask, rng=rng, ticket=self._ticket)
+
+    def eval_act(self, x):
+        """argmax of the mean over all heads, per row."""
+        with torch.no_grad():
+            return self.qf.all_heads(x).mean(dim=0).max(dim=-1)[1].detach()
+
+    def to(self, device):
+        self.qf.to(device)
+        return self
+
+    def parameters(self):
+        return self.qf.parameters()
+
+
 class CategoricalDisPolicy(networks.Net):
     """softmax over the net's outputs (discrete_policies.py:123-160).  `forward` / `explore` / `update` / `eval_act`
     keep the reference's torch semantics; the collector's `act_only` and the on-policy algorithms' fused minibatch

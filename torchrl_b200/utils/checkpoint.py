@@ -19,6 +19,7 @@ _COLLECTOR_SCALARS = ("_host_step", "_host_steps")
 _ENV_SCALARS = ("_host_elapsed", "_host_mirror_ok", "training")
 _BUFFER_SCALARS = ("_top", "_size")
 _POLICY_SCALARS = ("count", "epsilon")                 # epsilon-greedy schedule position
+_POLICY_TENSORS = ("head",)                            # Bootstrapped DQN: the per-env heads
 _OPT_TENSORS = ("exp_avg", "exp_avg_sq", "step_counts", "lr_host", "lr")
 
 
@@ -61,6 +62,8 @@ def save_checkpoint(agent, path, include_replay=None):
     state["episode_rewards"] = list(agent.episode_rewards)
     state["training_episode_rewards"] = list(agent.training_episode_rewards)
     state["policy_scalars"] = _scalars(agent.pf, _POLICY_SCALARS)
+    state["policy_tensors"] = {k: v.detach().to("cpu", copy=True) for k, v in _scalars(agent.pf, _POLICY_TENSORS).items()
+                               if torch.is_tensor(v)}
     state["collector_tensors"] = _tensors(col)
     state["collector_scalars"] = _scalars(col, _COLLECTOR_SCALARS)
     state["env_tensors"] = _tensors(env)
@@ -121,6 +124,7 @@ def load_checkpoint(agent, path):
         if hasattr(rb, "_ensure_prio"):
             rb._ensure_prio()                          # prioritised ring: priorities exist before they are restored
         _restore(rb, state["buffer_tensors"], "buffer", dev)
+        _restore(agent.pf, state.get("policy_tensors", {}), "policy", dev)
     for f in (getattr(agent, "opt", None), getattr(agent, "_target_flat", None)):
         if f is not None and hasattr(f, "refresh_split"):
             f.refresh_split()                          # TF32 planes follow the restored weights
