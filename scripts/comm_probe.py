@@ -70,7 +70,7 @@ def main():
     red = torch.zeros(total, device=dev)
     s3 = torch.zeros(9, dtype=torch.float64, device=dev)
     step = torch.zeros(3, dtype=torch.int32, device=dev)
-    scr = torch.zeros(int(pc.lib.trl_comm_scratch_doubles(3)), dtype=torch.float64, device=dev)
+    scr = torch.zeros(int(_lib.load().trl_comm_scratch_doubles(3)), dtype=torch.float64, device=dev)
     tick = torch.zeros(1, dtype=torch.int32, device=dev)
     seg_c = (ctypes.c_int64 * 4)(*seg)
     g[:total] = 1.0 + ctx.rank

@@ -80,14 +80,14 @@ for K, N in ((17, 6), (17, 1), (23, 8)):
     gup = torch.randn(M, H, device=dev)
     yact = torch.tanh(torch.randn(M, H, device=dev))
     dW = torch.empty(H, K, device=dev); dbh = torch.empty(H, device=dev)
-    ws = fused._tn_scratch(M, H, K, torch.device(dev))
+    ws = fused._scratch("tn", torch.device(dev), M, H, K)
     f = lambda: _lib.call("trl_skinny_act_wgrad", gup.data_ptr(), yact.data_ptr(), x.data_ptr(), dW.data_ptr(), dbh.data_ptr(), M, H, K, 1, ws.data_ptr(), st())
     f(); torch.cuda.synchronize()
     gzr = gup.double() * (1 - yact.double() ** 2)
 
     def sep():
         gz_ = torch.empty_like(gup); db_ = torch.empty(H, device=dev)
-        sc, tk = fused._Workspace.get(M, H, torch.device(dev))
+        sc, tk = fused._scratch("bias_act", torch.device(dev), M, H)
         _lib.call("trl_bias_act_bwd", gup.data_ptr(), yact.data_ptr(), gz_.data_ptr(), db_.data_ptr(), M, H, 1, sc.data_ptr(), tk.data_ptr(), st())
         fused.wgrad(gz_, x)
     print("act_wgrad K=%2d     err %.2e / db %.2e   fused %6.1f us   bias_act_bwd + wgrad %6.1f us" % (
@@ -102,7 +102,7 @@ for K, N in ((17, 6), (17, 1), (23, 8)):
     def sep2():
         dx_ = torch.mm(g, w2)
         gz_ = torch.empty_like(dx_); db_ = torch.empty(H, device=dev)
-        sc, tk = fused._Workspace.get(M, H, torch.device(dev))
+        sc, tk = fused._scratch("bias_act", torch.device(dev), M, H)
         _lib.call("trl_bias_act_bwd", dx_.data_ptr(), yact.data_ptr(), gz_.data_ptr(), db_.data_ptr(), M, H, 1, sc.data_ptr(), tk.data_ptr(), st())
     print("dgrad_act N=%d      err %.2e / db %.2e   fused %6.1f us   mm + bias_act_bwd %6.1f us" % (
         N, rel(gzo, refz), rel(dbh, refz.sum(0)), timeit(f), timeit(sep2)))

@@ -182,12 +182,12 @@ def add_launches(n):
     _LAUNCHES += int(n)
 
 
-def call(name, *args):
-    """Invoke a kernel-launching entry point and raise on error.  Counted as one launch (a few entry points launch a
-    second, small kernel: the count is a lower bound of the kernels launched)."""
+def call(name, *args, kernels=1):
+    """Invoke a kernel-launching entry point, raise on error and count the `kernels` kernels it launched (the
+    wrappers in ops.py know that number for each entry point and its arguments)."""
     global _LAUNCHES
     lib = load()
     rc = getattr(lib, name)(*args)
     if rc != 0:
         check(rc, name)
-    _LAUNCHES += 1
+    _LAUNCHES += kernels

@@ -11,7 +11,7 @@ import copy
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from ..env import synth_spec
 from ..networks import fused
 from ..policies import distribution as D
@@ -114,21 +114,16 @@ class VecCollector:
         env, rb = self.env, self.replay_buffer
         nrm = env._obs_normalizer if getattr(env, "obs_norm", False) else None
         ext = self._host_env            # host envs: the kernel stores rows / counters, the host env resets
-        _lib.call("trl_collect_finalize", self.current_ob.data_ptr(), env.obs_out.data_ptr(),
-                  None if ext else env.state.data_ptr(),
-                  self._act.data_ptr(), None if self._value is None else self._value.data_ptr(),
-                  None if v_next is None else v_next.data_ptr(), env.reward.data_ptr(), env.done.data_ptr(),
-                  env.time_limit.data_ptr(), None if ext else env.elapsed.data_ptr(),
-                  None if ext else env.episode.data_ptr(), None if ext else env.seeds.data_ptr(),
-                  self.current_step.data_ptr(), self.train_rew.data_ptr(), self._epoch_reward.data_ptr(),
-                  self._ret_log.data_ptr(), self._n_done.data_ptr(), None if ext else env.any_reset.data_ptr(),
-                  None if nrm is None else nrm._mean.data_ptr(), None if nrm is None else nrm._var.data_ptr(),
-                  self.current_ob.data_ptr(), rb._obs.data_ptr(), rb._next_obs.data_ptr(), rb._acts.data_ptr(),
-                  rb._values.data_ptr() if self.on_policy else None, rb._rewards.data_ptr(),
-                  rb._terminals.data_ptr(), rb._time_limits.data_ptr(), rb._top_dev.data_ptr(),
-                  self._N, self._o, self._a, int(self.max_episode_frames), float(getattr(self, "discount", 0.99)),
-                  float(synth_spec.INIT_SCALE), float(nrm.clip if nrm is not None else 10.0),
-                  1 if self.on_policy else 0, 1 if self.reference_quirks else 0, ops._stream())
+        ops.collect_finalize(self.current_ob, env.obs_out, None if ext else env.state, self._act, self._value, v_next,
+                             env.reward, env.done, env.time_limit, None if ext else env.elapsed,
+                             None if ext else env.episode, None if ext else env.seeds, self.current_step,
+                             self.train_rew, self._epoch_reward, self._ret_log, self._n_done,
+                             None if ext else env.any_reset, None if nrm is None else nrm._mean,
+                             None if nrm is None else nrm._var, self.current_ob, rb._obs, rb._next_obs, rb._acts,
+                             rb._values if self.on_policy else None, rb._rewards, rb._terminals, rb._time_limits,
+                             rb._top_dev, self.max_episode_frames, getattr(self, "discount", 0.99),
+                             synth_spec.INIT_SCALE, nrm.clip if nrm is not None else 10.0, self.on_policy,
+                             self.reference_quirks)
 
     def _step_body(self, bootstrap):
         with torch.no_grad():

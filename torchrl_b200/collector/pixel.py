@@ -18,7 +18,7 @@ rows cut by max_episode_frames, terminals include the cut).
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from ..policies import distribution as D
 from ..policies.discrete_policies import BootstrappedDQNDiscretePolicy
 from .base import VecCollector
@@ -109,18 +109,13 @@ class PixelVecCollector(VecCollector):
                 main.wait_stream(side)              # one value net, one set of per-stream scratch: V(obs) first
                 self._v_next.copy_(self.vf(env.to_float(env.obs, self._next_f)).reshape(-1))
                 v_next = self._v_next
-            _lib.call("trl_collect_finalize", self._d_ob.data_ptr(), self._d_ob.data_ptr(), self._d_state.data_ptr(),
-                      self._act.data_ptr(), None if self._value is None else self._value.data_ptr(),
-                      None if v_next is None else v_next.data_ptr(), env.reward.data_ptr(), env.done.data_ptr(),
-                      env.time_limit.data_ptr(), env.elapsed.data_ptr(), env.episode.data_ptr(), env.seeds.data_ptr(),
-                      self.current_step.data_ptr(), self.train_rew.data_ptr(), self._epoch_reward.data_ptr(),
-                      self._ret_log.data_ptr(), self._n_done.data_ptr(), None, None, None, self._d_ob.data_ptr(),
-                      self._d_rows.data_ptr(), self._d_rows.data_ptr(), rb._acts.data_ptr(),
-                      rb._values.data_ptr() if self.on_policy else None,
-                      rb._rewards.data_ptr(), rb._terminals.data_ptr(), rb._time_limits.data_ptr(),
-                      rb._top_dev.data_ptr(), self._N, 1, 1, int(self.max_episode_frames),
-                      float(getattr(self, "discount", 0.0)), 0.0, 10.0, 1 if self.on_policy else 0, 1,
-                      ops._stream())
+            ops.collect_finalize(self._d_ob, self._d_ob, self._d_state, self._act, self._value, v_next, env.reward,
+                                 env.done, env.time_limit, env.elapsed, env.episode, env.seeds, self.current_step,
+                                 self.train_rew, self._epoch_reward, self._ret_log, self._n_done, None, None, None,
+                                 self._d_ob, self._d_rows, self._d_rows, rb._acts,
+                                 rb._values if self.on_policy else None, rb._rewards, rb._terminals,
+                                 rb._time_limits, rb._top_dev, self.max_episode_frames,
+                                 getattr(self, "discount", 0.0), 0.0, 10.0, self.on_policy, True)
             # envs whose collector step counter was just zeroed need a fresh episode (done or timeout); the
             # finalize kernel already advanced their episode counter
             env._reset(zero_is_mask=self.current_step, episode_bias=1, bump=0)

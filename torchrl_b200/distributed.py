@@ -21,6 +21,8 @@ import os
 import torch
 import torch.distributed as dist
 
+from . import ops
+
 
 class _RawDeviceMemory:
     """__cuda_array_interface__ view of raw device memory (zero-copy into a torch tensor)."""
@@ -39,39 +41,23 @@ class PeerComm:
     BLOCK_BYTES = 8 << 20
 
     def __init__(self, ctx):
-        from . import _lib
         self.ctx = ctx
-        self.lib = _lib.load()
         self.rank, self.world = ctx.rank, ctx.world_size
         dev = ctx.device
-        base = ctypes.c_void_p()
-        _lib.check(self.lib.trl_comm_alloc(self.BLOCK_BYTES, ctypes.byref(base)), "trl_comm_alloc")
-        self.base = base.value
-        hb = int(self.lib.trl_comm_ipc_handle_bytes())
-        handle = ctypes.create_string_buffer(hb)
-        _lib.check(self.lib.trl_comm_ipc_get(base, handle), "trl_comm_ipc_get")
-        mine = torch.tensor(list(handle.raw), dtype=torch.uint8, device=dev)
+        self.base = ops.comm_alloc(self.BLOCK_BYTES)
+        mine = torch.tensor(list(ops.comm_ipc_get(self.base)), dtype=torch.uint8, device=dev)
         everyone = [torch.empty_like(mine) for _ in range(self.world)]
         dist.all_gather(everyone, mine)
-        self.bases = []
-        for r, h in enumerate(everyone):
-            if r == self.rank:
-                self.bases.append(self.base)
-                continue
-            raw = bytes(h.cpu().tolist())
-            ptr = ctypes.c_void_p()
-            _lib.check(self.lib.trl_comm_ipc_open(ctypes.create_string_buffer(raw, hb), ctypes.byref(ptr)),
-                       "trl_comm_ipc_open")
-            self.bases.append(ptr.value)
+        self.bases = [self.base if r == self.rank else ops.comm_ipc_open(bytes(h.cpu().tolist()))
+                      for r, h in enumerate(everyone)]
         self._whole = torch.as_tensor(_RawDeviceMemory(self.base, self.BLOCK_BYTES), device=dev)
-        self.flag_bytes = (int(self.lib.trl_comm_flag_bytes()) + 255) // 256 * 256
+        self.flag_bytes = (ops.comm_sizes()[0] + 255) // 256 * 256
         self._top = self.flag_bytes
         self.flag_ptrs = (ctypes.c_void_p * self.world)(*self.bases)
         self.seq = torch.zeros(1, dtype=torch.int32, device=dev)
         self.regions = {}
         # receive area of the flag-in-payload exchange of small fp64 vectors (all_reduce_f64), zero from trl_comm_alloc
-        self._ll_recv = self.region("__ll_recv__", int(self.lib.trl_comm_ll_recv_bytes(self.world, self.LL_NMAX)),
-                                    torch.uint8)[1]
+        self._ll_recv = self.region("__ll_recv__", ops.comm_ll_recv_bytes(self.world, self.LL_NMAX), torch.uint8)[1]
         self._ll_seq = torch.zeros(1, dtype=torch.int32, device=dev)
         torch.cuda.synchronize(dev)
         dist.barrier()                      # every rank has mapped every block before anyone launches on them
@@ -96,15 +82,11 @@ class PeerComm:
         """out = sum over ranks (or the (W, n) stack when gather) of the first n doubles of region `name`.  Up to
         LL_NMAX doubles travel as flag-carrying 16-byte packets pushed into the peers' receive areas (one NVLink
         traversal, no barrier phases: trl_allreduce_f64_ll); longer vectors take the two-phase pull kernel."""
-        from . import _lib, ops
         local, ptrs = self.regions[name]
         if int(n) <= self.LL_NMAX:
-            _lib.call("trl_allreduce_f64_ll", local.data_ptr(), self._ll_recv, self.rank, self.world, out.data_ptr(),
-                      int(n), self.LL_NMAX, int(bool(gather)), self._ll_seq.data_ptr(), ops._stream())
-            return out
-        _lib.call("trl_allreduce_f64", ptrs, self.flag_ptrs, self.rank, self.world, out.data_ptr(), int(n),
-                  int(bool(gather)), self.seq.data_ptr(), ops._stream())
-        return out
+            return ops.allreduce_f64_ll(local, self._ll_recv, self.rank, self.world, out, n, self.LL_NMAX, gather,
+                                        self._ll_seq)
+        return ops.allreduce_f64(ptrs, self.flag_ptrs, self.rank, self.world, out, n, gather, self.seq)
 
 
 def shard_range(total, world_size, rank):
@@ -190,14 +172,11 @@ class DataParallelContext:
             return 1.0, False
         if self.peer is None or getattr(opt, "_grad_region", None) is None:
             return self.all_reduce_grads(opt.grad), False
-        from . import _lib, ops
         pc = self.peer
         _, ptrs = pc.regions["flat_grad"]
         mask = opt.all_mask if active_mask is None else int(active_mask)
-        _lib.call("trl_allreduce_grad", ptrs, pc.flag_ptrs, pc.rank, pc.world, opt.reduced.data_ptr(), opt.total,
-                  opt._seg_c, opt.nseg, mask, opt.sumsq3.data_ptr(), opt.step_counts.data_ptr(), opt.betas[0],
-                  opt.betas[1], opt._comm_scratch.data_ptr(), opt._ticket.data_ptr(), pc.seq.data_ptr(), 1,
-                  ops._stream())
+        ops.allreduce_grad(ptrs, pc.flag_ptrs, pc.rank, pc.world, opt.reduced, opt._seg_c, opt.nseg, mask, opt.sumsq3,
+                           opt.step_counts, opt.betas, opt._comm_scratch, opt._ticket, pc.seq)
         return 1.0 / self.world_size, True
 
     def all_reduce_sum_(self, t):
@@ -215,25 +194,19 @@ class DataParallelContext:
         the same number of elements).  CUDA: one raw-moments launch, ONE all-gather of 4 doubles per rank, one
         combine launch (capturable).  CPU tensors (gloo tests): the same arithmetic in torch ops."""
         if x.is_cuda:
-            from . import _lib, ops
             if not hasattr(self, "_mom"):
                 self._mom = torch.zeros(4, dtype=torch.float64, device=x.device)
                 self._mom_all = torch.zeros(4 * self.world_size, dtype=torch.float64, device=x.device)
-            if self.active and self.peer is not None:
-                local, _ = self.peer.region("vec_moments", 32, torch.float64)
-                _lib.call("trl_vec_moments", ops._chk(x, torch.float32, "x"), x.numel(), local.data_ptr(), ops._stream())
-                self.peer.all_reduce_f64("vec_moments", 4, self._mom_all, gather=True)
-                _lib.call("trl_vec_stats_from_moments", self._mom_all.data_ptr(), self.world_size,
-                          float(x.numel() * self.world_size), ops._chk(out, torch.float32, "stats"), ops._stream())
-                return out
-            _lib.call("trl_vec_moments", ops._chk(x, torch.float32, "x"), x.numel(), self._mom.data_ptr(), ops._stream())
-            if self.active:
+            peer = self.peer if self.active else None
+            mom = peer.region("vec_moments", 32, torch.float64)[0] if peer is not None else self._mom
+            ops.vec_moments(x, mom)
+            if peer is not None:
+                peer.all_reduce_f64("vec_moments", 4, self._mom_all, gather=True)
+            elif self.active:
                 dist.all_gather_into_tensor(self._mom_all, self._mom)
             else:
                 self._mom_all.copy_(self._mom)
-            _lib.call("trl_vec_stats_from_moments", self._mom_all.data_ptr(), self.world_size,
-                      float(x.numel() * self.world_size), ops._chk(out, torch.float32, "stats"), ops._stream())
-            return out
+            return ops.vec_stats_from_moments(self._mom_all, self.world_size, x.numel() * self.world_size, out)
         xd = x.double()
         mom = torch.stack([xd.sum(), (xd * xd).sum()])
         ext = torch.stack([x.max(), -x.min()]).double()

@@ -11,7 +11,7 @@ import copy
 import numpy as np
 import torch
 
-from .. import ops, _lib
+from .. import ops
 from ..spaces import Box
 from . import synth_spec as spec
 
@@ -123,8 +123,7 @@ class SynthVecEnv:
         self.done = torch.zeros(N, dtype=U8, device=dev)
         self.time_limit = torch.zeros(N, dtype=U8, device=dev)
         self.obs_out = torch.zeros(N, o, dtype=F32, device=dev)     # what step() returns (normalised if obs_norm)
-        lib = _lib.load()
-        self._nblk = int(lib.trl_synth_env_num_ctas(N))
+        self._nblk = ops.synth_env_num_ctas(N)
         self._partial = torch.zeros(self._nblk, 2 * o, dtype=F64, device=dev)
         self.batch_sums = torch.zeros(2 * o, dtype=F64, device=dev)
         self._ticket = torch.zeros(1, dtype=I32, device=dev)
@@ -175,13 +174,10 @@ class SynthVecEnv:
         return None
 
     def seed(self, seed):
-        _lib.call("trl_synth_env_seed", self.seeds.data_ptr(), self.episode.data_ptr(), self.env_nums,
-                  int(seed) & 0xFFFFFFFF, self.total_envs & 0xFFFFFFFF, self.first_env & 0xFFFFFFFF, ops._stream())
+        ops.synth_env_seed(self.seeds, self.episode, seed, self.total_envs, self.first_env)
 
     def _reset_kernel(self, mask):
-        _lib.call("trl_synth_env_reset", self.state.data_ptr(), self.elapsed.data_ptr(), self.episode.data_ptr(),
-                  self.seeds.data_ptr(), None if mask is None else ops._chk(mask, U8, "mask"), self.env_nums,
-                  self.obs_dim, float(spec.INIT_SCALE), ops._stream())
+        ops.synth_env_reset(self.state, self.elapsed, self.episode, self.seeds, mask, spec.INIT_SCALE)
 
     def _observe(self, update):
         """NormObs.observation (/root/reference/torchrl/env/base_wrapper.py:118-121)."""
@@ -216,23 +212,17 @@ class SynthVecEnv:
     def launch_step(self, actions, step_count=None, max_episode_frames=0, t_ptr=None):
         """Advance all envs one step: state/reward/done/time_limit staging buffers are updated and
         `obs_out` receives what env.step would return.  No host sync."""
-        N, o, a = self.env_nums, self.obs_dim, self.act_dim
         update = self.obs_norm and self.training and self._obs_normalizer.should_estimate
         nrm = self._obs_normalizer
         distributed = self.dist is not None and self.dist.active
         rs = float(self._reward_scale) if self.training else 1.0
-        _lib.call("trl_synth_env_step", self.state.data_ptr(), ops._chk(actions, F32, "actions"),
-                  self.A.data_ptr(), self.B.data_ptr(), self.c.data_ptr(), self.lb.data_ptr(), self.ub.data_ptr(),
-                  self.elapsed.data_ptr(), None if step_count is None else step_count.data_ptr(),
-                  self.reward.data_ptr(), self.done.data_ptr(), self.time_limit.data_ptr(),
-                  self._partial.data_ptr() if update else None, self.batch_sums.data_ptr() if update else None,
-                  nrm._mean.data_ptr() if update else None, nrm._var.data_ptr() if update else None,
-                  nrm._count.data_ptr() if update else None, self._ticket.data_ptr(),
-                  self.any_reset.data_ptr(), None if t_ptr is None else t_ptr.data_ptr(),
-                  N, o, a, spec.RHO, spec.ETA, spec.CTRL_COST,
-                  float(self.term_thr) if np.isfinite(self.term_thr) else 3.0e38, rs, self._max_episode_steps,
-                  int(max_episode_frames) if step_count is not None else (1 << 30),
-                  1 if (update and not distributed) else 0, ops._stream())
+        moments = (self._partial, self.batch_sums, nrm._mean, nrm._var, nrm._count) if update else (None,) * 5
+        ops.synth_env_step(self.state, actions, self.A, self.B, self.c, self.lb, self.ub, self.elapsed, step_count,
+                           self.reward, self.done, self.time_limit, *moments, self._ticket, self.any_reset, t_ptr,
+                           spec.RHO, spec.ETA, spec.CTRL_COST,
+                           float(self.term_thr) if np.isfinite(self.term_thr) else 3.0e38, rs, self._max_episode_steps,
+                           int(max_episode_frames) if step_count is not None else (1 << 30),
+                           update and not distributed)
         if update and distributed:
             ops.obs_norm_merge(self._reduce_sums(), self.total_envs, nrm._mean, nrm._var, nrm._count)
         if self.obs_norm:

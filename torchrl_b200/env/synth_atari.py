@@ -9,7 +9,7 @@ import copy
 import numpy as np
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from ..spaces import Box, Discrete
 
 F32, U8, I32 = torch.float32, torch.uint8, torch.int32
@@ -60,15 +60,11 @@ class SynthAtariVecEnv:
         pass
 
     def seed(self, seed):
-        _lib.call("trl_synth_env_seed", self.seeds.data_ptr(), self.episode.data_ptr(), self.env_nums,
-                  int(seed) & 0xFFFFFFFF, self.total_envs & 0xFFFFFFFF, self.first_env & 0xFFFFFFFF, ops._stream())
+        ops.synth_env_seed(self.seeds, self.episode, seed, self.total_envs, self.first_env)
 
     def _reset(self, mask=None, zero_is_mask=None, episode_bias=0, bump=1):
-        _lib.call("trl_synth_atari_reset", self.obs.data_ptr(), self.latent.data_ptr(), self.elapsed.data_ptr(),
-                  self.episode.data_ptr(), self.seeds.data_ptr(),
-                  None if mask is None else ops._chk(mask, U8, "mask"),
-                  None if zero_is_mask is None else ops._chk(zero_is_mask, I32, "zero_is_mask"),
-                  int(episode_bias), int(bump), self.env_nums, ops._stream())
+        ops.synth_atari_reset(self.obs, self.latent, self.elapsed, self.episode, self.seeds, mask, zero_is_mask,
+                              episode_bias, bump)
 
     def reset(self, **kwargs):
         self._reset()
@@ -81,10 +77,8 @@ class SynthAtariVecEnv:
 
     def launch_step(self, actions):
         """actions: (N,) or (N,1) float tensor holding the action index.  Updates obs in place."""
-        _lib.call("trl_synth_atari_step", self.obs.data_ptr(), self.latent.data_ptr(),
-                  ops._chk(actions, F32, "actions"), self.elapsed.data_ptr(), self.reward.data_ptr(),
-                  self.done.data_ptr(), self.time_limit.data_ptr(), self.env_nums, self._max_episode_steps,
-                  ops._stream())
+        ops.synth_atari_step(self.obs, self.latent, actions, self.elapsed, self.reward, self.done, self.time_limit,
+                             self._max_episode_steps)
         return self.obs
 
     def step(self, actions):
@@ -94,11 +88,7 @@ class SynthAtariVecEnv:
 
     def to_float(self, obs_u8, out=None):
         """uint8 frames -> float32 in [0,1] (one launch)."""
-        if out is None:
-            out = torch.empty(obs_u8.shape, dtype=F32, device=obs_u8.device)
-        _lib.call("trl_u8_to_f32", ops._chk(obs_u8, U8, "obs"), out.data_ptr(), obs_u8.numel(), float(self.obs_scale),
-                  ops._stream())
-        return out
+        return ops.u8_to_f32(obs_u8, self.obs_scale, out)
 
     def __deepcopy__(self, memo):
         new = SynthAtariVecEnv.__new__(SynthAtariVecEnv)

@@ -10,7 +10,7 @@ import ctypes
 
 import torch
 
-from . import _lib, ops
+from . import ops
 
 F32, F64, I32 = torch.float32, torch.float64, torch.int32
 
@@ -83,8 +83,7 @@ class FlatParams:
 
     def refresh_split(self):
         """Recompute both planes from `data` (one launch)."""
-        _lib.call("trl_split_tf32", self.data.data_ptr(), self.total, self.hi.data_ptr(), self.lo.data_ptr(),
-                  ops._stream())
+        ops.split_tf32(self.data, self.hi, self.lo)
 
     def copy_from(self, src_flat_data):
         """data <- src (a flat tensor of the same layout); the planes follow."""
@@ -113,7 +112,7 @@ class FlatAdam(FlatParams):
             self.grad = region
             self.grad.zero_()
             self.reduced = torch.zeros(self.total, dtype=F32, device=self.device)
-            self._comm_scratch = torch.zeros(int(_lib.load().trl_comm_scratch_doubles(n)), dtype=F64, device=self.device)
+            self._comm_scratch = torch.zeros(ops.comm_scratch_doubles(n), dtype=F64, device=self.device)
         else:
             self.grad = torch.zeros(self.total, dtype=F32, device=self.device)
         self.exp_avg = torch.zeros(self.total, dtype=F32, device=self.device)
@@ -132,8 +131,7 @@ class FlatAdam(FlatParams):
         self.betas = (float(betas[0]), float(betas[1]))
         self.step_counts = torch.zeros(n, dtype=I32, device=self.device)
         self.sumsq3 = torch.zeros(3 * n, dtype=F64, device=self.device)
-        nb = int(_lib.load().trl_grad_sumsq_blocks(n))
-        self._scratch = torch.zeros(nb, dtype=F64, device=self.device)
+        self._scratch = torch.zeros(ops.grad_sumsq_blocks(n), dtype=F64, device=self.device)
         self._ticket = torch.zeros(1, dtype=I32, device=self.device)
         self._seg_c = (ctypes.c_int64 * (n + 1))(*self.seg_begin)
         self._max_norm_c = (ctypes.c_float * n)(*max_norms)
@@ -156,18 +154,14 @@ class FlatAdam(FlatParams):
         (A one-launch variant with a grid barrier between the norm and the update was measured at 9.3 us against 7.5 us
         for these two launches on the PPO agent's 141 k parameters, and dropped.)"""
         mask = self.all_mask if active_mask is None else int(active_mask)
-        st = ops._stream()
         src = self.grad
         if reduced:
             src, zero_grad = self.reduced, False
         else:
-            _lib.call("trl_grad_sumsq", self.grad.data_ptr(), self._seg_c, self.nseg, mask, self.sumsq3.data_ptr(),
-                      self.step_counts.data_ptr(), self.betas[0], self.betas[1], self._scratch.data_ptr(),
-                      self._ticket.data_ptr(), st)
-        _lib.call("trl_adam_step", self.data.data_ptr(), src.data_ptr(), self.exp_avg.data_ptr(),
-                  self.exp_avg_sq.data_ptr(), self._seg_c, self.nseg, mask, self.sumsq3.data_ptr(),
-                  self.lr.data_ptr(), self._max_norm_c, self._eps_c, self.betas[0], self.betas[1],
-                  float(grad_scale), int(bool(zero_grad)), self.hi.data_ptr(), self.lo.data_ptr(), st)
+            ops.grad_sumsq(self.grad, self._seg_c, self.nseg, mask, self.sumsq3, self.step_counts, self.betas,
+                           self._scratch, self._ticket)
+        ops.adam_step(self.data, src, self.exp_avg, self.exp_avg_sq, self._seg_c, self.nseg, mask, self.sumsq3, self.lr,
+                      self._max_norm_c, self._eps_c, self.betas, grad_scale, zero_grad, self.hi, self.lo)
 
     def grad_norms(self):
         """Pre-clip total norm per segment of the last step (what clip_grad_norm_ returns)."""

@@ -19,7 +19,8 @@ import weakref
 import torch
 import torch.nn as nn
 
-from .. import _lib, ops
+from .. import ops
+from ..ops import split_tf32
 
 ACT_CODES = {nn.Tanh: 1, nn.ReLU: 2}
 _ENABLED = True
@@ -181,21 +182,36 @@ def _tc3_ok(rows, n_out, k):
     return _MATMUL_MODE == "tc3" and rows >= _TC3_MIN_ROWS and n_out == 256 and k >= 32 and k % 32 == 0
 
 
-def split_tf32(t):
-    """(hi, lo) of a contiguous fp32 tensor."""
-    hi, lo = torch.empty_like(t), torch.empty_like(t)
-    _lib.call("trl_split_tf32", ops._chk(t, torch.float32, "x"), t.numel(), hi.data_ptr(), lo.data_ptr(),
-              ops._stream())
-    return hi, lo
-
-
-_WGRAD_WS = {}
-
-
 def _stream_key():
     """Scratch buffers (split-K slabs, reduction partials, tickets) are per CUDA stream: the critic and the actor
     branch of a minibatch run concurrently on two streams (algo/on_policy/a2c.py) and must not share them."""
     return torch.cuda.current_stream().cuda_stream
+
+
+_SCRATCH = {}
+_SCRATCH_KINDS = {      # kind -> (fp32 elements, zeroed int32 tickets) for the sizes (M, H, K) of the launch
+    "tn": lambda M, H, K: (ops.skinny_tn_scratch_floats(M, H, K), 0),      # skinny_tn / _act_wgrad slabs
+    "dgrad_act": lambda M, H, K: (ops.skinny_dgrad_act_scratch_floats(M, H), 0),
+    "bias_act": lambda M, H, K: (max(ops.bias_act_bwd_scratch_floats(M, H), 4), (H + 127) // 128),
+    "cluster": lambda M, H, K: (8 * H * 256, H // 8),                      # gemm3_pair_tn_cluster, H output rows
+    "splitk": lambda M, H, K: (64 * H * 256, 0),                           # gemm_tf32x3_tn, 64 slabs
+}
+
+
+def _scratch(kind, device, M=0, H=0, K=0, job=None):
+    """The scratch of one kind of launch, allocated on first use and reused: a float32 tensor, or (float32, tickets)
+    where the launch counts arrivals.  The float32 part is torch.empty (every launch writes its slabs before reading
+    them); tickets start zeroed and the kernels leave them zero.  One buffer per stream (_stream_key), or with
+    job = the kind of a deferred job: the buffer of the next _DEFER slot, whose slabs must survive until the flush."""
+    key = (kind, M, H, K, str(device), _stream_key() if job is None else ("defer", len(_DEFER), job))
+    ws = _SCRATCH.get(key)
+    if ws is None:
+        floats, tickets = _SCRATCH_KINDS[kind](M, H, K)
+        ws = torch.empty(floats, dtype=torch.float32, device=device)
+        if tickets:
+            ws = ws, torch.zeros(tickets, dtype=torch.int32, device=device)
+        _SCRATCH[key] = ws
+    return ws
 
 
 def wgrad(gz, x, out=None):
@@ -208,18 +224,10 @@ def wgrad(gz, x, out=None):
     K = x.shape[1]
     if _tc3_ok(M, K, M) and H % 128 == 0 and M % (32 * 64) == 0:
         # wgmma 3xTF32, operands consumed M/N-major from their row-major storage, deterministic split-K
-        pair = _GEMM_IMPL == "pair" and H % 256 == 0
-        key = (H, pair, str(gz.device), _stream_key())
-        ws = _WGRAD_WS.get(key)
-        if pair:
+        if _GEMM_IMPL == "pair" and H % 256 == 0:
             # split-K summed inside the launch (8 group partials + arrival tickets instead of 64 slabs)
-            if ws is None:
-                ws = _WGRAD_WS[key] = (torch.empty(8 * H * 256, dtype=torch.float32, device=gz.device),
-                                       torch.zeros(H // 8, dtype=torch.int32, device=gz.device))
-            return ops.gemm3_pair_tn_cluster(gz, x, *ws, out=out, splits=64)
-        if ws is None:
-            ws = _WGRAD_WS[key] = torch.empty(64 * H * 256, dtype=torch.float32, device=gz.device)
-        return ops.gemm_tf32x3_tn(gz, x, out=out, splits=64, workspace=ws)
+            return ops.gemm3_pair_tn_cluster(gz, x, *_scratch("cluster", gz.device, H=H), out=out, splits=64)
+        return ops.gemm_tf32x3_tn(gz, x, out=out, splits=64, workspace=_scratch("splitk", gz.device, H=H))
     if (_MATMUL_MODE != "fp32" and K <= 24 and H % 32 == 0 and H <= 256 and _skinny_ok(gz)
             and (out is None or out.is_contiguous())):
         return skinny_tn(gz, x, out=out)                 # (H,K) = gz^T x, first-layer weight gradient
@@ -322,25 +330,8 @@ def fused_enabled():
     return _ENABLED
 
 
-class _Workspace:
-    """Per-(M,H) scratch for the backward's column-sum partials + tickets (allocated once, reused)."""
-    cache = {}
-
-    @classmethod
-    def get(cls, M, H, device):
-        key = (int(M), int(H), str(device), _stream_key())
-        ws = cls.cache.get(key)
-        if ws is None:
-            n = int(_lib.load().trl_bias_act_bwd_scratch_floats(int(M), int(H)))
-            ws = (torch.empty(max(n, 4), dtype=torch.float32, device=device),
-                  torch.zeros((H + 127) // 128, dtype=torch.int32, device=device))
-            cls.cache[key] = ws
-        return ws
-
-
 _SKINNY_MIN_ROWS = 1024
 _SKINNY = True         # csrc/skinny.cu serves the first (K = obs_dim) and output (N <= 8) layers
-_TN_WS = {}
 
 
 def set_skinny(flag):
@@ -352,24 +343,6 @@ def set_skinny(flag):
 
 def _skinny_ok(x):
     return _SKINNY and _ENABLED and x.is_cuda and x.shape[0] >= _SKINNY_MIN_ROWS
-
-
-def _tn_scratch(M, H, K, device):
-    key = (M, H, K, str(device), _stream_key())
-    ws = _TN_WS.get(key)
-    if ws is None:
-        n = int(_lib.load().trl_skinny_tn_scratch_floats(M, H, K))
-        ws = _TN_WS[key] = torch.empty(n, dtype=torch.float32, device=device)
-    return ws
-
-
-def _dgrad_act_scratch(M, H, device):
-    key = ("dgrad_act", M, H, str(device), _stream_key())
-    ws = _TN_WS.get(key)
-    if ws is None:
-        n = int(_lib.load().trl_skinny_dgrad_act_scratch_floats(M, H))
-        ws = _TN_WS[key] = torch.empty(n, dtype=torch.float32, device=device)
-    return ws
 
 
 # ---- deferred second stages ---------------------------------------------------------------------------------------------
@@ -395,18 +368,6 @@ class deferred_reduces:
         return False
 
 
-def _defer_scratch(kind, M, H, K, device):
-    """One scratch buffer per pending job (its slabs must survive until the flush): keyed by the job's position."""
-    slot = len(_DEFER)
-    key = ("defer", slot, kind, M, H, K, str(device))
-    ws = _TN_WS.get(key)
-    if ws is None:
-        lib = _lib.load()
-        n = int(lib.trl_skinny_dgrad_act_scratch_floats(M, H)) if kind == 2 else int(lib.trl_skinny_tn_scratch_floats(M, H, K))
-        ws = _TN_WS[key] = torch.empty(n, dtype=torch.float32, device=device)
-    return ws
-
-
 def flush_reduces():
     """Second stages of every job recorded since the scope opened, on the current stream (which must already be ordered
     after the streams the first stages ran on)."""
@@ -419,17 +380,7 @@ def flush_reduces():
     _DEFER = []
 
 
-def _reduce_jobs(part):
-    """One trl_skinny_reduce_jobs launch for up to 8 jobs (kind, scratch, out, colsum, M, H, K, out_transposed)."""
-    import ctypes
-    n = len(part)
-    vp = ctypes.c_void_p
-    _lib.call("trl_skinny_reduce_jobs", n, (ctypes.c_int * n)(*[j[0] for j in part]),
-              (vp * n)(*[j[1].data_ptr() for j in part]),
-              (vp * n)(*[0 if j[2] is None else j[2].data_ptr() for j in part]),
-              (vp * n)(*[0 if j[3] is None else j[3].data_ptr() for j in part]),
-              (ctypes.c_int64 * n)(*[j[4] for j in part]), (ctypes.c_int * n)(*[j[5] for j in part]),
-              (ctypes.c_int * n)(*[j[6] for j in part]), (ctypes.c_int * n)(*[j[7] for j in part]), ops._stream())
+_reduce_jobs = ops.skinny_reduce_jobs          # one launch for up to 8 jobs of the _DEFER tuple format
 
 
 def _can_defer(*outs):
@@ -443,19 +394,13 @@ def skinny_tn(a, b, out=None, colsum=None, out_transposed=False, may_defer=False
     M, H = a.shape
     K = b.shape[1]
     if may_defer and _can_defer(out) and len(_DEFER) < 64:
-        ws = _defer_scratch(0, M, H, K, a.device)
-        _lib.call("trl_skinny_tn_partial", ops._chk(a, torch.float32, "a"), ops._chk(b, torch.float32, "b"), M, H, K,
-                  int(colsum is not None), ws.data_ptr(), ops._stream())
+        ws = _scratch("tn", a.device, M, H, K, job=0)
+        ops.skinny_tn_partial(a, b, colsum is not None, ws)
         _DEFER.append((0, ws, out, colsum, M, H, K, int(bool(out_transposed))))
         return out
-    ws = _tn_scratch(M, H, K, a.device)
     if out is None:
         out = torch.empty((K, H) if out_transposed else (H, K), dtype=torch.float32, device=a.device)
-    _lib.call("trl_skinny_tn", ops._chk(a, torch.float32, "a"), ops._chk(b, torch.float32, "b"),
-              ops._chk(out, torch.float32, "out"), None if colsum is None else ops._chk(colsum, torch.float32, "colsum"),
-              M, H, K, int(bool(out_transposed)), ws.data_ptr(), ops._stream())
-    _lib.add_launches(1)
-    return out
+    return ops.skinny_tn(a, b, out, colsum, out_transposed, _scratch("tn", a.device, M, H, K))
 
 
 class _LinearAct(torch.autograd.Function):
@@ -464,7 +409,7 @@ class _LinearAct(torch.autograd.Function):
         tc = (_MATMUL_MODE == "tf32x3" and min(x.shape[0], x.shape[1], weight.shape[0]) >= _TF32X3_MIN_DIM)
         if _first_skinny_ok(x, weight, bias):
             # skinny first layer: GEMM + bias + activation in one memory-bound launch
-            z = _skinny_first_fwd(x, weight, bias, act)
+            z = ops.skinny_k_fwd(x, weight, bias, act)
             ctx.save_for_backward(x, weight, z)
             ctx.act, ctx.tc, ctx.params = act, False, (weight, bias)
             return z
@@ -482,8 +427,7 @@ class _LinearAct(torch.autograd.Function):
         else:
             z = torch.mm(x, weight.t())
             ctx.save_for_backward(x, weight, z)
-        _lib.call("trl_bias_act_fwd", z.data_ptr(), ops._chk(bias, torch.float32, "bias"), z.shape[0], z.shape[1],
-                  act, ops._stream())
+        ops.bias_act_fwd(z, bias, act)
         ctx.act = act
         ctx.tc = tc
         ctx.params = (weight, bias)        # the Parameter objects themselves (for direct-grad mode)
@@ -501,13 +445,6 @@ def _first_skinny_ok(x, weight, bias):
     """The skinny first-layer forward (csrc/skinny.cu k_fwd) serves x (M, K <= 24) . weight^T."""
     return (_MATMUL_MODE != "fp32" and _skinny_ok(x) and x.shape[1] <= 24 and weight.shape[0] % 4 == 0
             and weight.shape[0] <= 1024 and weight.is_contiguous() and bias.is_contiguous())
-
-
-def _skinny_first_fwd(x, weight, bias, act):
-    z = torch.empty(x.shape[0], weight.shape[0], dtype=torch.float32, device=x.device)
-    _lib.call("trl_skinny_k_fwd", x.data_ptr(), weight.data_ptr(), bias.data_ptr(), z.data_ptr(), x.shape[0],
-              x.shape[1], weight.shape[0], act, ops._stream())
-    return z
 
 
 def _act_wgrad_ok(x, y, dw_out):
@@ -530,19 +467,14 @@ def _linear_act_bwd(g, x, weight, y, act, params, needs_input_grad):
         # (M, H) matrices; the activation gradient gz is never written to memory
         dw = dw_out if dw_out is not None else torch.empty(H, K, dtype=torch.float32, device=y.device)
         if _can_defer(dw_out, db_out):
-            ws = _defer_scratch(1, M, H, K, y.device)
-            _lib.call("trl_skinny_act_wgrad_partial", g.data_ptr(), y.data_ptr(), x.data_ptr(), M, H, K, act,
-                      ws.data_ptr(), ops._stream())
+            ws = _scratch("tn", y.device, M, H, K, job=1)
+            ops.skinny_act_wgrad_partial(g, y, x, act, ws)
             _DEFER.append((1, ws, dw, db, M, H, K, 0))
             return None, None, None
-        _lib.call("trl_skinny_act_wgrad", g.data_ptr(), y.data_ptr(), x.data_ptr(), dw.data_ptr(), db.data_ptr(),
-                  M, H, K, act, _tn_scratch(M, H, K, y.device).data_ptr(), ops._stream())
-        _lib.add_launches(1)
+        ops.skinny_act_wgrad(g, y, x, dw, db, act, _scratch("tn", y.device, M, H, K))
         return None, None if dw_out is not None else dw, None if db_out is not None else db
     gz = torch.empty_like(y)
-    scratch, tickets = _Workspace.get(M, H, y.device)
-    _lib.call("trl_bias_act_bwd", g.data_ptr(), y.data_ptr(), gz.data_ptr(), db.data_ptr(), M, H, act,
-              scratch.data_ptr(), tickets.data_ptr(), ops._stream())
+    ops.bias_act_bwd(g, y, gz, db, act, *_scratch("bias_act", y.device, M, H))
     dx = None
     if needs_input_grad[0]:
         if _tc3_ok(M, weight.shape[1], H) and weight.is_contiguous():
@@ -560,9 +492,7 @@ def _backward_tc(ctx, g):
     M, H = y.shape
     gz = torch.empty_like(y)
     db = torch.empty(H, dtype=torch.float32, device=y.device)
-    scratch, tickets = _Workspace.get(M, H, y.device)
-    _lib.call("trl_bias_act_bwd", g.data_ptr(), y.data_ptr(), gz.data_ptr(), db.data_ptr(), M, H, ctx.act,
-              scratch.data_ptr(), tickets.data_ptr(), ops._stream())
+    ops.bias_act_bwd(g, y, gz, db, ctx.act, *_scratch("bias_act", y.device, M, H))
     g_hi, g_lo = split_tf32(gz)
     dx = mm3(g_hi, g_lo, w_hi, w_lo) if ctx.needs_input_grad[0] else None
     dw = mm3(g_hi.t(), g_lo.t(), x_hi, x_lo) if ctx.needs_input_grad[1] else None
@@ -583,10 +513,7 @@ class _LinearPlain(torch.autograd.Function):
         ctx.skinny = (_MATMUL_MODE != "fp32" and _skinny_ok(x) and N <= 8 and H in (128, 256)
                       and weight.is_contiguous())
         if ctx.skinny:
-            y = torch.empty(x.shape[0], N, dtype=torch.float32, device=x.device)
-            _lib.call("trl_skinny_n_fwd", x.data_ptr(), weight.data_ptr(), bias.data_ptr(), y.data_ptr(), x.shape[0], H, N,
-                      ops._stream())
-            return y
+            return ops.skinny_n_fwd(x, weight, bias)
         return torch.addmm(bias, x, weight.t())
 
     @staticmethod
@@ -596,12 +523,8 @@ class _LinearPlain(torch.autograd.Function):
         w_param, b_param = ctx.params
         db_out, dw_out = _grad_out(b_param), _grad_out(w_param)
         if ctx.skinny:
-            N, H = weight.shape
-            dx = None
-            if ctx.needs_input_grad[0]:
-                dx = torch.empty(x.shape[0], H, dtype=torch.float32, device=x.device)
-                _lib.call("trl_skinny_n_dgrad", g.data_ptr(), weight.data_ptr(), dx.data_ptr(), x.shape[0], H, N,
-                          ops._stream())
+            N = weight.shape[0]
+            dx = ops.skinny_n_dgrad(g, weight) if ctx.needs_input_grad[0] else None
             db = db_out if db_out is not None else torch.empty(N, dtype=torch.float32, device=x.device)
             dw = skinny_tn(x, g, out=dw_out, colsum=db, out_transposed=True)     # dW (N,H) = g^T x, db = sum g
             return dx, None if dw_out is not None else dw, None if db_out is not None else db
@@ -628,13 +551,9 @@ class _MLPTail(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, w1, b1, act1, w2, b2, w3, b3, act):
-        h1 = _skinny_first_fwd(x, w1, b1, act1) if w1 is not None else x
+        h1 = ops.skinny_k_fwd(x, w1, b1, act1) if w1 is not None else x
         y2 = mm_fwd(h1, w2, bias=b2, act=act)
-        M, H = y2.shape
-        N = w3.shape[0]
-        out = torch.empty(M, N, dtype=torch.float32, device=x.device)
-        _lib.call("trl_skinny_n_fwd", y2.data_ptr(), w3.data_ptr(), b3.data_ptr(), out.data_ptr(), M, H, N,
-                  ops._stream())
+        out = ops.skinny_n_fwd(y2, w3, b3)
         ctx.save_for_backward(x, w1, h1, w2, y2, w3)
         ctx.act, ctx.act1 = act, act1
         ctx.params = (w1, b1, w2, b2, w3, b3)
@@ -657,23 +576,20 @@ class _MLPTail(torch.autograd.Function):
         if w3_fused:
             dw3 = dw3_out if dw3_out is not None else torch.empty(N, H, dtype=torch.float32, device=dev)
         if w3_fused and _can_defer(db2_out, dw3_out, db3_out) and len(_DEFER) < 63:     # skinny_tn's bound on jobs
-            ws = _defer_scratch(2, M, H, 0, dev)
+            ws = _scratch("dgrad_act", dev, M, H, job=2)
             _DEFER.append((2, ws, None, db2, M, H, 0, 0))
-            ws3 = _defer_scratch(0, M, H, N, dev)
+            ws3 = _scratch("tn", dev, M, H, N, job=0)
             _DEFER.append((0, ws3, dw3, db3, M, H, N, 1))
             ops.skinny_n_dgrad_act_wgrad_partial(g, w3, y2, ctx.act, gz, ws, ws3)
         elif w3_fused:
-            ops.skinny_n_dgrad_act_wgrad(g, w3, y2, ctx.act, gz, db2, dw3, db3, _dgrad_act_scratch(M, H, dev),
-                                         _tn_scratch(M, H, N, dev))
+            ops.skinny_n_dgrad_act_wgrad(g, w3, y2, ctx.act, gz, db2, dw3, db3, _scratch("dgrad_act", dev, M, H),
+                                         _scratch("tn", dev, M, H, N))
         elif _can_defer(db2_out):
-            ws = _defer_scratch(2, M, H, 0, dev)
-            _lib.call("trl_skinny_n_dgrad_act_partial", g.data_ptr(), w3.data_ptr(), y2.data_ptr(), gz.data_ptr(), M, H, N,
-                      ctx.act, ws.data_ptr(), ops._stream())
+            ws = _scratch("dgrad_act", dev, M, H, job=2)
+            ops.skinny_n_dgrad_act_partial(g, w3, y2, gz, ctx.act, ws)
             _DEFER.append((2, ws, None, db2, M, H, 0, 0))
         else:
-            _lib.call("trl_skinny_n_dgrad_act", g.data_ptr(), w3.data_ptr(), y2.data_ptr(), gz.data_ptr(), db2.data_ptr(),
-                      M, H, N, ctx.act, _dgrad_act_scratch(M, H, dev).data_ptr(), ops._stream())
-            _lib.add_launches(1)
+            ops.skinny_n_dgrad_act(g, w3, y2, gz, db2, ctx.act, _scratch("dgrad_act", dev, M, H))
         first = w1 is not None
         want_dx = ctx.needs_input_grad[0] and not first
         fk = _fork_here()
@@ -717,14 +633,13 @@ def _first_layer_bwd(ctx, gz, x0, w1, h1, w2):
     dw = dw_out if dw_out is not None else torch.empty(H, K, dtype=torch.float32, device=h1.device)
     db = db_out if db_out is not None else torch.empty(H, dtype=torch.float32, device=h1.device)
     if _can_defer(dw_out, db_out):
-        ws = _defer_scratch(1, M, H, K, h1.device)
+        ws = _scratch("tn", h1.device, M, H, K, job=1)
         ops.gemm3_pair_dgrad_act_wgrad(gz, planes_t, h1, x0, ctx.act1, ws)
         _DEFER.append((1, ws, dw, db, M, H, K, 0))
         return None, None
-    ws = _tn_scratch(M, H, K, h1.device)
+    ws = _scratch("tn", h1.device, M, H, K)
     ops.gemm3_pair_dgrad_act_wgrad(gz, planes_t, h1, x0, ctx.act1, ws)
     _reduce_jobs([(1, ws, dw, db, M, H, K, 0)])
-    _lib.add_launches(1)
     return None if dw_out is not None else dw, None if db_out is not None else db
 
 

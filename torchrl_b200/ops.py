@@ -174,6 +174,29 @@ def counter_advance(counter, t_ptr=None, T=1, size_ptr=None):
               _opt(counter, I64, "counter"), _stream())
 
 
+def collect_finalize(cur_ob_in, next_norm, state, act, value, v_next, reward, done, tl, elapsed, episode, seeds,
+                     step_count, ep_return, epoch_reward, ret_log, n_done, any_reset, norm_mean, norm_var, cur_ob_out,
+                     b_obs, b_next_obs, b_acts, b_values, b_rewards, b_terminals, b_time_limits, t_ptr,
+                     max_episode_frames, discount, init_scale, clip, terminal_includes_surpass, raw_obs_after_reset):
+    """The end of one collector step (csrc/collect.cu): row `*t_ptr` of the replay ring, episode returns, the timeout
+    bootstrap and the partial reset of the finished envs.  cur_ob_in (N, o), act (N, a).  state / elapsed / episode /
+    seeds / any_reset None: host envs (the host resets them afterwards)."""
+    N, o = cur_ob_in.shape
+    _lib.call("trl_collect_finalize", _chk(cur_ob_in, F32, "cur_ob_in"), _chk(next_norm, F32, "next_norm"),
+              _opt(state, F32, "state"), _chk(act, F32, "act"), _opt(value, F32, "value"), _opt(v_next, F32, "v_next"),
+              _chk(reward, F32, "reward"), _chk(done, U8, "done"), _chk(tl, U8, "time_limit"),
+              _opt(elapsed, I32, "elapsed"), _opt(episode, I32, "episode"), _opt(seeds, I32, "seeds"),
+              _chk(step_count, I32, "step_count"), _chk(ep_return, F64, "ep_return"),
+              _chk(epoch_reward, F64, "epoch_reward"), _chk(ret_log, F32, "ret_log"), _chk(n_done, I32, "n_done"),
+              _opt(any_reset, I32, "any_reset"), _opt(norm_mean, F64, "norm_mean"), _opt(norm_var, F64, "norm_var"),
+              _chk(cur_ob_out, F32, "cur_ob_out"), _chk(b_obs, F32, "b_obs"), _chk(b_next_obs, F32, "b_next_obs"),
+              _chk(b_acts, F32, "b_acts"), _opt(b_values, F32, "b_values"), _chk(b_rewards, F32, "b_rewards"),
+              _chk(b_terminals, U8, "b_terminals"), _chk(b_time_limits, U8, "b_time_limits"),
+              _chk(t_ptr, I32, "t_ptr"), N, o, act.numel() // N, int(max_episode_frames), float(discount),
+              float(init_scale), float(clip), int(bool(terminal_includes_surpass)), int(bool(raw_obs_after_reset)),
+              _stream())
+
+
 # ------------------------------------------------------------------------------------------ K7/K9/K4
 class RowCopyPlan:
     """Pre-built key table for trl_row_gather / trl_ring_write (host arrays of device pointers)."""
@@ -219,6 +242,19 @@ def vec_stats(x, out=None):
     return out
 
 
+def vec_moments(x, out):
+    """out (4) f64 = sum, sum of squares, max, -min of a float vector: one rank's share of vec_stats."""
+    _lib.call("trl_vec_moments", _chk(x, F32, "x"), x.numel(), _chk(out, F64, "moments"), _stream())
+    return out
+
+
+def vec_stats_from_moments(gathered, world, n_total, out):
+    """out (4) f32 = mean, unbiased std, max, min from `world` ranks' vec_moments, (world, 4) f64."""
+    _lib.call("trl_vec_stats_from_moments", _chk(gathered, F64, "moments"), int(world), float(n_total),
+              _chk(out, F32, "stats"), _stream())
+    return out
+
+
 # ------------------------------------------------------------------------------------------ K8
 class LossScratch:
     """Scratch + ticket for the two-level reductions of the loss kernels (allocated once)."""
@@ -254,7 +290,7 @@ def ppo_actor_loss(mean, log_std, actions, old_logp, advs, adv_stats, clip_para,
               float(clip_para),
               float(entropy_coeff), ls_lo, ls_hi, _chk(g_mean, F32, "g_mean"), _chk(g_log_std, F32, "g_log_std"),
               _opt(logp_out, F32, "logp_out"), _chk(info, F32, "info"), _chk(scratch.actor, F64, "scratch"),
-              scratch.tickets[0:1].data_ptr(), _stream())
+              _chk(scratch.tickets[0:1], I32, "ticket"), _stream())
     return g_mean, g_log_std, info
 
 
@@ -268,7 +304,7 @@ def ppo_critic_loss(values, returns, old_values, clipped, clip_para, scratch, g_
     _lib.call("trl_ppo_critic_loss", _chk(values, F32, "values"), _chk(returns, F32, "returns"),
               _opt(old_values, F32, "old_values"), B, int(bool(clipped)), float(clip_para),
               _chk(g_values, F32, "g_values"), _chk(info, F32, "info"), _chk(scratch.critic, F64, "scratch"),
-              scratch.tickets[1:2].data_ptr(), _stream())
+              _chk(scratch.tickets[1:2], I32, "ticket"), _stream())
     return g_values, info
 
 
@@ -330,7 +366,7 @@ def ppo_categorical_actor_loss(logits, actions, old_logp, advs, adv_stats, clip_
               _opt(old_logp, F32, "old_logp"), _chk(advs, F32, "advs"), _opt(adv_stats, F32, "adv_stats"),
               _opt(stats_pos, I32, "stats_pos"), B, A, float(clip_para), float(entropy_coeff),
               _chk(g_logits, F32, "g_logits"), _opt(logp_out, F32, "logp_out"), _chk(info, F32, "info"),
-              _chk(scratch.actor, F64, "scratch"), scratch.tickets[0:1].data_ptr(), _stream())
+              _chk(scratch.actor, F64, "scratch"), _chk(scratch.tickets[0:1], I32, "ticket"), _stream())
     return g_logits, info
 
 
@@ -362,6 +398,29 @@ def polyak_update(target_flat, source_flat, tau, planes=None):
               target_flat.numel(), float(tau), _opt(hi, F32, "hi"), _opt(lo, F32, "lo"), _stream())
 
 
+def grad_sumsq_blocks(nseg):
+    """float64 scratch elements of grad_sumsq for `nseg` segments."""
+    return int(_lib.load().trl_grad_sumsq_blocks(int(nseg)))
+
+
+def grad_sumsq(grad, seg_begin, nseg, mask, sumsq3, step_counts, betas, scratch, ticket):
+    """Per-segment sum of squares of the flat gradient, Adam step counts and bias corrections into sumsq3 (3 nseg f64)
+    for the active segments of `mask`.  seg_begin: host int64 array of the nseg + 1 segment offsets."""
+    _lib.call("trl_grad_sumsq", _chk(grad, F32, "grad"), seg_begin, int(nseg), int(mask), _chk(sumsq3, F64, "sumsq3"),
+              _chk(step_counts, I32, "step_counts"), float(betas[0]), float(betas[1]), _chk(scratch, F64, "scratch"),
+              _chk(ticket, I32, "ticket"), _stream())
+
+
+def adam_step(param, grad, exp_avg, exp_avg_sq, seg_begin, nseg, mask, sumsq3, lr, max_norm, eps, betas, grad_scale,
+              zero_grad, hi, lo):
+    """Clip (per segment, by the norms in sumsq3) + Adam on the flat buffers, optionally zeroing `grad`; hi / lo: the
+    TF32 planes of `param` kept current.  seg_begin / max_norm / eps: host arrays (int64, float, float)."""
+    _lib.call("trl_adam_step", _chk(param, F32, "param"), _chk(grad, F32, "grad"), _chk(exp_avg, F32, "exp_avg"),
+              _chk(exp_avg_sq, F32, "exp_avg_sq"), seg_begin, int(nseg), int(mask), _chk(sumsq3, F64, "sumsq3"),
+              _chk(lr, F32, "lr"), max_norm, eps, float(betas[0]), float(betas[1]), float(grad_scale),
+              int(bool(zero_grad)), _chk(hi, F32, "hi"), _chk(lo, F32, "lo"), _stream())
+
+
 # ------------------------------------------------------------------------------------------ K10
 class OffPolicyScratch:
     """Scratch + tickets for the off-policy loss kernels (allocated once per batch size)."""
@@ -373,7 +432,10 @@ class OffPolicyScratch:
         self.B = int(B)
 
     def t(self, i):
-        return self.tickets[i:i + 1].data_ptr()
+        return _chk(self.tickets[i:i + 1], I32, "ticket")
+
+    def b(self, i):
+        return _chk(self.buf[i], F64, "scratch")
 
 
 def td_target(rewards, terminals, q1_next, q2_next, logp_next, log_alpha, gamma, scratch, y=None, info=None,
@@ -388,7 +450,7 @@ def td_target(rewards, terminals, q1_next, q2_next, logp_next, log_alpha, gamma,
     _lib.call("trl_td_target", _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"),
               _chk(q1_next, F32, "q1_next"), _opt(q2_next, F32, "q2_next"), _opt(logp_next, F32, "logp_next"),
               _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha), float(gamma), B, _chk(y, F32, "y"),
-              _chk(info, F32, "info"), scratch.buf[0].data_ptr(), scratch.t(0), _stream())
+              _chk(info, F32, "info"), scratch.b(0), scratch.t(0), _stream())
     return y, info
 
 
@@ -411,7 +473,7 @@ def sac_alpha_step(logp, target_entropy, log_alpha, adam_state, lr, scratch, inf
         info = torch.zeros(2, dtype=F32, device=logp.device)
     _lib.call("trl_sac_alpha_step", _chk(logp, F32, "logp"), float(target_entropy), _chk(log_alpha, F32, "log_alpha"),
               _chk(adam_state, F32, "adam_state"), float(lr), float(betas[0]), float(betas[1]), float(eps),
-              logp.numel(), _chk(info, F32, "info"), scratch.buf[1].data_ptr(), scratch.t(1), _stream())
+              logp.numel(), _chk(info, F32, "info"), scratch.b(1), scratch.t(1), _stream())
     return info
 
 
@@ -423,7 +485,7 @@ def sac_policy_loss(logp, q1, q2, log_alpha, scratch, info=None, fixed_alpha=1.0
         info = torch.zeros(5, dtype=F32, device=logp.device)
     _lib.call("trl_sac_policy_loss", _chk(logp, F32, "logp"), _chk(q1, F32, "q1"), _chk(q2, F32, "q2"),
               _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha), B, _chk(g_lp, F32, "g_logp"),
-              _chk(g1, F32, "g_q1"), _chk(g2, F32, "g_q2"), _chk(info, F32, "info"), scratch.buf[2].data_ptr(),
+              _chk(g1, F32, "g_q1"), _chk(g2, F32, "g_q2"), _chk(info, F32, "info"), scratch.b(2),
               scratch.t(2), _stream())
     return g_lp, g1, g2, info
 
@@ -440,7 +502,7 @@ def sac_v_loss(logp, qn1, qn2, v_pred, log_alpha, scratch, reparameterization=Tr
     _lib.call("trl_sac_v_loss", _chk(logp, F32, "logp"), _chk(qn1, F32, "qn1"), _opt(qn2, F32, "qn2"),
               _chk(v_pred, F32, "v_pred"), _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha),
               int(bool(reparameterization)), B, _chk(g_lp, F32, "g_logp"), _chk(g1, F32, "g_qn1"),
-              _opt(g2, F32, "g_qn2"), _chk(g_v, F32, "g_v"), _chk(info, F32, "info"), scratch.buf[2].data_ptr(),
+              _opt(g2, F32, "g_qn2"), _chk(g_v, F32, "g_v"), _chk(info, F32, "info"), scratch.b(2),
               scratch.t(5), _stream())
     return g_lp, g1, g2, g_v, info
 
@@ -453,7 +515,7 @@ def twin_mse_loss(q1, q2, y, scratch, info=None):
     if info is None:
         info = torch.zeros(2, dtype=F32, device=q1.device)
     _lib.call("trl_twin_mse_loss", _chk(q1, F32, "q1"), _opt(q2, F32, "q2"), _chk(y, F32, "y"), B,
-              _chk(g1, F32, "g1"), _opt(g2, F32, "g2"), _chk(info, F32, "info"), scratch.buf[3].data_ptr(),
+              _chk(g1, F32, "g1"), _opt(g2, F32, "g2"), _chk(info, F32, "info"), scratch.b(3),
               scratch.t(3), _stream())
     return g1, g2, info
 
@@ -470,7 +532,7 @@ def qr_dqn_loss(pred, nxt, actions, rewards, terminals, gamma, scratch, n_action
               _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"), _opt(weights, F32, "weights"), B,
               int(n_actions), int(n_quantiles), float(gamma), float(kappa), int(bool(mse)), _chk(grad, F32, "grad"),
               _opt(td_out, F32, "td_out"), _chk(info, F32, "info"),
-              scratch.buf[4].data_ptr(), scratch.t(4), _stream())
+              scratch.b(4), scratch.t(4), _stream())
     return grad, info
 
 
@@ -486,7 +548,7 @@ def bootstrapped_dqn_loss(pred, nxt, actions, rewards, terminals, masks, gamma, 
     _lib.call("trl_bootstrapped_dqn_loss", _chk(pred, F32, "pred"), _chk(nxt, F32, "next"),
               _chk(actions, F32, "actions"), _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"),
               _chk(masks, U8, "masks"), B, H, A, float(gamma), _chk(grad, F32, "grad"), _chk(info, F32, "info"),
-              scratch.buf[4].data_ptr(), scratch.t(4), _stream())
+              scratch.b(4), scratch.t(4), _stream())
     return grad, info
 
 
@@ -546,9 +608,8 @@ def gemm_tf32x3_nt(a, b, out=None, splits=1, workspace=None, bias=None, act=0):
     if splits > 1 and workspace is None:
         workspace = torch.empty(splits * M * 256, dtype=F32, device=a.device)
     _lib.call("trl_gemm_tf32x3_nt", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K, int(splits),
-              None if workspace is None else workspace.data_ptr(), _opt(bias, F32, "bias"), int(act), _stream())
-    if splits > 1:
-        _lib.add_launches(1)      # + the split-K reduction launch
+              _opt(workspace, F32, "workspace"), _opt(bias, F32, "bias"), int(act), _stream(),
+              kernels=2 if splits > 1 else 1)       # + the split-K reduction
     return out
 
 
@@ -562,9 +623,7 @@ def gemm_tf32x3_tn(a, b, out=None, splits=1, workspace=None):
     if splits > 1 and workspace is None:
         workspace = torch.empty(splits * M * 256, dtype=F32, device=a.device)
     _lib.call("trl_gemm_tf32x3_tn", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K, int(splits),
-              None if workspace is None else workspace.data_ptr(), _stream())
-    if splits > 1:
-        _lib.add_launches(1)
+              _opt(workspace, F32, "workspace"), _stream(), kernels=2 if splits > 1 else 1)
     return out
 
 
@@ -596,9 +655,7 @@ def gemm3_pair_tn(a, b, out=None, splits=1, workspace=None):
     if splits > 1 and workspace is None:
         workspace = torch.empty(splits * M * 256, dtype=F32, device=a.device)
     _lib.call("trl_gemm3_pair_tn", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K, int(splits),
-              None if workspace is None else workspace.data_ptr(), _stream())
-    if splits > 1:
-        _lib.add_launches(1)
+              _opt(workspace, F32, "workspace"), _stream(), kernels=2 if splits > 1 else 1)
     return out
 
 
@@ -649,8 +706,7 @@ def skinny_n_dgrad_act_wgrad(g, w, y, act, gz, db, dw, dbias, db_scratch, w_scra
     assert db.shape == (H,) and dw.shape == (N, H) and dbias.shape == (N,)
     _lib.call("trl_skinny_n_dgrad_act_wgrad", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
               _chk(gz, F32, "gz"), _chk(db, F32, "db"), _chk(dw, F32, "dw"), _chk(dbias, F32, "dbias"), M, H, N,
-              int(act), _chk(db_scratch, F32, "db_scratch"), _chk(w_scratch, F32, "w_scratch"), _stream())
-    _lib.add_launches(1)
+              int(act), _chk(db_scratch, F32, "db_scratch"), _chk(w_scratch, F32, "w_scratch"), _stream(), kernels=2)
 
 
 def transpose_f32(x, out=None):
@@ -659,4 +715,297 @@ def transpose_f32(x, out=None):
     if out is None:
         out = torch.empty(C, R, dtype=F32, device=x.device)
     _lib.call("trl_transpose_f32", _chk(x, F32, "x"), _chk(out, F32, "out"), R, C, _stream())
+    return out
+
+
+def split_tf32(x, hi=None, lo=None):
+    """(hi, lo) TF32 planes of a contiguous fp32 tensor: hi = tf32(x), lo = x - hi (csrc/mlp_epilogue.cu)."""
+    hi = torch.empty_like(x) if hi is None else hi
+    lo = torch.empty_like(x) if lo is None else lo
+    assert hi.numel() == x.numel() and lo.numel() == x.numel()
+    _lib.call("trl_split_tf32", _chk(x, F32, "x"), x.numel(), _chk(hi, F32, "hi"), _chk(lo, F32, "lo"), _stream(),
+              kernels=int(x.numel() > 0))
+    return hi, lo
+
+
+# ------------------------------------------------------------------------------------------ MLP layer epilogues
+def bias_act_bwd_scratch_floats(M, H):
+    return int(_lib.load().trl_bias_act_bwd_scratch_floats(int(M), int(H)))
+
+
+def bias_act_fwd(z, bias, act):
+    """z (M,H) <- act(z + bias) in place."""
+    M, H = z.shape
+    _lib.call("trl_bias_act_fwd", _chk(z, F32, "z"), _chk(bias, F32, "bias"), M, H, int(act), _stream(),
+              kernels=int(M > 0))
+    return z
+
+
+def bias_act_bwd(g, y, gz, db, act, scratch, tickets):
+    """gz = g * act'(y) and db = colsum(gz) for y (M,H); scratch: bias_act_bwd_scratch_floats(M, H) floats, tickets:
+    (H + 127) // 128 zeroed int32 (left zero)."""
+    M, H = y.shape
+    _lib.call("trl_bias_act_bwd", _chk(g, F32, "g"), _chk(y, F32, "y"), _chk(gz, F32, "gz"), _chk(db, F32, "db"), M, H,
+              int(act), _chk(scratch, F32, "scratch"), _chk(tickets, I32, "tickets"), _stream())
+
+
+# ------------------------------------------------------------------------------------------ skinny layers
+# First layer (K = obs_dim <= 24) and output layer (N <= 8) of the MLPs (csrc/skinny.cu).  The weight / bias gradients
+# are per-CTA slabs in a scratch buffer, then a slab sum: the plain entry points launch both kernels, the *_partial
+# ones only the first and skinny_reduce_jobs sums the slabs of up to 8 jobs in one launch.
+def skinny_tn_scratch_floats(M, H, K):
+    return int(_lib.load().trl_skinny_tn_scratch_floats(int(M), int(H), int(K)))
+
+
+def skinny_dgrad_act_scratch_floats(M, H):
+    return int(_lib.load().trl_skinny_dgrad_act_scratch_floats(int(M), int(H)))
+
+
+def skinny_k_fwd(x, w, bias, act, out=None):
+    """out (M,H) = act(x (M,K) @ w (H,K)^T + bias)."""
+    M, K = x.shape
+    H = w.shape[0]
+    if out is None:
+        out = torch.empty(M, H, dtype=F32, device=x.device)
+    _lib.call("trl_skinny_k_fwd", _chk(x, F32, "x"), _chk(w, F32, "w"), _chk(bias, F32, "bias"), _chk(out, F32, "out"),
+              M, K, H, int(act), _stream())
+    return out
+
+
+def skinny_n_fwd(x, w, bias, out=None):
+    """out (M,N) = x (M,H) @ w (N,H)^T + bias."""
+    M, H = x.shape
+    N = w.shape[0]
+    if out is None:
+        out = torch.empty(M, N, dtype=F32, device=x.device)
+    _lib.call("trl_skinny_n_fwd", _chk(x, F32, "x"), _chk(w, F32, "w"), _chk(bias, F32, "bias"), _chk(out, F32, "out"),
+              M, H, N, _stream())
+    return out
+
+
+def skinny_n_dgrad(g, w, out=None):
+    """out (M,H) = g (M,N) @ w (N,H)."""
+    M = g.shape[0]
+    N, H = w.shape
+    if out is None:
+        out = torch.empty(M, H, dtype=F32, device=g.device)
+    _lib.call("trl_skinny_n_dgrad", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(out, F32, "dx"), M, H, N, _stream())
+    return out
+
+
+def skinny_tn(a, b, out, colsum, out_transposed, scratch):
+    """out = a^T @ b for a (M,H), b (M,K) ((H,K), or (K,H) when out_transposed) [+ colsum (K) = colsum(b)];
+    scratch: skinny_tn_scratch_floats(M, H, K) floats."""
+    M, H = a.shape
+    K = b.shape[1]
+    _lib.call("trl_skinny_tn", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), _opt(colsum, F32, "colsum"),
+              M, H, K, int(bool(out_transposed)), _chk(scratch, F32, "scratch"), _stream(), kernels=2)
+    return out
+
+
+def skinny_tn_partial(a, b, want_colsum, scratch):
+    """The slabs of skinny_tn (reduce job kind 0)."""
+    M, H = a.shape
+    K = b.shape[1]
+    _lib.call("trl_skinny_tn_partial", _chk(a, F32, "a"), _chk(b, F32, "b"), M, H, K, int(bool(want_colsum)),
+              _chk(scratch, F32, "scratch"), _stream())
+
+
+def skinny_act_wgrad(g, y, x, dw, db, act, scratch):
+    """The first layer's dW (H,K) = (g * act'(y))^T x and db = colsum(g * act'(y)) in one pass over g and y (M,H);
+    scratch: skinny_tn_scratch_floats(M, H, K) floats."""
+    M, H = y.shape
+    K = x.shape[1]
+    _lib.call("trl_skinny_act_wgrad", _chk(g, F32, "g"), _chk(y, F32, "y"), _chk(x, F32, "x"), _chk(dw, F32, "dw"),
+              _chk(db, F32, "db"), M, H, K, int(act), _chk(scratch, F32, "scratch"), _stream(), kernels=2)
+
+
+def skinny_act_wgrad_partial(g, y, x, act, scratch):
+    """The slabs of skinny_act_wgrad (reduce job kind 1)."""
+    M, H = y.shape
+    K = x.shape[1]
+    _lib.call("trl_skinny_act_wgrad_partial", _chk(g, F32, "g"), _chk(y, F32, "y"), _chk(x, F32, "x"), M, H, K,
+              int(act), _chk(scratch, F32, "scratch"), _stream())
+
+
+def skinny_n_dgrad_act(g, w, y, gz, db, act, scratch):
+    """gz (M,H) = (g (M,N) @ w (N,H)) * act'(y) and db = colsum(gz); scratch: skinny_dgrad_act_scratch_floats(M, H)."""
+    M, H = y.shape
+    N = w.shape[0]
+    _lib.call("trl_skinny_n_dgrad_act", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"), _chk(gz, F32, "gz"),
+              _chk(db, F32, "db"), M, H, N, int(act), _chk(scratch, F32, "scratch"), _stream(), kernels=2)
+
+
+def skinny_n_dgrad_act_partial(g, w, y, gz, act, scratch):
+    """gz of skinny_n_dgrad_act and the slabs of its db (reduce job kind 2)."""
+    M, H = y.shape
+    N = w.shape[0]
+    _lib.call("trl_skinny_n_dgrad_act_partial", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
+              _chk(gz, F32, "gz"), M, H, N, int(act), _chk(scratch, F32, "scratch"), _stream())
+
+
+def skinny_reduce_jobs(jobs):
+    """The slab sums of up to 8 jobs (kind, scratch, out, colsum, M, H, K, out_transposed) in one launch: kind 0 =
+    skinny_tn_partial (colsum None or (K)), 1 = skinny_act_wgrad_partial (colsum = db (H)), 2 =
+    skinny_n_dgrad_act_partial (colsum = db (H), out None)."""
+    n = len(jobs)
+    assert n <= 8
+    vp, ci = ctypes.c_void_p, ctypes.c_int
+    _lib.call("trl_skinny_reduce_jobs", n, (ci * n)(*[j[0] for j in jobs]),
+              (vp * n)(*[_chk(j[1], F32, "scratch") for j in jobs]),
+              (vp * n)(*[_opt(j[2], F32, "out") for j in jobs]), (vp * n)(*[_opt(j[3], F32, "colsum") for j in jobs]),
+              (ctypes.c_int64 * n)(*[j[4] for j in jobs]), (ci * n)(*[j[5] for j in jobs]),
+              (ci * n)(*[j[6] for j in jobs]), (ci * n)(*[j[7] for j in jobs]), _stream(), kernels=int(n > 0))
+
+
+# ------------------------------------------------------------------------------------------ K1 synthetic envs
+def synth_env_num_ctas(N):
+    return int(_lib.load().trl_synth_env_num_ctas(int(N)))
+
+
+def synth_env_seed(seeds, episode, seed, n_total, first_env):
+    """VecEnv.seed: env i of this shard gets seed * n_total + first_env + i; episode counters restart."""
+    _lib.call("trl_synth_env_seed", _chk(seeds, I32, "seeds"), _chk(episode, I32, "episode"), seeds.numel(),
+              int(seed) & 0xFFFFFFFF, int(n_total) & 0xFFFFFFFF, int(first_env) & 0xFFFFFFFF, _stream())
+
+
+def synth_env_reset(state, elapsed, episode, seeds, mask, init_scale):
+    """New episodes for every env (mask None) or the envs whose uint8 mask is set; state (N, o)."""
+    N, o = state.shape
+    _lib.call("trl_synth_env_reset", _chk(state, F32, "state"), _chk(elapsed, I32, "elapsed"),
+              _chk(episode, I32, "episode"), _chk(seeds, I32, "seeds"), _opt(mask, U8, "mask"), N, o,
+              float(init_scale), _stream())
+
+
+def synth_env_step(state, actions, A, B, c, lb, ub, elapsed, step_count, reward, done, time_limit, partial, batch_sums,
+                   norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, rho, eta, ctrl_cost, term_thr,
+                   reward_scale, max_episode_steps, max_episode_frames, merge_stats):
+    """One step of all N envs (csrc/env_step.cu): state (N, o) in place, actions (N, a).  partial / batch_sums /
+    norm_*: the observation-normaliser moments (all None: not estimated); step_count / t_ptr: the collector's step
+    counters and ring row (None outside a collector)."""
+    N, o = state.shape
+    _lib.call("trl_synth_env_step", _chk(state, F32, "state"), _chk(actions, F32, "actions"), _chk(A, F32, "A"),
+              _chk(B, F32, "B"), _chk(c, F32, "c"), _chk(lb, F32, "lb"), _chk(ub, F32, "ub"),
+              _chk(elapsed, I32, "elapsed"), _opt(step_count, I32, "step_count"), _chk(reward, F32, "reward"),
+              _chk(done, U8, "done"), _chk(time_limit, U8, "time_limit"), _opt(partial, F64, "partial"),
+              _opt(batch_sums, F64, "batch_sums"), _opt(norm_mean, F64, "norm_mean"), _opt(norm_var, F64, "norm_var"),
+              _opt(norm_count, F64, "norm_count"), _chk(ticket, I32, "ticket"), _chk(any_reset, I32, "any_reset"),
+              _opt(t_ptr, I32, "t_ptr"), N, o, actions.numel() // N, float(rho), float(eta), float(ctrl_cost),
+              float(term_thr), float(reward_scale), int(max_episode_steps), int(max_episode_frames),
+              int(bool(merge_stats)), _stream())
+
+
+def synth_atari_reset(obs, latent, elapsed, episode, seeds, mask=None, zero_is_mask=None, episode_bias=0, bump=1):
+    """New episodes for every env, the envs of the uint8 `mask`, or those whose int32 `zero_is_mask` entry is 0."""
+    _lib.call("trl_synth_atari_reset", _chk(obs, U8, "obs"), _chk(latent, I32, "latent"), _chk(elapsed, I32, "elapsed"),
+              _chk(episode, I32, "episode"), _chk(seeds, I32, "seeds"), _opt(mask, U8, "mask"),
+              _opt(zero_is_mask, I32, "zero_is_mask"), int(episode_bias), int(bump), obs.shape[0], _stream())
+
+
+def synth_atari_step(obs, latent, actions, elapsed, reward, done, time_limit, max_steps):
+    """One step of all envs: obs (N, 4, 84, 84) uint8 in place, actions (N) float action indices."""
+    _lib.call("trl_synth_atari_step", _chk(obs, U8, "obs"), _chk(latent, I32, "latent"), _chk(actions, F32, "actions"),
+              _chk(elapsed, I32, "elapsed"), _chk(reward, F32, "reward"), _chk(done, U8, "done"),
+              _chk(time_limit, U8, "time_limit"), obs.shape[0], int(max_steps), _stream())
+
+
+def u8_to_f32(x, scale, out=None):
+    """out = x * scale as float32."""
+    if out is None:
+        out = torch.empty(x.shape, dtype=F32, device=x.device)
+    assert out.numel() == x.numel()
+    _lib.call("trl_u8_to_f32", _chk(x, U8, "x"), _chk(out, F32, "out"), x.numel(), float(scale), _stream())
+    return out
+
+
+# ------------------------------------------------------------------------------------------ frame-stack ring
+def frame_ring_write(stack, ring, top, age=None, elapsed=None, hist=None, hist_count=None, size=None):
+    """Newest frame of every env's (N, C, ...) uint8 stack -> row *top of ring (T, N, F); age / elapsed: also the age
+    byte min(elapsed, C-1); hist / hist_count / size: the (C-1)-deep history of overwritten frames (csrc/frames.cu)."""
+    T, N, F = ring.shape
+    C = stack.shape[1]
+    assert stack.numel() == N * C * F
+    _lib.call("trl_frame_ring_write", _chk(stack, U8, "stack"), _chk(ring, U8, "ring"), _opt(age, U8, "age"),
+              _opt(elapsed, I32, "elapsed"), _opt(hist, U8, "hist"), _opt(hist_count, I32, "hist_count"),
+              _chk(top, I32, "top"), _opt(size, I32, "size"), N, C, F, T, C - 1, _stream())
+
+
+def frame_hist_advance(hist_count, size, T):
+    """Once per step after the step's frame_ring_write calls."""
+    _lib.call("trl_frame_hist_advance", _chk(hist_count, I32, "hist_count"), _chk(size, I32, "size"), int(T), _stream())
+
+
+def frame_stack_gather(obs_last, next_last, age, hist, hist_count, idx, rows, top, size, scale, out_obs, out_next,
+                       pos=None):
+    """out_obs / out_next (rows*N, C, ...) f32 = scale * the frame stacks of ring rows idx[pos*rows + k] (pos None:
+    idx[k]), rebuilt from the de-duplicated ring: obs_last / next_last (T, N, F), hist (C-1, N, F)."""
+    T, N, F = obs_last.shape
+    C = hist.shape[0] + 1
+    _lib.call("trl_frame_stack_gather", _chk(obs_last, U8, "obs_last"), _chk(next_last, U8, "next_last"),
+              _chk(age, U8, "age"), _chk(hist, U8, "hist"), _chk(hist_count, I32, "hist_count"), _chk(idx, I64, "idx"),
+              _opt(pos, I32, "pos"), int(rows), _chk(top, I32, "top"), _chk(size, I32, "size"), N, C, F, T,
+              float(scale), _chk(out_obs, F32, "out_obs"), _chk(out_next, F32, "out_next"), _stream(),
+              kernels=int(rows > 0))
+
+
+# ------------------------------------------------------------------------------------------ K12 peer communication
+# Host-side management of the peer-mapped communication blocks (no kernel launches) and the collectives of
+# csrc/comm.cu.  peer_* / flags: host arrays of `world` device pointers (distributed.PeerComm.region).
+def comm_sizes():
+    """(flag pad bytes, cudaIpc handle bytes)."""
+    lib = _lib.load()
+    return int(lib.trl_comm_flag_bytes()), int(lib.trl_comm_ipc_handle_bytes())
+
+
+def comm_scratch_doubles(nseg):
+    return int(_lib.load().trl_comm_scratch_doubles(int(nseg)))
+
+
+def comm_ll_recv_bytes(world, nmax):
+    return int(_lib.load().trl_comm_ll_recv_bytes(int(world), int(nmax)))
+
+
+def comm_alloc(nbytes):
+    """Device address of a new zeroed communication block of `nbytes`."""
+    ptr = ctypes.c_void_p()
+    _lib.check(_lib.load().trl_comm_alloc(int(nbytes), ctypes.byref(ptr)), "trl_comm_alloc")
+    return ptr.value
+
+
+def comm_ipc_get(ptr):
+    """The cudaIpc handle (bytes) of a block made by comm_alloc."""
+    handle = ctypes.create_string_buffer(comm_sizes()[1])
+    _lib.check(_lib.load().trl_comm_ipc_get(ptr, handle), "trl_comm_ipc_get")
+    return handle.raw
+
+
+def comm_ipc_open(handle):
+    """This process's device address of a peer's block, from its comm_ipc_get handle."""
+    ptr = ctypes.c_void_p()
+    _lib.check(_lib.load().trl_comm_ipc_open(ctypes.create_string_buffer(bytes(handle), len(handle)),
+                                             ctypes.byref(ptr)), "trl_comm_ipc_open")
+    return ptr.value
+
+
+def allreduce_grad(peer_data, flags, rank, world, out, seg_begin, nseg, mask, sumsq3, step_counts, betas, scratch,
+                   ticket, seq, zero_local=True):
+    """out = the sum over ranks of the peers' flat gradients, with what grad_sumsq computes for it; zero_local: this
+    rank's gradient is zeroed once every peer has read it."""
+    _lib.call("trl_allreduce_grad", peer_data, flags, int(rank), int(world), _chk(out, F32, "out"), out.numel(),
+              seg_begin, int(nseg), int(mask), _chk(sumsq3, F64, "sumsq3"), _chk(step_counts, I32, "step_counts"),
+              float(betas[0]), float(betas[1]), _chk(scratch, F64, "scratch"), _chk(ticket, I32, "ticket"),
+              _chk(seq, I32, "seq"), int(bool(zero_local)), _stream())
+
+
+def allreduce_f64(peer_data, flags, rank, world, out, n, gather, seq):
+    """out = the sum over ranks (gather: the (world, n) stack) of the first n doubles of the peers' regions."""
+    _lib.call("trl_allreduce_f64", peer_data, flags, int(rank), int(world), _chk(out, F64, "out"), int(n),
+              int(bool(gather)), _chk(seq, I32, "seq"), _stream())
+    return out
+
+
+def allreduce_f64_ll(local, peer_recv, rank, world, out, n, nmax, gather, ll_seq):
+    """allreduce_f64 for n <= nmax doubles of `local` in one NVLink traversal (flag-carrying packets)."""
+    _lib.call("trl_allreduce_f64_ll", _chk(local, F64, "local"), peer_recv, int(rank), int(world),
+              _chk(out, F64, "out"), int(n), int(nmax), int(bool(gather)), _chk(ll_seq, I32, "ll_seq"), _stream())
     return out

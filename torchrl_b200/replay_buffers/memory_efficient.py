@@ -11,7 +11,7 @@ already overwritten (a C-1 deep history of overwritten frames) -- and hands them
 """
 import torch
 
-from .. import _lib, ops
+from .. import ops
 from .base import BaseReplayBuffer
 
 U8, I32, F32 = torch.uint8, torch.int32, torch.float32
@@ -48,18 +48,13 @@ class MemoryEfficientReplayBuffer(BaseReplayBuffer):
 
     def write_obs(self, stack_u8, elapsed):
         """Collector step, before env.step: newest frame of the (N, C, H, W) stack -> row `_top` (+ age, history)."""
-        _lib.call("trl_frame_ring_write", ops._chk(stack_u8, U8, "stack"), self._obs.data_ptr(), self._age.data_ptr(),
-                  ops._chk(elapsed, I32, "elapsed"), self._hist.data_ptr(), self._hist_count.data_ptr(),
-                  self._top_dev.data_ptr(), self._size_dev.data_ptr(), self.env_nums, self._C, self._F,
-                  self._max_replay_buffer_size, self._C - 1, ops._stream())
-        _lib.call("trl_frame_hist_advance", self._hist_count.data_ptr(), self._size_dev.data_ptr(),
-                  self._max_replay_buffer_size, ops._stream())
+        ops.frame_ring_write(stack_u8, self._obs, self._top_dev, age=self._age, elapsed=elapsed, hist=self._hist,
+                             hist_count=self._hist_count, size=self._size_dev)
+        ops.frame_hist_advance(self._hist_count, self._size_dev, self._max_replay_buffer_size)
 
     def write_next_obs(self, stack_u8):
         """Collector step, after env.step: newest frame of the new stack -> row `_top`."""
-        _lib.call("trl_frame_ring_write", ops._chk(stack_u8, U8, "stack"), self._next_obs.data_ptr(), None, None, None,
-                  None, self._top_dev.data_ptr(), None, self.env_nums, self._C, self._F, self._max_replay_buffer_size,
-                  self._C - 1, ops._stream())
+        ops.frame_ring_write(stack_u8, self._next_obs, self._top_dev)
 
     def add_sample(self, sample_dict, episode_steps=None, **kwargs):
         """Reference-style row insertion with full (N, C, H, W) uint8 stacks under "obs" / "next_obs".
@@ -94,11 +89,8 @@ class MemoryEfficientReplayBuffer(BaseReplayBuffer):
                 shape = (rows * self.env_nums,) + self._stack
                 bufs = self._stack_cache[rows] = (torch.empty(shape, dtype=F32, device=self.device),
                                                   torch.empty(shape, dtype=F32, device=self.device))
-            _lib.call("trl_frame_stack_gather", self._obs.data_ptr(), self._next_obs.data_ptr(), self._age.data_ptr(),
-                      self._hist.data_ptr(), self._hist_count.data_ptr(), ops._chk(indices, torch.int64, "indices"),
-                      None if pos_ptr is None else ops._chk(pos_ptr, I32, "pos"), rows, self._top_dev.data_ptr(),
-                      self._size_dev.data_ptr(), self.env_nums, self._C, self._F, self._max_replay_buffer_size,
-                      self.obs_scale, bufs[0].data_ptr(), bufs[1].data_ptr(), ops._stream())
+            ops.frame_stack_gather(self._obs, self._next_obs, self._age, self._hist, self._hist_count, indices, rows,
+                                   self._top_dev, self._size_dev, self.obs_scale, bufs[0], bufs[1], pos=pos_ptr)
             if "obs" in frame_keys:
                 out["obs"] = bufs[0]
             if "next_obs" in frame_keys:
