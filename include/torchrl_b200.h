@@ -163,6 +163,27 @@ int trl_ppo_categorical_actor_loss(const float* logits, const float* actions, co
                                    const float* adv_stats, const int* adv_stats_pos, int64_t B, int num_actions,
                                    float clip_para, float entropy_coeff, float* g_logits, float* logp_out,
                                    float* info16, double* scratch, unsigned* ticket, void* stream);
+/* V-MPO's top-half selection (algo/on_policy/v_mpo.py:65-71: torch.sort(advs, descending) then idx.chunk(2)[0]) for
+ * `groups` minibatches in one launch.  Minibatch u is the time rows perm[u*b .. (u+1)*b) x row_elems envs in
+ * trl_row_gather order (perm NULL: rows 0..b-1, the explicit vector of eager updates); its B = b * row_elems
+ * advantages are normalised with stats4 row u, advn = (adv - mean) / (std + 1e-5), and the positions of the
+ * k = B - B/2 largest (ties: the lower position first) are written to sel (groups, k) in ascending order.
+ * 1 <= B < 2^31. */
+int trl_vmpo_select(const float* advs, const int64_t* perm, int groups, int b, int64_t row_elems, const float* stats4,
+                    int64_t* sel, void* stream);
+int64_t trl_vmpo_categorical_scratch_doubles(int64_t k);
+/* V-MPO's actor loss for a categorical policy on the k selected rows (v_mpo.py:73-99 with
+ * CategoricalDisPolicy.update, policies/discrete_policies.py:156-167 and torch's categorical KL):
+ * phi = softmax(advn / eta), L = mean(-phi * logp) + alpha * K + eta * eta_eps + eta * log(mean(exp(advn / eta)))
+ * + alpha * alpha_eps - alpha * K, with K = sum_i KL_i (per_row_kl = 0: the reference's summed KL) or mean_i KL_i
+ * (per_row_kl = 1).  dual (2) = [eta, alpha] on the device.  Writes dL/dlogits (k, A), g_dual (2) = [dL/deta,
+ * dL/dalpha] and info12 = [policy_loss, alpha_loss, -, -, logprob mean, std, max, min, KL mean, std, max, min]
+ * (the summed KL logs K, NaN, K, K).  The log-mean-exp subtracts the maximum. */
+int trl_vmpo_categorical_loss(const float* logits, const float* target_logits, const float* actions,
+                              const float* advs, const float* adv_stats, const int* adv_stats_pos, const float* dual,
+                              int64_t k, int num_actions, float eta_eps, float alpha_eps, int per_row_kl,
+                              float* g_logits, float* g_dual, float* info12, double* scratch, unsigned* ticket,
+                              void* stream);
 
 /* ---- K11: flat-buffer grad-norm clip + Adam, Polyak (algo/utils.py:16-25, ppo.py:72-74,117-119). */
 int trl_grad_sumsq_blocks(int nseg);

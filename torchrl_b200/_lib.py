@@ -58,6 +58,9 @@ SIGNATURES = {
     "trl_categorical_log_prob": [vp, vp, i64, i32, vp, vp],
     "trl_ppo_categorical_actor_scratch_doubles": [i64],
     "trl_ppo_categorical_actor_loss": [vp, vp, vp, vp, vp, vp, i64, i32, f32, f32, vp, vp, vp, vp, vp, vp],
+    "trl_vmpo_select": [vp, vp, i32, i32, i64, vp, vp, vp],
+    "trl_vmpo_categorical_scratch_doubles": [i64],
+    "trl_vmpo_categorical_loss": [vp, vp, vp, vp, vp, vp, vp, i64, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
     "trl_grad_sumsq_blocks": [i32],
     "trl_grad_sumsq": [vp, vp, i32, u32, vp, vp, f64, f64, vp, vp, vp],
     "trl_adam_step": [vp, vp, vp, vp, vp, i32, u32, vp, vp, vp, vp, f32, f32, f32, i32, vp, vp, vp],
@@ -121,13 +124,15 @@ SIGNATURES = {
 }
 _RESTYPES = {"trl_last_error": ctypes.c_char_p, "trl_ppo_actor_scratch_doubles": ctypes.c_int64,
              "trl_ppo_categorical_actor_scratch_doubles": ctypes.c_int64,
+             "trl_vmpo_categorical_scratch_doubles": ctypes.c_int64,
              "trl_offpolicy_scratch_doubles": ctypes.c_int64, "trl_bias_act_bwd_scratch_floats": ctypes.c_int64,
              "trl_skinny_tn_scratch_floats": ctypes.c_int64,
              "trl_skinny_dgrad_act_scratch_floats": ctypes.c_int64, "trl_comm_ll_recv_bytes": ctypes.c_int64}
 # entry points that return a value rather than an error code
 _VALUE_FUNCS = ("trl_abi_version", "trl_synth_env_smem_bytes", "trl_synth_env_num_ctas", "trl_comm_flag_bytes",
                 "trl_comm_ipc_handle_bytes", "trl_comm_scratch_doubles", "trl_comm_ll_recv_bytes",
-                "trl_ppo_actor_scratch_doubles", "trl_ppo_categorical_actor_scratch_doubles", "trl_grad_sumsq_blocks")
+                "trl_ppo_actor_scratch_doubles", "trl_ppo_categorical_actor_scratch_doubles", "trl_vmpo_categorical_scratch_doubles",
+                "trl_grad_sumsq_blocks")
 
 _lib = None
 

@@ -127,6 +127,25 @@ class CategoricalHead:
     def old_log_prob(self, pf, obs, acts, out):
         return ops.categorical_log_prob(self._logits(pf, obs), acts.reshape(-1).contiguous(), out=out)
 
+    # ---- V-MPO (v_mpo.py:57-133)
+    def vmpo_scratch(self, B, device):
+        return ops.VMPOScratch(B - B // 2, device)
+
+    def vmpo_actor(self, pf, target_pf, obs, acts, advs, adv_stats, stats_pos, dual, eta_eps, alpha_eps, per_row_kl,
+                   scratch, info, fork=False):
+        """The actor step on the k selected rows: both policies' logits on those rows only, one loss kernel that writes
+        dL/d[eta, alpha] straight into the duals' slice of the flat gradient, autograd through the policy's logits."""
+        logits = self._logits(pf, obs)
+        with torch.no_grad():
+            tlogits = self._logits(target_pf, obs)
+        g = ops.vmpo_categorical_loss(logits, tlogits, acts.reshape(-1), advs.reshape(-1), adv_stats, dual.detach(),
+                                      eta_eps, alpha_eps, per_row_kl, scratch, dual.grad, info, stats_pos=stats_pos)
+        if fork:
+            with fused.backward_fork():
+                torch.autograd.backward([logits], [g])
+        else:
+            torch.autograd.backward([logits], [g])
+
 
 def policy_head(pf):
     from ...policies.discrete_policies import CategoricalDisPolicy

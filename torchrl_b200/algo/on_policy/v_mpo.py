@@ -8,6 +8,12 @@ multiplier alpha by their dual losses, clamp both at 1e-8.  The MLPs run on the 
 per-sample loss assembly (sort, softmax, KL) is a handful of elementwise torch ops inside the captured graph.
 eta and alpha live in one 2-element parameter optimised by a third segment of the flat Adam (lr = plr, eps = 1e-5,
 no clipping: v_mpo.py:33-37).
+
+With a CategoricalDisPolicy the actor step runs on the library's kernels instead (csrc/categorical.cu): one launch per
+epoch selects the top half of every minibatch (`_epoch_adv_stats`), and one launch per minibatch computes the loss,
+its gradient wrt the selected rows' logits and the duals' gradient.  reference_quirks=True keeps the reference's
+summed KL: for a Categorical, kl_divergence(...).sum(-1, keepdim=True) sums over the rows (one scalar K that enters
+every row's loss and the alpha loss); False uses the per-row KL of the Gaussian path and the V-MPO paper.
 """
 import copy
 
@@ -17,13 +23,16 @@ import torch
 from ... import ops
 from ...flat import FlatParams
 from .a2c import A2C, _ADV_KEYS
+from .policy_heads import CategoricalHead
 
 _STAT = ("mean", "std", "max", "min")
 
 
 class VMPO(A2C):
-    def __init__(self, pf, opt_epochs=10, eta_eps=0.02, alpha_eps=0.1, clipped_value_loss=False, **kwargs):
+    def __init__(self, pf, opt_epochs=10, eta_eps=0.02, alpha_eps=0.1, clipped_value_loss=False,
+                 reference_quirks=True, **kwargs):
         self.target_pf = copy.deepcopy(pf)
+        self.reference_quirks = reference_quirks
         self.eta_eps, self.alpha_eps = eta_eps, alpha_eps
         self.opt_epochs = opt_epochs
         dev = torch.device(kwargs.get("device", "cuda"))
@@ -31,6 +40,7 @@ class VMPO(A2C):
         super().__init__(pf=pf, **kwargs)
         self.sample_key = ["obs", "acts", "advs", "estimate_returns", "values"]
         self._target_flat = FlatParams([self.target_pf], device=self.device)
+        self._categorical = isinstance(self._head, CategoricalHead)
 
     @property
     def eta(self):
@@ -82,6 +92,14 @@ class VMPO(A2C):
 
     def _actor_step(self, batch, info):
         st = self._mb_state
+        if self._categorical:
+            sel = st["sel"].index_select(0, st["upd"].long()).reshape(-1)        # this minibatch's top half
+            self._head.vmpo_actor(self.pf, self.target_pf, batch["obs"].index_select(0, sel),
+                                  batch["acts"].reshape(-1).index_select(0, sel),
+                                  batch["advs"].reshape(-1).index_select(0, sel), st["adv_table"], st["upd"], self.dual,
+                                  self.eta_eps, self.alpha_eps, not self.reference_quirks, st["vmpo_scratch"],
+                                  info[32:44], fork=True)
+            return
         row = st["adv_table"].index_select(0, st["upd"].long())                  # this minibatch's statistics
         advn = (batch["advs"].reshape(-1, 1) - row[:, 0:1]) / (row[:, 1:2] + 1e-5)
         acts = batch["acts"].reshape(advn.shape[0], -1)
@@ -102,7 +120,18 @@ class VMPO(A2C):
     def _mb_setup(self):
         st = super()._mb_setup()
         st["dual_log"] = torch.zeros(st["U"], 2, dtype=torch.float32, device=self.device)
+        if self._categorical:
+            B = st["B"]
+            st["sel"] = torch.zeros(st["U"], B - B // 2, dtype=torch.int64, device=self.device)
+            st["vmpo_scratch"] = self._head.vmpo_scratch(B, self.device)
         return st
+
+    def _epoch_adv_stats(self):
+        super()._epoch_adv_stats()
+        if self._categorical:                  # every minibatch's top half, once per epoch
+            st, rb = self._mb_state, self.replay_buffer
+            ops.vmpo_select(rb._advs.reshape(rb._advs.shape[0], -1), st["adv_table"], st["U"], st["b"],
+                            perm=st["perm"], out=st["sel"])
 
     def _flush_infos(self, n_updates):
         self._dual_rows = self._mb_state["dual_log"][:n_updates].cpu().numpy()
@@ -139,8 +168,16 @@ class VMPO(A2C):
             v = self.vf(obs)
             g_v, _ = ops.ppo_critic_loss(v.reshape(-1), rets.reshape(-1), None, False, 0.0, scratch, info=info[16:17])
             torch.autograd.backward([v], [g_v.reshape(v.shape)])
-            advn = (advs.reshape(-1, 1) - stats[0]) / (stats[1] + 1e-5)
-            self._actor_loss(obs, acts, advn, info).backward()
+            if self._categorical:
+                a = advs.reshape(-1)
+                sel = ops.vmpo_select(a, stats, 1, B).reshape(-1)
+                self._head.vmpo_actor(self.pf, self.target_pf, obs.index_select(0, sel),
+                                      acts.reshape(-1).index_select(0, sel), a.index_select(0, sel), stats, None,
+                                      self.dual, self.eta_eps, self.alpha_eps, not self.reference_quirks,
+                                      self._head.vmpo_scratch(B, self.device), info[32:44])
+            else:
+                advn = (advs.reshape(-1, 1) - stats[0]) / (stats[1] + 1e-5)
+                self._actor_loss(obs, acts, advn, info).backward()
             scale, fused_norm = 1.0, False
             if self.dist is not None:
                 scale, fused_norm = self.dist.reduce_grads(self.opt)

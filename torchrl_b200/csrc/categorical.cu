@@ -6,6 +6,8 @@
 //   (softmax, torch.distributions.Categorical(probs).sample / log_prob / entropy)
 //   the actor half of PPO.update_actor                 /root/reference/torchrl/algo/on_policy/ppo.py:41-91
 //   and of A2C.update                                  /root/reference/torchrl/algo/on_policy/a2c.py:45-112
+//   VMPO.update_actor for this policy (top-half selection, loss, dual gradients)
+//                                                      /root/reference/torchrl/algo/on_policy/v_mpo.py:57-133
 // The distribution is torch's Categorical(probs=softmax(x)): p = softmax(x) (maximum subtracted, then renormalised as
 // Categorical does), l_j = log(clamp(p_j, eps, 1-eps)) (probs_to_logits, NOT log_softmax), log_prob(a) = l_a,
 // entropy = -sum_j p_j l_j.  Gradients wrt x, with m_j = 1 where the clamp passes (eps <= p_j <= 1-eps):
@@ -137,6 +139,29 @@ __global__ void categorical_logprob_kernel(const float* __restrict__ logits, con
 }
 
 // ------------------------------------------------------------------------------------ actor loss
+// The last CTA's fold of the per-CTA partials (NP quantities per CTA, the first NS sums, the rest maxima) into tot:
+// warp w folds quantities w, w + 8, ...; lane l takes partials l, l+32, ... then a fixed shuffle tree.  Ends with a
+// barrier, after which tot is valid in every thread.
+template <int NP, int NS>
+__device__ __forceinline__ void cat_fold_partials(const double* __restrict__ partial, double* tot) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int k = wid; k < NP; k += kCatThreads / 32) {
+    const bool is_max = k >= NS;
+    double acc = is_max ? -INFINITY : 0.0;
+    for (unsigned i = lane; i < gridDim.x; i += 32) {
+      const double v = __ldcg(partial + static_cast<long long>(i) * NP + k);
+      acc = is_max ? fmax(acc, v) : acc + v;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const double w = __shfl_xor_sync(0xffffffffu, acc, o);
+      acc = is_max ? fmax(acc, w) : acc + w;
+    }
+    if (lane == 0) tot[k] = acc;
+  }
+  __syncthreads();
+}
+
 struct CatLossParams {
   const float* __restrict__ logits;     // (B,A)
   const float* __restrict__ actions;    // (B) index as float
@@ -223,24 +248,8 @@ __global__ void __launch_bounds__(kCatThreads) ppo_categorical_actor_loss_kernel
                          ok ? -ratio : -INFINITY};
   block_partials<kCatThreads / 32>(sums, maxs, sh_d, sh_f, p.partial + static_cast<long long>(blockIdx.x) * kCatPartials);
   if (!last_cta(p.ticket, gridDim.x)) return;
-  // last CTA: warp w folds quantities w and w + 8; lane l takes partials l, l+32, ... then a fixed shuffle tree
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   __shared__ double tot[kCatPartials];
-  for (int k = wid; k < kCatPartials; k += kCatThreads / 32) {
-    const bool is_max = k >= 5;
-    double acc = is_max ? -INFINITY : 0.0;
-    for (unsigned i = lane; i < gridDim.x; i += 32) {
-      const double v = __ldcg(p.partial + static_cast<long long>(i) * kCatPartials + k);
-      acc = is_max ? fmax(acc, v) : acc + v;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double w = __shfl_xor_sync(0xffffffffu, acc, o);
-      acc = is_max ? fmax(acc, w) : acc + w;
-    }
-    if (lane == 0) tot[k] = acc;
-  }
-  __syncthreads();
+  cat_fold_partials<kCatPartials, 5>(p.partial, tot);
   if (threadIdx.x == 0) {
     const double Bn = static_cast<double>(p.B);
     const double ent_mean = tot[3] / Bn;
@@ -256,6 +265,245 @@ __global__ void __launch_bounds__(kCatThreads) ppo_categorical_actor_loss_kernel
     for (int k = 7; k < 11; ++k) p.info[k] = 0.f;  // the log-std slots of the Gaussian kernel
     p.info[11] = static_cast<float>(ent_mean);
     p.info[12] = static_cast<float>(tot[4] / Bn);
+  }
+}
+
+// ------------------------------------------------------------------------------------ V-MPO
+// Top-half selection (v_mpo.py:65-67): of a minibatch's B normalised advantages keep the k = B - B/2 largest, ties to
+// the lower position (torch.sort(stable=True) then chunk(2)[0]).  One CTA per minibatch: an MSB-first radix select
+// over a descending-order key (4 passes of 8-bit histograms in shared memory) finds the key of the k-th largest value
+// and how many of the values equal to it are kept; one ordered pass then writes the kept positions in ascending order
+// with block-wide ballot scans.  Every pass reads the same values, so the counts are consistent whatever they are (NaN
+// included) and the kernel always finishes.
+constexpr int kSelThreads = 1024;
+
+// minibatch position q of group u: time row perm[u*b + q / n] (row q / n if perm is null), env q % n -- the order of
+// gather_rows -- normalised exactly as the loss normalises it
+// (B < 2^31: 32-bit division, which compiles inline)
+__device__ __forceinline__ float vmpo_advn(const float* __restrict__ advs, const long long* __restrict__ perm,
+                                           long long base, unsigned n, unsigned q, float mean, float den) {
+  const unsigned t = q / n;
+  const long long r = perm ? perm[base + t] : static_cast<long long>(t);
+  return (advs[r * n + (q - t * n)] - mean) / den;
+}
+
+// key(a) < key(b) iff a > b as floats; -0 and +0 share a key (they compare equal in torch.sort)
+__device__ __forceinline__ unsigned vmpo_desc_key(float v) {
+  if (v == 0.f) v = 0.f;
+  const unsigned x = __float_as_uint(v);
+  return (x & 0x80000000u) ? x : ~(x | 0x80000000u);
+}
+
+__global__ void __launch_bounds__(kSelThreads) vmpo_select_kernel(const float* __restrict__ advs,
+                                                                  const long long* __restrict__ perm, int b,
+                                                                  unsigned n, const float* __restrict__ stats,
+                                                                  long long* __restrict__ sel, unsigned k) {
+  __shared__ unsigned hist[256];
+  __shared__ unsigned s_prefix, s_need;
+  __shared__ unsigned s_cnt[2][kSelThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const unsigned B = static_cast<unsigned>(b) * n;
+  const long long base = static_cast<long long>(blockIdx.x) * b;
+  const float mean = stats[4LL * blockIdx.x], den = stats[4LL * blockIdx.x + 1] + 1e-5f;
+  unsigned prefix = 0u, need = k;  // need: 1-based rank of the k-th key among those matching
+  if (tid == 0) { s_prefix = 0u; s_need = need; }
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += kSelThreads) hist[i] = 0u;
+    __syncthreads();
+    const unsigned hi = shift == 24 ? 0u : (0xFFFFFFFFu << (shift + 8));
+    for (unsigned q = tid; q < B; q += kSelThreads) {
+      const unsigned key = vmpo_desc_key(vmpo_advn(advs, perm, base, n, q, mean, den));
+      if ((key & hi) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (wid == 0) {  // lane l owns bins 8l .. 8l+7: a warp scan finds the bin holding rank `need`
+      unsigned c[8], s = 0u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { c[j] = hist[lane * 8 + j]; s += c[j]; }
+      unsigned incl = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+      }
+      const unsigned ball = __ballot_sync(0xffffffffu, incl >= need);
+      if (ball != 0u && lane == __ffs(ball) - 1) {
+        unsigned acc = incl - s;
+        int jb = 7;
+#pragma unroll
+        for (int j = 7; j >= 0; --j) {  // the first bin whose running count reaches `need`, in registers
+          unsigned before = acc;
+#pragma unroll
+          for (int m = 0; m < j; ++m) before += c[m];
+          if (before + c[j] >= need) jb = j;
+        }
+#pragma unroll
+        for (int m = 0; m < 8; ++m) acc += m < jb ? c[m] : 0u;
+        s_prefix = prefix | (static_cast<unsigned>(lane * 8 + jb) << shift);
+        s_need = need - acc;
+      }
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    need = s_need;
+  }
+  // keep key < prefix, and the first `need` positions with key == prefix
+  const unsigned lt_mask = (1u << lane) - 1u;
+  unsigned eq_base = 0u, out_base = 0u;
+  for (unsigned q0 = 0; q0 < B && out_base < k; q0 += kSelThreads) {
+    const unsigned q = q0 + tid;
+    bool lt = false, eq = false;
+    if (q < B) {
+      const unsigned key = vmpo_desc_key(vmpo_advn(advs, perm, base, n, q, mean, den));
+      lt = key < prefix;
+      eq = key == prefix;
+    }
+    const unsigned be = __ballot_sync(0xffffffffu, eq);
+    if (lane == 0) s_cnt[0][wid] = __popc(be);
+    __syncthreads();
+    unsigned eq_before = eq_base + __popc(be & lt_mask), eq_tot = 0u;
+    for (int w = 0; w < kSelThreads / 32; ++w) {
+      eq_before += w < wid ? s_cnt[0][w] : 0u;
+      eq_tot += s_cnt[0][w];
+    }
+    const bool take = lt || (eq && eq_before < need);
+    const unsigned bt = __ballot_sync(0xffffffffu, take);
+    if (lane == 0) s_cnt[1][wid] = __popc(bt);
+    __syncthreads();
+    unsigned pos = out_base + __popc(bt & lt_mask), t_tot = 0u;
+    for (int w = 0; w < kSelThreads / 32; ++w) {
+      pos += w < wid ? s_cnt[1][w] : 0u;
+      t_tot += s_cnt[1][w];
+    }
+    if (take && pos < k) sel[static_cast<long long>(blockIdx.x) * k + pos] = q;
+    eq_base += eq_tot;
+    out_base += t_tot;
+    __syncthreads();  // s_cnt is rewritten by the next chunk
+  }
+}
+
+// The categorical V-MPO actor loss on the k selected rows (v_mpo.py:69-99 with CategoricalDisPolicy.update,
+// discrete_policies.py:156-167), value and gradient in one launch.  phi = softmax(advn / eta) needs the maximum and
+// the sum of exp over all k rows before any row's gradient: every CTA computes both itself from the k advantages (the
+// same block reductions in the same order, so every CTA holds the same values), which saves a second launch.
+// KL_i = sum_j p_j (l_j - lq_j) as torch's _kl_categorical_categorical: a term with q_j == 0 is +inf (no gradient), a
+// term with p_j == 0 is 0.  With g_j = l_j - lq_j + m_j on the live terms (0 elsewhere),
+//   dKL_i / dz_k = p_k (g_k - sum_j p_j g_j),   dL/dz_i = -(phi_i / k) m_a (delta_a - p) + c dKL_i/dz_i,
+// c = alpha (the reference's summed KL, reference_quirks) or alpha / k (per-row KL).
+// per-CTA partials: [0] sum phi logp [1] sum logp [2] sum logp^2 [3] sum KL [4] sum KL^2 [5] sum phi advn
+// [6] max logp [7] max -logp [8] max KL [9] max -KL
+constexpr int kVmpoPartials = 10;
+
+struct VmpoLossParams {
+  const float* __restrict__ logits;     // (k,A)
+  const float* __restrict__ tlogits;    // (k,A) target policy
+  const float* __restrict__ actions;    // (k)
+  const float* __restrict__ advs;       // (k) raw advantages of the selected rows
+  const float* __restrict__ adv_stats;  // rows of [mean, std, max, min]
+  const int* __restrict__ stats_pos;    // device scalar: row of adv_stats (nullptr: row 0)
+  const float* __restrict__ dual;       // [eta, alpha]
+  float* __restrict__ g_logits;         // (k,A)
+  float* __restrict__ g_dual;           // (2)
+  float* __restrict__ info;             // (12)
+  double* __restrict__ partial;         // (grid, kVmpoPartials)
+  unsigned* __restrict__ ticket;
+  long long k;
+  int A;
+  float eta_eps, alpha_eps;
+  int per_row;
+};
+
+__global__ void __launch_bounds__(kCatThreads) vmpo_categorical_loss_kernel(const VmpoLossParams p) {
+  __shared__ double sh_d[kCatThreads / 32][6];
+  __shared__ float sh_f[kCatThreads / 32][4];
+  __shared__ double sh_sum[32];
+  __shared__ float sh_max[32];
+  __shared__ double s_norm[2];
+  const int A = p.A;
+  const float* st = p.adv_stats + (p.stats_pos ? 4LL * (*p.stats_pos) : 0LL);
+  const float mean = st[0], den = st[1] + 1e-5f;
+  const float eta = p.dual[0], alpha = p.dual[1];
+  // phi's normaliser over all k rows: M = max advn / eta, S = sum exp(advn / eta - M)
+  float mx = -INFINITY;
+  for (long long i = threadIdx.x; i < p.k; i += kCatThreads) mx = fmaxf(mx, ((p.advs[i] - mean) / den) / eta);
+  mx = block_reduce_max(mx, sh_max);
+  if (threadIdx.x == 0) s_norm[0] = mx;
+  __syncthreads();
+  mx = static_cast<float>(s_norm[0]);
+  double se = 0.0;
+  for (long long i = threadIdx.x; i < p.k; i += kCatThreads)
+    se += static_cast<double>(expf(((p.advs[i] - mean) / den) / eta - mx));
+  se = block_reduce_sum(se, sh_sum);
+  if (threadIdx.x == 0) s_norm[1] = se;
+  __syncthreads();
+  se = s_norm[1];
+
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const bool ok = i < p.k;
+  const float invk = 1.0f / static_cast<float>(p.k);
+  float logp = 0.f, kl = 0.f, phi = 0.f, advn = 0.f;
+  if (ok) {
+    // target row first, kept as lq and a bit mask of its zero probabilities
+    float pr[kCatMaxA], l[kCatMaxA], lq[kCatMaxA];
+    unsigned pass, qzero = 0u;
+    cat_row(p.tlogits + i * A, A, pr, lq, pass);
+#pragma unroll
+    for (int j = 0; j < kCatMaxA; ++j)
+      if (j < A && pr[j] == 0.f) qzero |= 1u << j;
+    cat_row(p.logits + i * A, A, pr, l, pass);
+    const int ai = cat_action(p.actions[i], A);
+    logp = cat_pick(l, A, ai);
+    advn = (p.advs[i] - mean) / den;
+    phi = static_cast<float>(static_cast<double>(expf(advn / eta - mx)) / se);
+    bool inf_term = false;
+    float spg = 0.f;
+#pragma unroll
+    for (int j = 0; j < kCatMaxA; ++j) {
+      if (j < A) {
+        const bool pz = pr[j] == 0.f, qz = (qzero >> j) & 1u;
+        inf_term |= qz && !pz;
+        const bool live = !pz && !qz;
+        l[j] -= lq[j];  // from here l holds l - lq
+        kl += live ? pr[j] * l[j] : 0.f;
+        spg += live ? pr[j] * (l[j] + ((pass >> j) & 1u ? 1.f : 0.f)) : 0.f;
+      }
+    }
+    if (inf_term) kl = INFINITY;
+    const float ca = (ai >= 0 && ((pass >> ai) & 1u)) ? -phi * invk : 0.f;  // dL/dlogp_i, times m_a
+    const float c = p.per_row ? alpha * invk : alpha;
+#pragma unroll
+    for (int j = 0; j < kCatMaxA; ++j) {
+      if (j < A) {
+        const bool live = pr[j] != 0.f && !((qzero >> j) & 1u);
+        const float gj = live ? l[j] + ((pass >> j) & 1u ? 1.f : 0.f) : 0.f;
+        p.g_logits[i * A + j] = ((j == ai ? ca : 0.f) - ca * pr[j]) + c * (pr[j] * (gj - spg));
+      }
+    }
+  }
+
+  const double sums[6] = {static_cast<double>(phi) * logp, static_cast<double>(logp),
+                          static_cast<double>(logp) * logp, static_cast<double>(kl), static_cast<double>(kl) * kl,
+                          static_cast<double>(phi) * advn};
+  const float maxs[4] = {ok ? logp : -INFINITY, ok ? -logp : -INFINITY, ok ? kl : -INFINITY, ok ? -kl : -INFINITY};
+  block_partials<kCatThreads / 32>(sums, maxs, sh_d, sh_f, p.partial + static_cast<long long>(blockIdx.x) * kVmpoPartials);
+  if (!last_cta(p.ticket, gridDim.x)) return;
+  __shared__ double tot[kVmpoPartials];
+  cat_fold_partials<kVmpoPartials, 6>(p.partial, tot);
+  if (threadIdx.x == 0) {
+    const double kn = static_cast<double>(p.k);
+    const double K = p.per_row ? tot[3] / kn : tot[3];  // what multiplies alpha
+    p.info[0] = static_cast<float>(-tot[0] / kn + static_cast<double>(alpha) * K);    // policy_loss
+    p.info[1] = static_cast<float>(static_cast<double>(alpha) * p.alpha_eps - static_cast<double>(alpha) * K);
+    stats_from_moments(tot[1], tot[2], tot[6], -tot[7], kn, p.info + 4);               // logprob/*
+    if (p.per_row) {
+      stats_from_moments(tot[3], tot[4], tot[8], -tot[9], kn, p.info + 8);            // KL/*
+    } else {  // the KL is one summed value: its std is torch's std of one element
+      p.info[8] = p.info[10] = p.info[11] = static_cast<float>(tot[3]);
+      p.info[9] = NAN;
+    }
+    const double lme = static_cast<double>(mx) + log(se / kn);  // log(mean(exp(advn / eta))), maximum subtracted
+    p.g_dual[0] = static_cast<float>(p.eta_eps + lme - tot[5] / eta);
+    p.g_dual[1] = static_cast<float>(p.alpha_eps - K);
   }
 }
 
@@ -309,4 +557,40 @@ TRL_API int trl_ppo_categorical_actor_loss(const float* logits, const float* act
   ppo_categorical_actor_loss_kernel<<<static_cast<unsigned>(ceil_div<long long>(B, kCatThreads)), kCatThreads, 0,
                                       static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("ppo_categorical_actor_loss_kernel");
+}
+
+TRL_API int trl_vmpo_select(const float* advs, const int64_t* perm, int groups, int b, int64_t row_elems,
+                            const float* stats4, int64_t* sel, void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(groups >= 1 && b >= 1 && row_elems >= 1 && static_cast<long long>(b) * row_elems < (1LL << 31),
+              "trl_vmpo_select: bad sizes groups=%d b=%d row_elems=%lld (B = b * row_elems >= 1, < 2^31)", groups, b,
+              (long long)row_elems);
+  TRL_REQUIRE(advs && stats4 && sel, "trl_vmpo_select: null pointer");
+  const long long B = static_cast<long long>(b) * row_elems;
+  vmpo_select_kernel<<<static_cast<unsigned>(groups), kSelThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      advs, reinterpret_cast<const long long*>(perm), b, static_cast<unsigned>(row_elems), stats4,
+      reinterpret_cast<long long*>(sel), static_cast<unsigned>(B - B / 2));
+  return check_launch("vmpo_select_kernel");
+}
+
+TRL_API int64_t trl_vmpo_categorical_scratch_doubles(int64_t k) {
+  return trl::ceil_div<long long>(k, trl::kCatThreads) * trl::kVmpoPartials;
+}
+
+TRL_API int trl_vmpo_categorical_loss(const float* logits, const float* target_logits, const float* actions,
+                                      const float* advs, const float* adv_stats, const int* adv_stats_pos,
+                                      const float* dual, int64_t k, int num_actions, float eta_eps, float alpha_eps,
+                                      int per_row_kl, float* g_logits, float* g_dual, float* info12, double* scratch,
+                                      unsigned* ticket, void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(k >= 1 && num_actions >= 1 && num_actions <= kCatMaxA,
+              "trl_vmpo_categorical_loss: bad sizes k=%lld A=%d (1 <= A <= %d)", (long long)k, num_actions, kCatMaxA);
+  TRL_REQUIRE(logits && target_logits && actions && advs && adv_stats && dual && g_logits && g_dual && info12 &&
+                  scratch && ticket,
+              "trl_vmpo_categorical_loss: null pointer");
+  VmpoLossParams p{logits, target_logits, actions, advs, adv_stats, adv_stats_pos, dual, g_logits, g_dual, info12,
+                   scratch, ticket, k, num_actions, eta_eps, alpha_eps, per_row_kl ? 1 : 0};
+  vmpo_categorical_loss_kernel<<<static_cast<unsigned>(ceil_div<long long>(k, kCatThreads)), kCatThreads, 0,
+                                 static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("vmpo_categorical_loss_kernel");
 }

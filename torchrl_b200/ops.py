@@ -370,6 +370,60 @@ def ppo_categorical_actor_loss(logits, actions, old_logp, advs, adv_stats, clip_
     return g_logits, info
 
 
+def vmpo_select(advs, stats, groups, b, perm=None, out=None):
+    """V-MPO's top half of every minibatch (v_mpo.py:65-71) in one launch: out (groups, k) int64, k = B - B // 2, the
+    ascending positions of the k largest normalised advantages of minibatch u (ties: lower position first), where
+    minibatch u is the time rows perm[u*b:(u+1)*b] of advs (rows, n) in gather_rows order, B = b * n, normalised with
+    stats row u.  perm None: advs holds one minibatch of B = b * n values in order (groups must be 1)."""
+    n = advs.numel() // advs.shape[0] if perm is not None else advs.numel() // b
+    B = b * n
+    if perm is None and groups != 1:
+        raise ValueError("vmpo_select without a permutation selects from one minibatch")
+    if stats.numel() < 4 * groups:
+        raise ValueError("vmpo_select needs a (groups, 4) statistics table")
+    if out is None:
+        out = torch.empty(groups, B - B // 2, dtype=I64, device=advs.device)
+    if out.numel() != groups * (B - B // 2):
+        raise ValueError("vmpo_select: out must hold (groups, B - B // 2) positions")
+    _lib.call("trl_vmpo_select", _chk(advs, F32, "advs"), _opt(perm, I64, "perm"), int(groups), int(b), int(n),
+              _chk(stats, F32, "stats"), _chk(out, I64, "sel"), _stream())
+    return out
+
+
+class VMPOScratch:
+    """Scratch + ticket of trl_vmpo_categorical_loss for up to k selected rows (allocated once)."""
+
+    def __init__(self, k, device):
+        n = int(_lib.load().trl_vmpo_categorical_scratch_doubles(int(k)))
+        self.partial = torch.zeros(max(n, 1), dtype=F64, device=device)
+        self.ticket = torch.zeros(1, dtype=I32, device=device)
+        self.k = int(k)
+
+
+def vmpo_categorical_loss(logits, target_logits, actions, advs, adv_stats, dual, eta_eps, alpha_eps, per_row_kl,
+                          scratch, g_dual, info, stats_pos=None, g_logits=None):
+    """The categorical V-MPO actor loss on the k selected rows (v_mpo.py:73-99): dL/dlogits (returned), dL/d[eta,
+    alpha] written into g_dual (2) -- the duals' slice of the flat gradient -- and info (12) = policy_loss,
+    alpha_loss, -, -, logprob/{mean,std,max,min}, KL/{mean,std,max,min}.  per_row_kl False: the reference's summed KL
+    (reference_quirks); True: the per-row KL."""
+    k, A = logits.shape
+    if target_logits.shape != logits.shape:
+        raise ValueError("target_logits must have the shape of logits")
+    if actions.numel() != k or advs.numel() != k or dual.numel() != 2 or g_dual.numel() != 2 or info.numel() < 12:
+        raise ValueError("vmpo_categorical_loss: (k) actions and advs, (2) dual and g_dual, (12) info")
+    if scratch.k < k:
+        raise ValueError("vmpo_categorical_loss: scratch sized for %d rows, got %d" % (scratch.k, k))
+    if g_logits is None:
+        g_logits = torch.empty_like(logits)
+    _lib.call("trl_vmpo_categorical_loss", _chk(logits, F32, "logits"), _chk(target_logits, F32, "target_logits"),
+              _chk(actions, F32, "actions"), _chk(advs, F32, "advs"), _chk(adv_stats, F32, "adv_stats"),
+              _opt(stats_pos, I32, "stats_pos"), _chk(dual, F32, "dual"), int(k), int(A), float(eta_eps),
+              float(alpha_eps), int(bool(per_row_kl)), _chk(g_logits, F32, "g_logits"), _chk(g_dual, F32, "g_dual"),
+              _chk(info, F32, "info"), _chk(scratch.partial, F64, "scratch"), _chk(scratch.ticket, I32, "ticket"),
+              _stream())
+    return g_logits
+
+
 def row_group_moments(x, idx, groups, b, out=None):
     """out (groups,4) f64 = sum, sum of squares, max, -min over the rows idx[u*b:(u+1)*b] of x (rows, n)."""
     n = x.numel() // x.shape[0]
