@@ -41,10 +41,9 @@ class BootstrappedDQN(DQN):
         grad, _ = ops.bootstrapped_dqn_loss(pred, next_q, acts, rewards, terminals, masks, self.discount,
                                             ub["scratch"], info=info[0:3])
         torch.autograd.backward([pred], [grad])
-        self._step()
+        self._optimizer_step()
         self._update_target_networks()
-        if self._explicit_batch is None:
-            self._finish_update()
+        self._finish_update()
 
     def _decode_info(self, row, variant):
         return {'Reward_Mean': float(row[2]), 'Training/qf_loss': float(row[0]), 'q_s_a': float(row[1])}

@@ -11,11 +11,8 @@ import torch
 import torch.optim as optim
 
 from ... import ops
-from ...flat import FlatAdam, FlatParams
-from ..rl_algo import SegmentOptimizer
+from ..utils import four_stats
 from .off_rl_algo import OffRLAlgo
-
-_STAT = ("mean", "std", "max", "min")
 
 
 class DDPG(OffRLAlgo):
@@ -27,16 +24,9 @@ class DDPG(OffRLAlgo):
         self.target_qf = copy.deepcopy(qf)
         self.to(self.device)
         self.plr, self.qlr = plr, qlr
-        if optimizer_class is not optim.Adam:
-            raise NotImplementedError("torchrl_b200 fuses clip+Adam in CUDA; only optim.Adam is supported")
-        clip = self.grad_clip if self.grad_clip else 0.0
-        self.opt = FlatAdam([self.pf, self.qf], lrs=[plr, qlr], eps=1e-8, max_norms=[clip] * 2, device=self.device, dist=self.dist)
-        self.pf_optimizer = SegmentOptimizer(self.opt, 0)
-        self.qf_optimizer = SegmentOptimizer(self.opt, 1)
-        self._target_flat = FlatParams([self.target_pf, self.target_qf], device=self.device)
-
-    def _target_source(self):
-        return self.opt.data
+        self._init_optimizer(optimizer_class, [("pf", pf, plr), ("qf", qf, qlr)], eps=1e-8,
+                             max_norms=[self.grad_clip or 0.0] * 2)
+        self._init_targets()
 
     # info: 0 Reward_Mean | 4 qf_loss | 6 policy_loss | 10..13 new_actions stats
     def _update_body(self, variant):
@@ -60,17 +50,15 @@ class DDPG(OffRLAlgo):
         q_pred = self.qf([obs, acts])
         g, _, _ = ops.twin_mse_loss(q_pred.reshape(-1), None, y, sc, info=info[4:6])
         torch.autograd.backward([q_pred], [g.reshape(q_pred.shape)], inputs=self.opt.segments[1])
-        self._step(active_mask=0b11)
+        self._optimizer_step(0b11)
         self._update_target_networks()
         ops.vec_stats(new_actions.detach().reshape(-1), out=info[10:14])
-        if self._explicit_batch is None:
-            self._finish_update()
+        self._finish_update()
 
     def _decode_info(self, row, variant):
         info = {'Reward_Mean': float(row[0]), 'Training/policy_loss': float(row[6]),
                 'Training/qf_loss': float(row[4])}
-        for i, s in enumerate(_STAT):
-            info['new_actions/' + s] = float(row[10 + i])
+        info.update(four_stats('new_actions', row[10:14]))
         return info
 
     @property

@@ -12,8 +12,6 @@ import torch
 import torch.optim as optim
 
 from ... import ops
-from ...flat import FlatAdam, FlatParams
-from ..rl_algo import SegmentOptimizer
 from .off_rl_algo import OffRLAlgo
 
 
@@ -28,17 +26,10 @@ class DQN(OffRLAlgo):
         self.target_qf = copy.deepcopy(qf)
         self.qlr = qlr
         self.to(self.device)
-        if optimizer_class is not optim.Adam:
-            raise NotImplementedError("torchrl_b200 fuses Adam in CUDA; only optim.Adam is supported "
-                                      "(the reference's dqn_pong config uses RMSprop: out of this round's scope)")
-        eps = optimizer_info.get("eps", 1e-8)
-        self.opt = FlatAdam([self.qf], lrs=[qlr], eps=eps, max_norms=[0.0], device=self.device, dist=self.dist)
-        self.qf_optimizer = SegmentOptimizer(self.opt, 0)
-        self._target_flat = FlatParams([self.target_qf], device=self.device)
+        # no clipping, whatever grad_clip says: the reference's DQN never clips
+        self._init_optimizer(optimizer_class, [("qf", qf, qlr)], eps=optimizer_info.get("eps", 1e-8), max_norms=[0.0])
+        self._init_targets()
         self.obs_scale = getattr(self.env, "obs_scale", None)
-
-    def _target_source(self):
-        return self.opt.data
 
     def _prep_obs(self, x):
         """uint8 frames -> float32 * obs_scale (ScaledFloatFrame) in one launch; float inputs pass through."""
@@ -71,10 +62,9 @@ class DQN(OffRLAlgo):
                                   weights=None if weights is None else weights.reshape(-1).contiguous(),
                                   td_out=self._td)
         torch.autograd.backward([pred], [grad])
-        self._step()
+        self._optimizer_step()
         self._update_target_networks()
-        if self._explicit_batch is None:
-            self._finish_update()
+        self._finish_update()
 
     def _decode_info(self, row, variant):
         return {'Reward_Mean': float(row[2]), 'Training/qf_loss': float(row[0]),

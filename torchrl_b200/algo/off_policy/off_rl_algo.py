@@ -61,6 +61,9 @@ class OffRLAlgo(RLAlgo):
         return self.replay_buffer.gather_rows(ub["idx"], self.sample_key, pos_ptr=ub["upd"], rows=ub["b"])
 
     def _finish_update(self):
+        """Log row of a gathered update, then upd += 1 (an explicit batch's info row is read directly)."""
+        if self._explicit_batch is not None:
+            return
         ub = self._ub
         ops.ring_write_advance(ub["log_plan"], ub["upd"], ub["U"], ub["log_ticket"])     # log row, then upd += 1
 
@@ -72,14 +75,6 @@ class OffRLAlgo(RLAlgo):
     @property
     def _dp(self):
         return self.dist is not None and self.dist.active
-
-    def _step(self, active_mask=None):
-        """Optimizer step of the flat buffer.  Data parallel (ring sharded by env, every rank draws the same row
-        indices from the same host seed): the flat gradient is summed over ranks first and scaled by 1/G inside
-        the Adam kernel, before clipping -- what a single process over all envs would apply.  NOT yet exercised on
-        more than one GPU (the single-process path is unchanged)."""
-        scale, fused_norm = self.dist.reduce_grads(self.opt, active_mask) if self._dp else (1.0, False)
-        self.opt.step(active_mask=active_mask, grad_scale=scale, reduced=fused_norm)
 
     def _all_ranks(self, vec):
         """Concatenation of a per-rank (B,) vector over ranks (rank order), identical on every rank."""
@@ -121,24 +116,14 @@ class OffRLAlgo(RLAlgo):
         infos = []
         for _ in range(self.opt_times):
             batch = rb.random_batch(self.batch_size, self.sample_key)
-            self.training_update_num += 1
-            variant = self._variant()
-            self._explicit_batch = batch
-            try:
-                self._update_body(variant)
-                self._maybe_hard_update()
-            finally:
-                self._explicit_batch = None
+            variant = self._explicit_update(batch)
             td = getattr(self, "_td", None)
             if td is not None:
                 rb.update_priorities(batch["indices"], td)
             if flush_infos:
                 infos.append(self._decode_info(self._ub["info"][0].cpu().numpy(), variant))
         if flush_infos:
-            self._last_infos = infos
-            if self.logger is not None:
-                for info in infos:
-                    self.logger.add_update_info(info)
+            self._record_infos(infos)
 
     @fused.presplit_scope
     def update_per_epoch(self, flush_infos=True):
@@ -153,13 +138,9 @@ class OffRLAlgo(RLAlgo):
         ub["idx"].copy_(ub["idx_host"], non_blocking=True)
         ub["upd"].zero_()
         variants = [self._run_update() for _ in range(ub["U"])]
-        if not flush_infos:
-            return
-        log = ub["log32"][:len(variants)].cpu().numpy()
-        self._last_infos = [self._decode_info(log[u], variants[u]) for u in range(len(variants))]
-        if self.logger is not None:
-            for info in self._last_infos:
-                self.logger.add_update_info(info)
+        if flush_infos:
+            log = ub["log32"][:len(variants)].cpu().numpy()
+            self._record_infos([self._decode_info(log[u], variants[u]) for u in range(len(variants))])
 
     @fused.presplit_scope
     def update(self, batch):
@@ -172,18 +153,23 @@ class OffRLAlgo(RLAlgo):
             v = torch.as_tensor(np.asarray(v)) if not torch.is_tensor(v) else v
             dt = torch.uint8 if k in ("terminals", "masks") else torch.float32   # masks: Bootstrapped DQN
             conv[k] = v.to(device=dev, dtype=dt).contiguous()
+        variant = self._explicit_update(conv)
+        ub["upd"].zero_()
+        return self._decode_info(ub["info"][0].cpu().numpy(), variant)
+
+    _explicit_batch = None
+
+    def _explicit_update(self, batch):
+        """One eager update on a batch dict of device tensors instead of the gathered rows; returns its variant."""
         self.training_update_num += 1
         variant = self._variant()
-        self._explicit_batch = conv
+        self._explicit_batch = batch
         try:
             self._update_body(variant)
             self._maybe_hard_update()
         finally:
             self._explicit_batch = None
-        ub["upd"].zero_()
-        return self._decode_info(ub["info"][0].cpu().numpy(), variant)
-
-    _explicit_batch = None
+        return variant
 
     def _batch(self):
         return self._explicit_batch if self._explicit_batch is not None else self._gather()

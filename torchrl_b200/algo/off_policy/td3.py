@@ -11,13 +11,10 @@ import torch
 import torch.optim as optim
 
 from ... import ops
-from ...flat import FlatAdam, FlatParams
 from ...policies import distribution as D
 from ...policies.continuous_policy import _DeviceRng
-from ..rl_algo import SegmentOptimizer
+from ..utils import four_stats
 from .off_rl_algo import OffRLAlgo
-
-_STAT = ("mean", "std", "max", "min")
 
 
 class TD3(OffRLAlgo):
@@ -31,22 +28,13 @@ class TD3(OffRLAlgo):
         self.target_qf2 = copy.deepcopy(qf2)
         self.to(self.device)
         self.plr, self.qlr = plr, qlr
-        if optimizer_class is not optim.Adam:
-            raise NotImplementedError("torchrl_b200 fuses clip+Adam in CUDA; only optim.Adam is supported")
-        clip = self.grad_clip if self.grad_clip else 0.0
-        self.opt = FlatAdam([self.pf, self.qf1, self.qf2], lrs=[plr, qlr, qlr], eps=1e-8, max_norms=[clip] * 3,
-                            device=self.device, dist=self.dist)
-        self.pf_optimizer = SegmentOptimizer(self.opt, 0)
-        self.qf1_optimizer = SegmentOptimizer(self.opt, 1)
-        self.qf2_optimizer = SegmentOptimizer(self.opt, 2)
-        self._target_flat = FlatParams([self.target_pf, self.target_qf1, self.target_qf2], device=self.device)
+        self._init_optimizer(optimizer_class, [("pf", pf, plr), ("qf1", qf1, qlr), ("qf2", qf2, qlr)], eps=1e-8,
+                             max_norms=[self.grad_clip or 0.0] * 3)
+        self._init_targets()
         self.policy_update_delay = policy_update_delay
         self.norm_std_policy = norm_std_policy
         self.noise_clip = noise_clip
         self._rng = _DeviceRng()
-
-    def _target_source(self):
-        return self.opt.data
 
     def _variant(self):
         return 1 if (self.training_update_num % self.policy_update_delay) else 0
@@ -79,25 +67,23 @@ class TD3(OffRLAlgo):
         g1, g2, _ = ops.twin_mse_loss(q1_pred.reshape(-1), q2_pred.reshape(-1), y, sc, info=info[4:6])
         torch.autograd.backward([q1_pred, q2_pred], [g1.reshape(q1_pred.shape), g2.reshape(q2_pred.shape)],
                                 inputs=self.opt.segments[1] + self.opt.segments[2])
-        self._step(active_mask=0b110)
+        self._optimizer_step(0b110)
         if variant == 1:
             new_actions = self.pf(obs)
             q_new = self.qf1([obs, new_actions])            # uses qf1 AFTER its step, like the reference
             info[6:7].copy_((-q_new.detach().mean()).reshape(1))
             seed = torch.full_like(q_new, -1.0 / q_new.numel())
             torch.autograd.backward([q_new], [seed], inputs=self.opt.segments[0])
-            self._step(active_mask=0b001)
+            self._optimizer_step(0b001)
             self._update_target_networks()
             ops.vec_stats(new_actions.detach().reshape(-1), out=info[10:14])
-        if self._explicit_batch is None:
-            self._finish_update()
+        self._finish_update()
 
     def _decode_info(self, row, variant):
         info = {'Reward_Mean': float(row[0]), 'Training/qf1_loss': float(row[4]), 'Training/qf2_loss': float(row[5])}
         if variant == 1:
             info['Training/policy_loss'] = float(row[6])
-            for i, s in enumerate(_STAT):
-                info['new_actions/' + s] = float(row[10 + i])
+            info.update(four_stats('new_actions', row[10:14]))
         return info
 
     @property

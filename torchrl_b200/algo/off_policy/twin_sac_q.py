@@ -5,6 +5,8 @@ Q1,Q2(obs,a) -> temperature loss + its Adam step (1 launch) -> [no grad] pf(next
 target Q's, TD-target kernel -> twin MSE kernel -> Q1,Q2(obs, a~) -> policy-loss kernel -> two
 autograd.backward calls seeded with the kernel gradients -> fused clip+Adam over pf|qf1|qf2 ->
 Polyak over the flat target buffer -> log row.
+The temperature, the sample and the policy's regularisers and statistics live in SoftActorCritic, which SAC and
+TwinSAC (sac.py) share.
 """
 import copy
 
@@ -13,33 +15,22 @@ import torch
 import torch.optim as optim
 
 from ... import ops
-from ...flat import FlatAdam, FlatParams
 from ...policies import distribution as D
-from ..rl_algo import SegmentOptimizer
+from ..utils import four_stats
 from .off_rl_algo import OffRLAlgo
 
-_STAT = ("mean", "std", "max", "min")
 
+class SoftActorCritic(OffRLAlgo):
+    """What TwinSAC-Q and SAC / TwinSAC (sac.py) share: the temperature, the policy's sample, the std / mean
+    regularisers and the policy statistics.  Info row slots: 0 Reward_Mean | 1 Alpha 2 Alpha_loss | 4.. critic losses |
+    10..13 log_std stats | 14..17 mean stats | 18 std_reg 19 mean_reg | 20 policy_loss (kernel part), then the loss
+    kernel's log_probs statistics at `_LOG_PROBS`."""
+    _LOG_PROBS = None
 
-class TwinSACQ(OffRLAlgo):
-    def __init__(self, pf, qf1, qf2, plr, qlr, optimizer_class=optim.Adam, policy_std_reg_weight=1e-3,
-                 policy_mean_reg_weight=1e-3, reparameterization=True, automatic_entropy_tuning=True,
-                 target_entropy=None, **kwargs):
+    def __init__(self, pf, policy_std_reg_weight, policy_mean_reg_weight, reparameterization, automatic_entropy_tuning,
+                 target_entropy, **kwargs):
         super().__init__(**kwargs)
-        self.pf, self.qf1, self.qf2 = pf, qf1, qf2
-        self.target_qf1 = copy.deepcopy(qf1)
-        self.target_qf2 = copy.deepcopy(qf2)
-        self.to(self.device)
-        self.plr, self.qlr = plr, qlr
-        if optimizer_class is not optim.Adam:
-            raise NotImplementedError("torchrl_b200 fuses clip+Adam in CUDA; only optim.Adam is supported")
-        clip = self.grad_clip if self.grad_clip else 0.0
-        self.opt = FlatAdam([self.pf, self.qf1, self.qf2], lrs=[plr, qlr, qlr], eps=1e-8, max_norms=[clip] * 3,
-                            device=self.device, dist=self.dist)
-        self.pf_optimizer = SegmentOptimizer(self.opt, 0)
-        self.qf1_optimizer = SegmentOptimizer(self.opt, 1)
-        self.qf2_optimizer = SegmentOptimizer(self.opt, 2)
-        self._target_flat = FlatParams([self.target_qf1, self.target_qf2], device=self.device)
+        self.pf = pf
         self.automatic_entropy_tuning = automatic_entropy_tuning
         if self.automatic_entropy_tuning:
             self.target_entropy = target_entropy if target_entropy else \
@@ -48,18 +39,9 @@ class TwinSACQ(OffRLAlgo):
             self._alpha_state = torch.zeros(3, device=self.device)     # exp_avg, exp_avg_sq, step
         self.policy_std_reg_weight = policy_std_reg_weight
         self.policy_mean_reg_weight = policy_mean_reg_weight
-        if not reparameterization:
-            raise NotImplementedError
-        self.reparameterization = reparameterization
+        self.reparameterization = bool(reparameterization)
         self.tanh_action = bool(getattr(pf, "tanh_action", True))
 
-    def _target_source(self):
-        return self.opt.seg_slice(1, 3)
-
-    # info row layout
-    #  0 Reward_Mean | 1 Alpha 2 Alpha_loss | 3 policy_loss(kernel part) 4 qf1_loss 5 qf2_loss
-    #  6..9 log_probs mean/std/max/min | 10..13 log_std stats | 14..17 mean stats | 18 std_reg 19 mean_reg
-    #  20.. scratch for the 5-float policy info
     def _sample(self, obs, want_grad):
         mean, std, log_std = self.pf(obs)
         mean_c = mean if mean.is_contiguous() else mean.contiguous()
@@ -77,6 +59,70 @@ class TwinSACQ(OffRLAlgo):
             ops.counter_advance(rng.counter)
         return action, logp, mean_c, ls
 
+    def _alpha_step(self, log_probs, sc, info):
+        """Temperature loss + its Adam step (one launch); returns log_alpha, or None without entropy tuning."""
+        if not self.automatic_entropy_tuning:
+            return None
+        lp_all = self._all_ranks(log_probs.detach().reshape(-1))      # temperature sees every rank's samples
+        alpha_sc = sc
+        if lp_all.numel() != sc.B:                  # more samples than the per-rank scratch was sized for
+            alpha_sc = getattr(self, "_alpha_sc", None)
+            if alpha_sc is None or alpha_sc.B != lp_all.numel():
+                alpha_sc = self._alpha_sc = ops.OffPolicyScratch(lp_all.numel(), lp_all.device)
+        ops.sac_alpha_step(lp_all, self.target_entropy, self.log_alpha, self._alpha_state, self.plr, alpha_sc,
+                           info=info[1:3])
+        return self.log_alpha
+
+    def _policy_backward(self, roots, seeds, mean, log_std, info):
+        """log_std/* and mean/* statistics, the std / mean regularisers, then one backward into the policy segment
+        from the loss kernel's seeded roots plus the regularisers."""
+        ops.vec_stats(log_std.detach().reshape(-1) if log_std.is_contiguous() else log_std.detach().contiguous().reshape(-1),
+                      out=info[10:14])
+        ops.vec_stats(mean.detach().reshape(-1), out=info[14:18])
+        if self.policy_std_reg_weight or self.policy_mean_reg_weight:
+            std_reg = self.policy_std_reg_weight * (log_std ** 2).mean()
+            mean_reg = self.policy_mean_reg_weight * (mean ** 2).mean()
+            info[18:19].copy_(std_reg.detach().reshape(1))
+            info[19:20].copy_(mean_reg.detach().reshape(1))
+            roots.append(std_reg + mean_reg)
+            seeds.append(torch.ones((), device=mean.device))
+        torch.autograd.backward(roots, seeds, inputs=self.opt.segments[0])
+
+    def _critic_info(self, row):
+        raise NotImplementedError
+
+    def _decode_info(self, row, variant):
+        info = {'Reward_Mean': float(row[0])}
+        if self.automatic_entropy_tuning:
+            info["Alpha"] = float(row[1])
+            info["Alpha_loss"] = float(row[2])
+        info['Training/policy_loss'] = float(row[20] + row[18] + row[19])
+        info.update(self._critic_info(row))
+        info.update(four_stats('log_std', row[10:14]))
+        info.update(four_stats('log_probs', row[self._LOG_PROBS:self._LOG_PROBS + 4]))
+        info.update(four_stats('mean', row[14:18]))
+        return info
+
+
+class TwinSACQ(SoftActorCritic):
+    _LOG_PROBS = 21              # sac_policy_loss writes [policy_loss, log_probs stats] at 20..24
+
+    def __init__(self, pf, qf1, qf2, plr, qlr, optimizer_class=optim.Adam, policy_std_reg_weight=1e-3,
+                 policy_mean_reg_weight=1e-3, reparameterization=True, automatic_entropy_tuning=True,
+                 target_entropy=None, **kwargs):
+        if not reparameterization:
+            raise NotImplementedError
+        super().__init__(pf, policy_std_reg_weight, policy_mean_reg_weight, reparameterization,
+                         automatic_entropy_tuning, target_entropy, **kwargs)
+        self.qf1, self.qf2 = qf1, qf2
+        self.target_qf1 = copy.deepcopy(qf1)
+        self.target_qf2 = copy.deepcopy(qf2)
+        self.to(self.device)
+        self.plr, self.qlr = plr, qlr
+        self._init_optimizer(optimizer_class, [("pf", pf, plr), ("qf1", qf1, qlr), ("qf2", qf2, qlr)], eps=1e-8,
+                             max_norms=[self.grad_clip or 0.0] * 3)
+        self._init_targets()
+
     def _update_body(self, variant):
         ub = self._ub
         batch = self._batch()
@@ -89,17 +135,7 @@ class TwinSACQ(OffRLAlgo):
         new_actions, log_probs, mean, log_std = self._sample(obs, True)
         q1_pred = self.qf1([obs, acts])
         q2_pred = self.qf2([obs, acts])
-        log_alpha = None
-        if self.automatic_entropy_tuning:
-            lp_all = self._all_ranks(log_probs.detach().reshape(-1))      # temperature sees every rank's samples
-            alpha_sc = sc
-            if lp_all.numel() != sc.B:                  # more samples than the per-rank scratch was sized for
-                alpha_sc = getattr(self, "_alpha_sc", None)
-                if alpha_sc is None or alpha_sc.B != lp_all.numel():
-                    alpha_sc = self._alpha_sc = ops.OffPolicyScratch(lp_all.numel(), lp_all.device)
-            ops.sac_alpha_step(lp_all, self.target_entropy, self.log_alpha, self._alpha_state, self.plr, alpha_sc,
-                               info=info[1:3])
-            log_alpha = self.log_alpha
+        log_alpha = self._alpha_step(log_probs, sc, info)
         with torch.no_grad():
             t_actions, t_logp, _, _ = self._sample(next_obs, False)
             tq1 = self.target_qf1([next_obs, t_actions]).reshape(-1)
@@ -111,42 +147,17 @@ class TwinSACQ(OffRLAlgo):
         qn2 = self.qf2([obs, new_actions])
         g_lp, g_qn1, g_qn2, _ = ops.sac_policy_loss(log_probs.reshape(-1), qn1.reshape(-1), qn2.reshape(-1),
                                                     log_alpha, sc, info=info[20:25], fixed_alpha=1.0)
-        ops.vec_stats(log_std.detach().reshape(-1) if log_std.is_contiguous() else log_std.detach().contiguous().reshape(-1),
-                      out=info[10:14])
-        ops.vec_stats(mean.detach().reshape(-1), out=info[14:18])
-        roots = [log_probs, qn1, qn2]
-        seeds = [g_lp.reshape(log_probs.shape), g_qn1.reshape(qn1.shape), g_qn2.reshape(qn2.shape)]
-        if self.policy_std_reg_weight or self.policy_mean_reg_weight:
-            std_reg = self.policy_std_reg_weight * (log_std ** 2).mean()
-            mean_reg = self.policy_mean_reg_weight * (mean ** 2).mean()
-            info[18:19].copy_(std_reg.detach().reshape(1))
-            info[19:20].copy_(mean_reg.detach().reshape(1))
-            roots.append(std_reg + mean_reg)
-            seeds.append(torch.ones((), device=obs.device))
-        pf_params = self.opt.segments[0]
-        torch.autograd.backward(roots, seeds, inputs=pf_params)
+        self._policy_backward([log_probs, qn1, qn2],
+                              [g_lp.reshape(log_probs.shape), g_qn1.reshape(qn1.shape), g_qn2.reshape(qn2.shape)],
+                              mean, log_std, info)
         torch.autograd.backward([q1_pred, q2_pred], [g1.reshape(q1_pred.shape), g2.reshape(q2_pred.shape)],
                                 inputs=self.opt.segments[1] + self.opt.segments[2])
-        self._step()
+        self._optimizer_step()
         self._update_target_networks()
-        if self._explicit_batch is None:
-            self._finish_update()
+        self._finish_update()
 
-    def _decode_info(self, row, variant):
-        info = {'Reward_Mean': float(row[0])}
-        if self.automatic_entropy_tuning:
-            info["Alpha"] = float(row[1])
-            info["Alpha_loss"] = float(row[2])
-        info['Training/policy_loss'] = float(row[20] + row[18] + row[19])
-        info['Training/qf1_loss'] = float(row[4])
-        info['Training/qf2_loss'] = float(row[5])
-        for i, s in enumerate(_STAT):
-            info['log_std/' + s] = float(row[10 + i])
-        for i, s in enumerate(_STAT):
-            info['log_probs/' + s] = float(row[21 + i])
-        for i, s in enumerate(_STAT):
-            info['mean/' + s] = float(row[14 + i])
-        return info
+    def _critic_info(self, row):
+        return {'Training/qf1_loss': float(row[4]), 'Training/qf2_loss': float(row[5])}
 
     @property
     def networks(self):

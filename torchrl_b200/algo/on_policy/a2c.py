@@ -10,21 +10,17 @@ The advantage statistics of every minibatch of the epoch are computed once up-fr
 syncs with the host inside the loop: the reference's 12 `.item()` calls per update (a2c.py:82-98) become one device
 log fetched per epoch.  The constructor re-homes pf and vf into one flat buffer (flat.FlatAdam).
 """
-import os
-
 import numpy as np
 import torch
 import torch.optim as optim
 
 from ... import ops
-from ...flat import FlatAdam
 from ...networks import fused
-from ..rl_algo import SegmentOptimizer
+from ..utils import four_stats
 from .on_rl_algo import OnRLAlgo
 from .policy_heads import gaussian_outputs, policy_head
 
 _HALF_LOG_2PI = 0.5 * float(np.log(2.0 * np.pi))
-_ADV_KEYS = ['advs/mean', 'advs/std', 'advs/max', 'advs/min']
 
 
 class A2C(OnRLAlgo):
@@ -35,15 +31,11 @@ class A2C(OnRLAlgo):
         self.to(self.device)
         self.plr = plr
         self.vlr = vlr
-        if optimizer_class is not optim.Adam:
-            raise NotImplementedError("torchrl_b200 fuses clip+Adam in CUDA; only optim.Adam is supported")
         self.optimizer_class = optimizer_class
-        # segment 0 = policy, segment 1 = value net (+ whatever a subclass optimises besides, e.g. V-MPO's duals)
+        # segment 0 = policy, segment 1 = value net, then whatever a subclass optimises besides (unclipped)
         extra = self._extra_opt_segments()
-        self.opt = FlatAdam([self.pf, self.vf] + [e[0] for e in extra], lrs=[plr, vlr] + [e[1] for e in extra], eps=1e-5,
-                            max_norms=[0.5, 0.5] + [e[2] for e in extra], device=self.device, dist=self.dist)
-        self.pf_optimizer = SegmentOptimizer(self.opt, 0)
-        self.vf_optimizer = SegmentOptimizer(self.opt, 1)
+        self._init_optimizer(optimizer_class, [("pf", self.pf, plr), ("vf", self.vf, vlr)] + extra, eps=1e-5,
+                             max_norms=[0.5, 0.5] + [0.0] * len(extra))
         self.entropy_coeff = entropy_coeff
         self.vf_criterion = torch.nn.MSELoss()
         self.sample_key = ["obs", "acts", "advs", "estimate_returns"]
@@ -53,12 +45,11 @@ class A2C(OnRLAlgo):
         self._mb_eager_runs = 0
         self._mb_state = None
         self._last_infos = []
-        self.overlap_nets = os.environ.get("TORCHRL_B200_OVERLAP_NETS", "1") == "1"
         self._side_stream = torch.cuda.Stream(device=self.device)
 
     # ------------------------------------------------------------------ what subclasses specialise
     def _extra_opt_segments(self):
-        """[(parameter list, lr, max grad norm or 0)] optimised by the same fused step besides pf and vf."""
+        """[(name or None, parameter list, lr)] optimised without clipping by the same fused step besides pf and vf."""
         return []
 
     def _step_mask(self):
@@ -90,9 +81,8 @@ class A2C(OnRLAlgo):
         """Host-side work of an epoch before the minibatch loop (schedules, target copies)."""
 
     def _decode_info(self, row, norms, gs):
-        info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16]),
-                'v_pred/mean': float(row[24]), 'v_pred/std': float(row[25]), 'v_pred/max': float(row[26]),
-                'v_pred/min': float(row[27])}
+        info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16])}
+        info.update(four_stats('v_pred', row[24:28]))
         info.update(self._head.a2c_std_info(row, self._mb_state["B"], self.replay_buffer._acts.shape[-1]))
         info['ent'] = float(row[11])
         info['log_prob'] = float(row[1])
@@ -151,25 +141,18 @@ class A2C(OnRLAlgo):
             batch = rb.gather_rows(st["perm"], st["keys"], pos_ptr=st["upd"], rows=st["b"])
             batch["obs"] = self._prep_obs(batch["obs"])
             info = st["info"][0]
-            if self.overlap_nets:
-                # the critic and the actor branch share nothing but their (read-only) inputs: run them on two streams
-                # -- under capture this becomes two parallel branches of the graph -- so that their many
-                # latency-bound launches overlap instead of queueing behind one another
-                main = torch.cuda.current_stream(self.device)
-                side = self._side_stream
-                side.wait_stream(main)
-                with torch.cuda.stream(side):
-                    self._critic_step(batch, info)
-                self._actor_step(batch, info)
-                main.wait_stream(side)
-            else:
+            # the critic and the actor branch share nothing but their (read-only) inputs: run them on two streams --
+            # under capture this becomes two parallel branches of the graph -- so that their many latency-bound
+            # launches overlap instead of queueing behind one another
+            main = torch.cuda.current_stream(self.device)
+            side = self._side_stream
+            side.wait_stream(main)
+            with torch.cuda.stream(side):
                 self._critic_step(batch, info)
-                self._actor_step(batch, info)
+            self._actor_step(batch, info)
+            main.wait_stream(side)
             fused.flush_reduces()              # the slab sums of both networks' skinny gradients, one launch
-            scale, fused_norm = 1.0, False
-            if self.dist is not None:
-                scale, fused_norm = self.dist.reduce_grads(self.opt, self._step_mask())   # exchange + norms, one kernel
-            self.opt.step(active_mask=self._step_mask(), grad_scale=scale, reduced=fused_norm)
+            self._optimizer_step(self._step_mask())
             ops.ring_write_advance(st["log_plan"], st["upd"], st["U"], st["log_ticket"])   # log row, then upd += 1
 
     def _run_minibatch(self):
@@ -231,6 +214,10 @@ class A2C(OnRLAlgo):
             return super().update_per_epoch()
         self.process_epoch_samples()
         self._pre_update()
+        self._minibatch_epoch(flush_infos)
+
+    def _minibatch_epoch(self, flush_infos):
+        """`passes` sweeps of row-order minibatches over the stored rollout, one captured minibatch graph each."""
         st = self._mb_state or self._mb_setup()
         st["upd"].zero_()
         T = self.replay_buffer._max_replay_buffer_size
@@ -244,21 +231,12 @@ class A2C(OnRLAlgo):
         n = st["U"]
         for _ in range(n):
             self._run_minibatch()
-        if not flush_infos:
-            return
-        self._last_infos = self._flush_infos(n)
-        if self.logger is not None:
-            for info in self._last_infos:
-                self.logger.add_update_info(info)
+        if flush_infos:
+            self._record_infos(self._flush_infos(n))
 
     def _minibatch(self, batch, keys):
         return [torch.as_tensor(np.asarray(batch[k]) if not torch.is_tensor(batch[k]) else batch[k],
                                 dtype=torch.float32, device=self.device).contiguous() for k in keys]
-
-    @staticmethod
-    def _four_stats(prefix, t):
-        return {prefix + '/mean': t.mean().item(), prefix + '/std': t.std().item(),
-                prefix + '/max': t.max().item(), prefix + '/min': t.min().item()}
 
     @fused.presplit_scope
     def update(self, batch):
@@ -276,15 +254,12 @@ class A2C(OnRLAlgo):
         torch.autograd.backward([values], [g_v.reshape(values.shape)])
         std = self._head.eager_actor(self.pf, obs, acts, None, advs.reshape(-1), adv_stats, 0.0, self.entropy_coeff,
                                      scratch, info32[0:16])
-        scale, fused_norm = 1.0, False
-        if self.dist is not None:
-            scale, fused_norm = self.dist.reduce_grads(self.opt)
-        self.opt.step(grad_scale=scale, reduced=fused_norm)
+        self._optimizer_step()
         row = info32.cpu().numpy()
         info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16])}
-        info.update(self._four_stats('v_pred', values.detach()))
-        if std is not None:
-            info.update(self._four_stats('std', std))
+        for prefix, t in (('v_pred', values.detach()), ('std', std)):
+            if t is not None:
+                info.update(four_stats(prefix, (t.mean(), t.std(), t.max(), t.min())))
         info['ent'] = float(row[11])
         info['log_prob'] = float(row[1])
         return info

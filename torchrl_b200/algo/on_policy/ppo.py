@@ -19,10 +19,9 @@ import numpy as np
 import torch
 
 from ... import ops
-from ...flat import FlatParams
 from ...networks import fused
 from .. import utils as atu
-from .a2c import A2C, _ADV_KEYS
+from .a2c import A2C
 
 # info slots 0-6 of the actor loss kernels; slots 7-10 hold the head's extra keys (log_std/* of a Gaussian policy)
 _INFO_KEYS_ACTOR = ['Training/policy_loss', 'logprob/mean', 'logprob/std', 'logprob/max', 'logprob/min',
@@ -37,7 +36,7 @@ class PPO(A2C):
         self.opt_epochs = opt_epochs
         self.clipped_value_loss = clipped_value_loss
         self.sample_key = ["obs", "acts", "advs", "estimate_returns", "values"]
-        self._target_flat = FlatParams([self.target_pf], device=self.device)
+        self._init_targets()
 
     # ------------------------------------------------------------------ specialisation of the minibatch loop
     def _passes(self):
@@ -85,13 +84,11 @@ class PPO(A2C):
         """ppo.py:29-34: linear LR decay, target <- pf; then the epoch's old log-probs."""
         atu.update_linear_schedule(self.pf_optimizer, self.current_epoch, self.num_epochs, self.plr)
         atu.update_linear_schedule(self.vf_optimizer, self.current_epoch, self.num_epochs, self.vlr)
-        self._target_flat.copy_from(self.opt.seg_slice(0))       # copy_model_params_from_to(pf, target_pf)
+        self._hard_update_targets()                              # copy_model_params_from_to(pf, target_pf)
         self._cache_old_logp()
 
     def _decode_info(self, row, norms, gs):
-        info = {}
-        for i, k in enumerate(_ADV_KEYS):
-            info[k] = float(row[20 + i])
+        info = atu.four_stats('advs', row[20:24])
         info['Training/vf_loss'] = float(row[16])
         info['grad_norm/vf'] = float(norms[1])
         for i, k in enumerate(_INFO_KEYS_ACTOR):
@@ -109,15 +106,13 @@ class PPO(A2C):
         Python floats (this entry point syncs; the epoch loop does not use it)."""
         self.training_update_num += 1
         dev = self.device
-        f = lambda k: torch.as_tensor(np.asarray(batch[k]) if not torch.is_tensor(batch[k]) else batch[k],
-                                      dtype=torch.float32, device=dev).contiguous()
-        obs, acts, advs, rets, old_v = f('obs'), f('acts'), f('advs'), f('estimate_returns'), f('values')
+        obs, acts, advs, rets, old_v = self._minibatch(batch, ('obs', 'acts', 'advs', 'estimate_returns', 'values'))
         B = obs.shape[0]
         scratch = self._head.loss_scratch(B, acts.reshape(B, -1), dev)
         info32 = torch.zeros(32, dtype=torch.float32, device=dev)
         adv_stats = ops.vec_stats(advs.reshape(-1), out=info32[20:24])
         if 'old_logp' in batch:
-            old_logp = f('old_logp').reshape(-1)
+            old_logp = self._minibatch(batch, ('old_logp',))[0].reshape(-1)
         else:
             with torch.no_grad():
                 old_logp = self._head.old_log_prob(self.target_pf, obs, acts, None)
@@ -128,10 +123,7 @@ class PPO(A2C):
             torch.autograd.backward([v], [g_v.reshape(v.shape)])
         self._head.eager_actor(self.pf, obs, acts, old_logp, advs.reshape(-1), adv_stats, self.clip_para,
                                self.entropy_coeff, scratch, info32[0:16], fork=True)
-        scale, fused_norm = 1.0, False
-        if self.dist is not None:
-            scale, fused_norm = self.dist.reduce_grads(self.opt)
-        self.opt.step(grad_scale=scale, reduced=fused_norm)
+        scale = self._optimizer_step()
         row = info32.cpu().numpy()
         norms = self.opt.grad_norms().cpu().numpy() * scale
         return self._decode_info(row, norms, scale)
@@ -139,3 +131,7 @@ class PPO(A2C):
     @property
     def networks(self):
         return [self.pf, self.vf, self.target_pf]
+
+    @property
+    def target_networks(self):
+        return [(self.pf, self.target_pf)]

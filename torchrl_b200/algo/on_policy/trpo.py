@@ -29,9 +29,7 @@ import torch
 from ... import ops
 from ...networks import fused
 from .. import utils as atu
-from .a2c import A2C, _ADV_KEYS
-
-_STAT = ("mean", "std", "max", "min")
+from .a2c import A2C
 
 
 class TRPO(A2C):
@@ -188,10 +186,9 @@ class TRPO(A2C):
             self.opt.refresh_split()
         del mean, log_std
         row = info32.cpu().numpy()
-        info = {k: float(row[20 + i]) for i, k in enumerate(_ADV_KEYS)}
+        info = atu.four_stats('advs', row[20:24])
         info['Training/policy_loss'] = float(surrogate.item())
-        for i, k in enumerate(_STAT):
-            info['logprob/' + k] = float(row[24 + i])
+        info.update(atu.four_stats('logprob', row[24:28]))
         return info
 
     def _conjugate_gradient(self, fvp, b):
@@ -243,10 +240,7 @@ class TRPO(A2C):
             v = self.vf(obs)
             g_v, _ = ops.ppo_critic_loss(v.reshape(-1), rets.reshape(-1), None, False, 0.0, scratch, info=info32[16:17])
             torch.autograd.backward([v], [0.5 * g_v.reshape(v.shape)])
-            scale, fused_norm = 1.0, False
-            if self.dist is not None:
-                scale, fused_norm = self.dist.reduce_grads(self.opt, 0b10)
-            self.opt.step(active_mask=0b10, grad_scale=scale, reduced=fused_norm)
+            scale = self._optimizer_step(0b10)
         return {'Training/vf_loss': 0.5 * float(info32[16].item()),
                 'grad_norm/vf': float(self.opt.grad_norms()[1].item()) * scale}
 
@@ -260,22 +254,5 @@ class TRPO(A2C):
         self._last_policy_info = info
         if self.logger is not None:
             self.logger.add_update_info(info)
-        self._value_sweeps(flush_infos)
-
-    @fused.presplit_scope
-    def _value_sweeps(self, flush_infos):
-        st = self._mb_state or self._mb_setup()
-        st["upd"].zero_()
-        T = rb_rows = self.replay_buffer._max_replay_buffer_size
-        for e in range(st["passes"]):
-            order = self.replay_buffer.epoch_order(self.shuffle)
-            st["perm_host"][e * T:(e + 1) * T].copy_(torch.from_numpy(np.ascontiguousarray(order, dtype=np.int64)))
-        st["perm"].copy_(st["perm_host"], non_blocking=True)
-        for _ in range(st["U"]):
-            self._run_minibatch()
-        if not flush_infos:
-            return
-        self._last_infos = self._flush_infos(st["U"])
-        if self.logger is not None:
-            for info in self._last_infos:
-                self.logger.add_update_info(info)
+        with fused.presplit():
+            self._minibatch_epoch(flush_infos)                   # the value sweeps

@@ -17,15 +17,12 @@ every row's loss and the alpha loss); False uses the per-row KL of the Gaussian 
 """
 import copy
 
-import numpy as np
 import torch
 
 from ... import ops
-from ...flat import FlatParams
-from .a2c import A2C, _ADV_KEYS
+from ..utils import four_stats
+from .a2c import A2C
 from .policy_heads import CategoricalHead
-
-_STAT = ("mean", "std", "max", "min")
 
 
 class VMPO(A2C):
@@ -39,7 +36,7 @@ class VMPO(A2C):
         self.dual = torch.nn.Parameter(torch.tensor([1.0, 0.1], dtype=torch.float32, device=dev))   # [eta, alpha]
         super().__init__(pf=pf, **kwargs)
         self.sample_key = ["obs", "acts", "advs", "estimate_returns", "values"]
-        self._target_flat = FlatParams([self.target_pf], device=self.device)
+        self._init_targets()
         self._categorical = isinstance(self._head, CategoricalHead)
 
     @property
@@ -51,7 +48,7 @@ class VMPO(A2C):
         return self.dual[1:2]
 
     def _extra_opt_segments(self):
-        return [([self.dual], self.plr if hasattr(self, "plr") else 3e-4, 0.0)]
+        return [(None, [self.dual], self.plr)]
 
     def _passes(self):
         return self.opt_epochs
@@ -60,7 +57,7 @@ class VMPO(A2C):
         return ["obs", "acts", "advs", "estimate_returns"]
 
     def _pre_update(self):
-        self._target_flat.copy_from(self.opt.seg_slice(0))       # copy_model_params_from_to(pf, target_pf)
+        self._hard_update_targets()                              # copy_model_params_from_to(pf, target_pf)
 
     def _critic_step(self, batch, info):
         v = self.vf(batch["obs"])
@@ -141,16 +138,14 @@ class VMPO(A2C):
         return infos
 
     def _decode_info(self, row, norms, gs):
-        info = {k: float(row[20 + i]) for i, k in enumerate(_ADV_KEYS)}
+        info = four_stats('advs', row[20:24])
         info['Training/vf_loss'] = float(row[16])
         info['grad_norm/vf'] = float(norms[1])
         info['Training/policy_loss'] = float(row[32])
         info['Training/alpha_loss'] = float(row[33])
         info['Training/alpha'] = info['Training/eta'] = float("nan")             # filled by _flush_infos
-        for i, k in enumerate(_STAT):
-            info['logprob/' + k] = float(row[36 + i])
-        for i, k in enumerate(_STAT):
-            info['KL/' + k] = float(row[40 + i])
+        info.update(four_stats('logprob', row[36:40]))
+        info.update(four_stats('KL', row[40:44]))
         info['grad_norm/pf'] = float(norms[0])
         return info
 
@@ -178,10 +173,7 @@ class VMPO(A2C):
             else:
                 advn = (advs.reshape(-1, 1) - stats[0]) / (stats[1] + 1e-5)
                 self._actor_loss(obs, acts, advn, info).backward()
-            scale, fused_norm = 1.0, False
-            if self.dist is not None:
-                scale, fused_norm = self.dist.reduce_grads(self.opt)
-            self.opt.step(grad_scale=scale, reduced=fused_norm)
+            scale = self._optimizer_step()
             with torch.no_grad():
                 self.dual.clamp_(min=1e-8)
             out = self._decode_info(info.cpu().numpy(), self.opt.grad_norms().cpu().numpy() * scale, scale)
@@ -191,3 +183,7 @@ class VMPO(A2C):
     @property
     def networks(self):
         return [self.pf, self.vf, self.target_pf]
+
+    @property
+    def target_networks(self):
+        return [(self.pf, self.target_pf)]

@@ -7,10 +7,11 @@ from collections import deque
 
 import numpy as np
 import torch
+import torch.optim as optim
 
+from ..flat import FlatAdam, FlatParams
 from ..spaces import is_box
 from .. import ops
-from . import utils as atu
 
 
 class _LRGroup(dict):
@@ -214,17 +215,72 @@ class RLAlgo:
     def update(self, batch):
         raise NotImplementedError
 
+    def _record_infos(self, infos):
+        """Keep the epoch's per-update info dicts and hand them to the logger."""
+        self._last_infos = infos
+        if self.logger is not None:
+            for info in infos:
+                self.logger.add_update_info(info)
+
+    # ------------------------------------------------------------------ the fused optimizer
+    def _init_optimizer(self, optimizer_class, segments, eps, max_norms):
+        """self.opt = one FlatAdam over `segments`, [(name or None, module or parameter list, lr)] in flat-buffer order,
+        with one max grad norm per segment (0: no clipping).  A named segment gets the reference's handle
+        `self.<name>_optimizer`.  Returns {name: segment index}."""
+        if optimizer_class is not optim.Adam:
+            raise NotImplementedError("torchrl_b200 fuses clip + Adam in CUDA; only optim.Adam is supported "
+                                      "(DESIGN.md section 6, deviation 10)")
+        self.opt = FlatAdam([params for _, params, _ in segments], lrs=[lr for _, _, lr in segments], eps=eps,
+                            max_norms=max_norms, device=self.device, dist=self.dist)
+        index = {name: i for i, (name, _, _) in enumerate(segments) if name is not None}
+        for name, i in index.items():
+            setattr(self, name + "_optimizer", SegmentOptimizer(self.opt, i))
+        return index
+
+    def _optimizer_step(self, active_mask=None):
+        """Clip + Adam over the segments in `active_mask` (None: all).  Data parallel (every rank draws the same rows
+        from the same host seed): the flat gradient is summed over ranks first and scaled by 1/G inside the Adam
+        kernel, before clipping -- what a single process over all envs would apply.  Returns that scale."""
+        scale, reduced = self.dist.reduce_grads(self.opt, active_mask) if self.dist is not None else (1.0, False)
+        self.opt.step(active_mask=active_mask, grad_scale=scale, reduced=reduced)
+        return scale
+
+    # ------------------------------------------------------------------ target networks
+    def _init_targets(self):
+        """self._target_flat: one flat buffer over the target networks in `target_networks` order.  Polyak averaging
+        and hard copies read the online networks as one slice of the optimizer's buffer, so each online network must
+        be exactly one optimizer segment, and those segments must be contiguous and in the same order."""
+        pairs = self.target_networks
+        segs = []
+        for online, _ in pairs:
+            params = list(online.parameters())
+            matches = [i for i, seg in enumerate(self.opt.segments)
+                       if len(seg) == len(params) and all(p is q for p, q in zip(seg, params))]
+            assert len(matches) == 1, "an online network of target_networks is not one optimizer segment"
+            segs.append(matches[0])
+        assert segs == list(range(segs[0], segs[0] + len(segs))), \
+            "target_networks must follow contiguous optimizer segments in order"
+        self._target_segs = (segs[0], segs[-1] + 1)
+        self._target_flat = FlatParams([target for _, target in pairs], device=self.device)
+        begin = self.opt.seg_begin[segs[0]]
+        assert self._target_flat.seg_begin == [b - begin for b in self.opt.seg_begin[segs[0]:segs[-1] + 2]], \
+            "target and online networks differ in layout"
+
     def _update_target_networks(self):
         """Polyak update of the target nets (rl_algo.py:169-172) on the flat buffers: one launch,
         captured inside the update graph.  The periodic HARD copy (rl_algo.py:173-176) depends on a
         host counter, so it is applied by `_maybe_hard_update` outside of any captured graph."""
         if self.use_soft_update:
-            ops.polyak_update(self._target_flat.data, self._target_source(), self.tau,
+            ops.polyak_update(self._target_flat.data, self.opt.seg_slice(*self._target_segs), self.tau,
                               planes=(self._target_flat.hi, self._target_flat.lo))
 
     def _maybe_hard_update(self):
         if not self.use_soft_update and self.training_update_num % self.target_hard_update_period == 0:
-            self._target_flat.copy_from(self._target_source())
+            self._hard_update_targets()
+
+    def _hard_update_targets(self):
+        """Targets <- online networks (copy_model_params_from_to on the flat buffers)."""
+        self._target_flat.copy_from(self.opt.seg_slice(*self._target_segs))
 
     @property
     def networks(self):

@@ -3,6 +3,12 @@ agents use the fused kernels (trl_qr_dqn_loss, trl_polyak_update) on their flat 
 import torch
 
 
+def four_stats(prefix, values):
+    """{prefix/mean, prefix/std, prefix/max, prefix/min} from four values in that order (an info-row slice written by
+    ops.vec_stats, or four 0-d tensors)."""
+    return {prefix + "/" + s: float(v) for s, v in zip(("mean", "std", "max", "min"), values)}
+
+
 def huber(x, k=1.0):
     """0.5 x^2 inside |x| < k, k (|x| - k/2) outside."""
     magnitude = x.abs()

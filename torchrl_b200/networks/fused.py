@@ -13,7 +13,6 @@ Routing of one Linear layer (default matmul mode "tc3"):
 Numerically every route is fp32 arithmetic (3xTF32: 2e-6 relative at K = 256); the bias gradient is a fixed-order
 two-level sum.
 """
-import os
 import weakref
 
 import torch
@@ -32,8 +31,6 @@ _ENABLED = True
 _MATMUL_MODE = "tc3"
 _TC3_MIN_ROWS = 2048             # below this the SIMT sgemm's latency wins
 _TF32X3_MIN_DIM = 64             # layers narrower than this stay on the plain path
-# "pair": csrc/gemm_pair.cu (pre-split weights, N-major dgrad operand) [default]; "single": csrc/gemm_tf32x3.cu
-_GEMM_IMPL = os.environ.get("TORCHRL_B200_GEMM", "pair")
 
 
 def set_matmul_mode(mode):
@@ -43,12 +40,6 @@ def set_matmul_mode(mode):
     global _MATMUL_MODE
     assert mode in ("fp32", "tf32x3", "tc3")
     _MATMUL_MODE = mode
-
-
-def set_gemm_impl(impl):
-    global _GEMM_IMPL
-    assert impl in ("pair", "single")
-    _GEMM_IMPL = impl
 
 
 # ---- pre-split weight planes ------------------------------------------------------------------------------------
@@ -81,7 +72,7 @@ class presplit:
 
     def __enter__(self):
         global _PRESPLIT_DEPTH
-        if _PRESPLIT_DEPTH == 0 and _MATMUL_MODE == "tc3" and _GEMM_IMPL == "pair":
+        if _PRESPLIT_DEPTH == 0 and _MATMUL_MODE == "tc3":
             for f in list(_FLATS):
                 f.refresh_split()
         _PRESPLIT_DEPTH += 1
@@ -121,7 +112,7 @@ class transposed_planes:
     def __enter__(self):
         global _TRANSPOSED
         self.prev, self.event, self.joined, self.table = _TRANSPOSED, None, set(), {}
-        if _PRESPLIT_DEPTH > 0 and _MATMUL_MODE == "tc3" and _GEMM_IMPL == "pair":
+        if _PRESPLIT_DEPTH > 0 and _MATMUL_MODE == "tc3":
             self.main = torch.cuda.current_stream()
             key = self.main.cuda_stream
             if key not in _T_STREAMS:
@@ -156,20 +147,16 @@ class transposed_planes:
 
 def mm_fwd(x, weight, bias=None, act=0):
     """act(x (M,K) @ weight (256,K)^T + bias) on the tensor cores."""
-    if _GEMM_IMPL == "pair":
-        return ops.gemm3_pair(x, weight, planes=_planes_of(weight), bias=bias, act=act)
-    return ops.gemm_tf32x3_nt(x, weight, bias=bias, act=act)
+    return ops.gemm3_pair(x, weight, planes=_planes_of(weight), bias=bias, act=act)
 
 
 def mm_dgrad(gz, weight):
     """gz (M,256) @ weight (256,256): inside `transposed_planes()` from the weight's transposed pre-split planes
     (K-major, the forward's route), elsewhere the pair kernel reads the weights N-major (no transpose)."""
-    if _GEMM_IMPL == "pair":
-        planes_t = _TRANSPOSED.planes(weight) if _TRANSPOSED is not None else None
-        if planes_t is not None:
-            return ops.gemm3_pair(gz, weight, planes=planes_t)
-        return ops.gemm3_pair(gz, weight, planes=_planes_of(weight), b_nmajor=True)
-    return ops.gemm_tf32x3_nt(gz, ops.transpose_f32(weight))
+    planes_t = _TRANSPOSED.planes(weight) if _TRANSPOSED is not None else None
+    if planes_t is not None:
+        return ops.gemm3_pair(gz, weight, planes=planes_t)
+    return ops.gemm3_pair(gz, weight, planes=_planes_of(weight), b_nmajor=True)
 
 
 def get_matmul_mode():
@@ -194,7 +181,6 @@ _SCRATCH_KINDS = {      # kind -> (fp32 elements, zeroed int32 tickets) for the 
     "dgrad_act": lambda M, H, K: (ops.skinny_dgrad_act_scratch_floats(M, H), 0),
     "bias_act": lambda M, H, K: (max(ops.bias_act_bwd_scratch_floats(M, H), 4), (H + 127) // 128),
     "cluster": lambda M, H, K: (8 * H * 256, H // 8),                      # gemm3_pair_tn_cluster, H output rows
-    "splitk": lambda M, H, K: (64 * H * 256, 0),                           # gemm_tf32x3_tn, 64 slabs
 }
 
 
@@ -224,10 +210,10 @@ def wgrad(gz, x, out=None):
     K = x.shape[1]
     if _tc3_ok(M, K, M) and H % 128 == 0 and M % (32 * 64) == 0:
         # wgmma 3xTF32, operands consumed M/N-major from their row-major storage, deterministic split-K
-        if _GEMM_IMPL == "pair" and H % 256 == 0:
+        if H % 256 == 0:
             # split-K summed inside the launch (8 group partials + arrival tickets instead of 64 slabs)
             return ops.gemm3_pair_tn_cluster(gz, x, *_scratch("cluster", gz.device, H=H), out=out, splits=64)
-        return ops.gemm_tf32x3_tn(gz, x, out=out, splits=64, workspace=_scratch("splitk", gz.device, H=H))
+        return ops.gemm_tf32x3_tn(gz, x, out=out, splits=64)
     if (_MATMUL_MODE != "fp32" and K <= 24 and H % 32 == 0 and H <= 256 and _skinny_ok(gz)
             and (out is None or out.is_contiguous())):
         return skinny_tn(gz, x, out=out)                 # (H,K) = gz^T x, first-layer weight gradient
@@ -288,11 +274,8 @@ class backward_fork:
         self.keep.clear()
 
 
-_FORK_ENABLED = os.environ.get("TORCHRL_B200_BWD_FORK", "1") == "1"
-
-
 def _fork_here():
-    f = _FORK if _FORK_ENABLED else None
+    f = _FORK
     if f is not None and torch.cuda.current_stream().cuda_stream == f.main.cuda_stream:
         return f
     return None
@@ -626,7 +609,7 @@ def _first_layer_bwd(ctx, gz, x0, w1, h1, w2):
     K = x0.shape[1]
     w1p, b1p = ctx.params[0], ctx.params[1]
     dw_out, db_out = _grad_out(w1p), _grad_out(b1p)
-    planes_t = (_TRANSPOSED.planes(w2) if _TRANSPOSED is not None and _GEMM_IMPL == "pair" and H == 256
+    planes_t = (_TRANSPOSED.planes(w2) if _TRANSPOSED is not None and H == 256
                 and tuple(w2.shape) == (256, 256) else None)
     if planes_t is None or M > _DGRAD_FIRST_MAX_ROWS or not _act_wgrad_ok(x0, h1, dw_out):
         return _linear_act_bwd(mm_dgrad(gz, w2), x0, w1, h1, ctx.act1, (w1p, b1p), (False, True, True))[1:]
