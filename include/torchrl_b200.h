@@ -184,6 +184,23 @@ int trl_vmpo_categorical_loss(const float* logits, const float* target_logits, c
                               int64_t k, int num_actions, float eta_eps, float alpha_eps, int per_row_kl,
                               float* g_logits, float* g_dual, float* info12, double* scratch, unsigned* ticket,
                               void* stream);
+/* TRPO's Fisher-vector product in logit space (algo/on_policy/trpo.py:29-86, the KL over probs of trpo.py:53-61):
+ * per row g = scale * (p * t - p <p, t>) with p = softmax(logits) (maximum subtracted) and t (M, A) the tangent of the
+ * logits along the parameter direction, J v.  This is the Hessian of the reference's KL at theta0 applied to J v,
+ * without its O(1e-8) terms (DESIGN §6 deviation 20); the caller back-propagates g through the logits.  M >= 0. */
+int trl_categorical_fisher_vp(const float* logits, const float* tangent, int64_t M, int num_actions, float scale,
+                              float* g_logits, void* stream);
+/* The bias and activation step of TRPO's tangent forward pass (replaces the elementwise part of trpo.py:65-86's
+ * double backward), in place over (M, C, S) -- NCHW conv outputs (S = H * W) or (M, H) linear outputs (S = 1):
+ * t <- (t + bias_tangent[c]) * act'(y), act'(y) = 1 - y*y (act 1, tanh), y > 0 (act 2, ReLU) or 1 (act 0, y may be
+ * NULL), from the cached layer output y; each operation rounded on its own, as torch evaluates it. */
+int trl_tangent_bias_act(float* t, const float* bias_tangent, const float* y, int64_t M, int C, int64_t S, int act,
+                         void* stream);
+/* TRPO's line-search score of one candidate (trpo.py:113-129): out[0] = -mean(exp(logp - logp_old) * advn), logp
+ * as trl_categorical_log_prob; deterministic fp64 sum, one launch.  scratch: ceil(M / 256) doubles; ticket zeroed
+ * once. */
+int trl_categorical_surrogate(const float* logits, const float* actions, const float* logp_old, const float* advn,
+                              int64_t M, int num_actions, float* out, double* scratch, unsigned* ticket, void* stream);
 
 /* ---- K11: flat-buffer grad-norm clip + Adam, Polyak (algo/utils.py:16-25, ppo.py:72-74,117-119). */
 int trl_grad_sumsq_blocks(int nseg);

@@ -61,6 +61,9 @@ SIGNATURES = {
     "trl_vmpo_select": [vp, vp, i32, i32, i64, vp, vp, vp],
     "trl_vmpo_categorical_scratch_doubles": [i64],
     "trl_vmpo_categorical_loss": [vp, vp, vp, vp, vp, vp, vp, i64, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
+    "trl_categorical_fisher_vp": [vp, vp, i64, i32, f32, vp, vp],
+    "trl_tangent_bias_act": [vp, vp, vp, i64, i32, i64, i32, vp],
+    "trl_categorical_surrogate": [vp, vp, vp, vp, i64, i32, vp, vp, vp, vp],
     "trl_grad_sumsq_blocks": [i32],
     "trl_grad_sumsq": [vp, vp, i32, u32, vp, vp, f64, f64, vp, vp, vp],
     "trl_adam_step": [vp, vp, vp, vp, vp, i32, u32, vp, vp, vp, vp, f32, f32, f32, i32, vp, vp, vp],

@@ -1,6 +1,7 @@
-"""What the on-policy algorithms (A2C, PPO) need to know about the policy's action distribution, in one place: how the
-fused minibatch loop and the eager `update` compute the actor loss and its gradient, the old log-probs and which
-distribution-specific scalars are logged.  `policy_head(pf)` picks the helper once, at construction.
+"""What the on-policy algorithms (A2C, PPO, V-MPO, TRPO) need to know about the policy's action distribution, in one
+place: how the fused minibatch loop and the eager `update` compute the actor loss and its gradient, the old log-probs,
+TRPO's surrogate gradient, KL weighting and line-search score, and which distribution-specific scalars are logged.
+`policy_head(pf)` picks the helper once, at construction.
 
   GaussianHead     -- the (tanh-)Gaussian policies of policies/continuous_policy.py (csrc/ppo_loss.cu);
   CategoricalHead  -- CategoricalDisPolicy over logits (csrc/categorical.cu).
@@ -80,6 +81,54 @@ class GaussianHead:
         mean, _, ls = gaussian_outputs(pf, obs)
         return ops.gaussian_log_prob(mean, ls, acts.reshape(mean.shape[0], -1), self.tanh_action, out=out)
 
+    # ---- TRPO (trpo.py:29-230)
+    trpo_unsupported = ("TRPO supports a Gaussian policy with a free log-std vector (GuassianContPolicyBasicBias) or a "
+                        "CategoricalDisPolicy, over MLPBase or CNNBase with Tanh or ReLU activations and no LayerNorm")
+
+    def trpo_ok(self, pf):
+        return hasattr(pf, "logstd")
+
+    def trpo_forward(self, pf, obs):
+        """The outputs whose graph the policy step keeps: (mean, log_std)."""
+        mean, _, ls = gaussian_outputs(pf, obs)
+        return mean, ls
+
+    def trpo_log_prob(self, pf, obs, acts):
+        with torch.no_grad():
+            return self.old_log_prob(pf, obs, acts, None)
+
+    def trpo_actor(self, outs, acts, advw, ent_coef, info):
+        """The surrogate's gradient at ratio = 1: policy-gradient mode of the actor kernel on advn * w, then one
+        backward (graph kept for the Fisher-vector products)."""
+        mean, ls = outs
+        B = mean.shape[0]
+        scratch = ops.LossScratch(B, mean.shape[1], mean.device)
+        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, ls, acts.reshape(B, -1), None, advw, None, 0.0, ent_coef,
+                                             self.tanh_action, scratch, info=info)
+        torch.autograd.backward([mean, ls], [g_mean, g_ls], retain_graph=True)
+
+    def trpo_fisher_backward(self, pf, outs, dmean, v_of, kl_scale):
+        """Back-propagates D J v with D = diag(1/std^2, 2/std^2), the Hessian of the Gaussian KL wrt (mean, std)."""
+        from ...policies.continuous_policy import LOG_SIG_MIN, LOG_SIG_MAX
+        mean = outs[0]
+        ls = pf.logstd
+        with torch.no_grad():
+            std_vec = torch.exp(torch.clamp(ls, LOG_SIG_MIN, LOG_SIG_MAX))
+            inside = ((ls > LOG_SIG_MIN) & (ls < LOG_SIG_MAX)).to(ls.dtype)         # derivative of the clamp
+            dstd = std_vec * inside * v_of(ls)
+            u_mean = (dmean / (std_vec * std_vec)) * (kl_scale / mean.shape[0])
+            u_std = (2.0 * dstd / (std_vec * std_vec)) * kl_scale
+        std_param = torch.exp(torch.clamp(ls, LOG_SIG_MIN, LOG_SIG_MAX))
+        torch.autograd.backward([mean, std_param], [u_mean, u_std], retain_graph=True)
+
+    def trpo_scratch(self, B, device):
+        return None
+
+    def trpo_score(self, pf, obs, acts, logp_old, advn, scratch):
+        """The line search's surrogate -mean(exp(logp - logp_old) * advn) (trpo.py:113-129), a device scalar."""
+        logp = self.trpo_log_prob(pf, obs, acts)
+        return -torch.mean(torch.exp(logp - logp_old) * advn)
+
 
 class CategoricalHead:
     # the reference's PPO.update_actor reads out['log_std'] (ppo.py:52), which CategoricalDisPolicy.update does not
@@ -145,6 +194,42 @@ class CategoricalHead:
                 torch.autograd.backward([logits], [g])
         else:
             torch.autograd.backward([logits], [g])
+
+    # ---- TRPO (trpo.py:29-230 with the KL over probs, trpo.py:53-61)
+    trpo_unsupported = GaussianHead.trpo_unsupported
+
+    def trpo_ok(self, pf):
+        return True
+
+    def trpo_forward(self, pf, obs):
+        return (self._logits(pf, obs),)
+
+    def trpo_log_prob(self, pf, obs, acts):
+        with torch.no_grad():
+            return self.old_log_prob(pf, obs, acts, None)
+
+    def trpo_actor(self, outs, acts, advw, ent_coef, info):
+        logits, = outs
+        B = logits.shape[0]
+        scratch = ops.LossScratch(B, 1, logits.device, categorical=True)
+        g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1).contiguous(), None, advw, None, 0.0, ent_coef,
+                                              scratch, info=info)
+        torch.autograd.backward([logits], [g], retain_graph=True)
+
+    def trpo_fisher_backward(self, pf, outs, dlogits, v_of, kl_scale):
+        """Back-propagates (diag p - p p^T) J v / B * kl_scale, the Hessian of the mean categorical KL wrt the
+        logits applied to the logits' tangent: one trl_categorical_fisher_vp launch, then autograd."""
+        logits, = outs
+        g = ops.categorical_fisher_vp(logits.detach(), dlogits, kl_scale / logits.shape[0])
+        torch.autograd.backward([logits], [g], retain_graph=True)
+
+    def trpo_scratch(self, B, device):
+        return ops.SurrogateScratch(B, device)
+
+    def trpo_score(self, pf, obs, acts, logp_old, advn, scratch):
+        with torch.no_grad():
+            return ops.categorical_surrogate(self._logits(pf, obs), acts.reshape(-1).contiguous(), logp_old, advn,
+                                             scratch)[0]
 
 
 def policy_head(pf):

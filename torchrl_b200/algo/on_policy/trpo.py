@@ -8,28 +8,61 @@ How the policy step maps onto this library:
   * surrogate gradient: at ratio = 1 the gradient of -mean(ratio * adv) - c_ent * mean(ent) is the policy gradient,
     i.e. the actor loss kernel in policy-gradient mode + one backward through the fused MLP layers into the flat
     gradient buffer (the flat layout replaces parameters_to_vector);
-  * Fisher-vector products WITHOUT double backward: for a Gaussian policy the Hessian of KL(pi_theta || pi_theta0) at
-    theta0 is J^T D J with J = d(mean, std)/d theta and D = diag(1/std^2, 2/std^2) (what trpo.py:64-84 obtains by
-    differentiating the KL twice).  J v is a tangent forward pass through the MLP on activations cached once per
-    epoch (two GEMMs per layer); J^T u is an ordinary backward pass (retained graph) through the fused layers.  One
-    product = 1 tangent forward + 1 backward instead of a double backward through autograd graphs the custom layers
-    do not provide;
+  * Fisher-vector products WITHOUT double backward: the Hessian of KL(pi_theta || pi_theta0) at theta0 is J^T D J
+    with J the Jacobian of the policy's outputs (what trpo.py:64-84 obtains by differentiating the KL twice).  For a
+    Gaussian policy the outputs are (mean, std) and D = diag(1/std^2, 2/std^2); for a categorical one they are the
+    logits and D = diag(p) - p p^T (trl_categorical_fisher_vp, DESIGN §6 deviation 20).  J v is a tangent forward
+    pass through the net (`layer_plan`: Linear or Conv2d layers of the trunk, then append_fcs) on activations cached
+    once per policy step: per layer x dW^T + t W^T (cuBLAS) or conv(x, dW) + conv(t, W) (cuDNN), then the bias and
+    activation-derivative step in one launch (trl_tangent_bias_act).  J^T u is an ordinary backward pass (retained
+    graph).  One product = 1 tangent forward + 1 backward instead of a double backward through autograd graphs the
+    custom layers do not provide;
   * conjugate gradient with fp64 dot products like trpo.py:88-111, entirely on the device (the early exit on
     rdotr < residual_tol becomes a mask: no host sync per iteration);
-  * line search (trpo.py:131-151): candidate parameters are written into the flat buffer and scored with the
-    log-prob kernel; one host comparison per backtrack (the control flow IS the algorithm).
+  * line search (trpo.py:131-151): candidate parameters are written into the flat buffer and scored (categorical:
+    one trl_categorical_surrogate launch after the forward); one host comparison per backtrack (the control flow IS
+    the algorithm).
+The distribution-specific pieces (surrogate gradient, KL weighting of J v, log-probs, score) live on the policy heads
+(policy_heads.py); this class does not branch on the policy type.  On the pixel path the whole rollout's uint8 frames
+are scaled once per policy step (OnRLAlgo._prep_obs).
 Reference quirk kept (SURVEY.md appendix A style): with a vec env the reference feeds (T, N, .) tensors, so
-`torch.sum(kl, 1)` in mean_kl_divergence sums over the ENV axis and the mean runs over (T, act_dim): its KL -- and
-therefore its Fisher matrix -- is N / act_dim times the per-sample KL.  `reference_quirks=True` (default) reproduces
-that scaling for rollouts with N > 1 so that step sizes match the reference; False uses the per-sample KL.
+`torch.sum(kl, 1)` in mean_kl_divergence sums over the ENV axis and the mean runs over (T, act_dim) -- (T, A) for the
+categorical KL over probs: its KL -- and therefore its Fisher matrix -- is N / act_dim (N / A) times the per-sample
+KL.  `reference_quirks=True` (default) reproduces that scaling for (T, N) batches so that step sizes match the
+reference; False uses the per-sample KL.
 """
 import numpy as np
 import torch
+import torch.nn as nn
+import torch.nn.functional as F
 
 from ... import ops
 from ...networks import fused
+from ...networks.base import CNNBase, MLPBase
 from .. import utils as atu
 from .a2c import A2C
+
+_LAYERS = (nn.Linear, nn.Conv2d)
+
+
+def layer_plan(net):
+    """[(Linear | Conv2d, activation module or None)] of a networks.Net in forward order: the trunk's layers
+    (MLPBase.fcs or CNNBase.convs), then append_fcs.  None if the net holds anything else (a LayerNorm, an
+    activation other than Tanh / ReLU, a layer without bias)."""
+    if getattr(net, "add_ln", False) or not isinstance(getattr(net, "base", None), (MLPBase, CNNBase)):
+        return None
+    mods = list(net.base.convs if isinstance(net.base, CNNBase) else net.base.fcs) + list(net.append_fcs)
+    plan, i = [], 0
+    while i < len(mods):
+        layer = mods[i]
+        if not isinstance(layer, _LAYERS) or layer.bias is None:
+            return None
+        act = mods[i + 1] if i + 1 < len(mods) and not isinstance(mods[i + 1], _LAYERS) else None
+        if act is not None and type(act) not in fused.ACT_CODES:
+            return None
+        plan.append((layer, act))
+        i += 1 if act is None else 2
+    return plan if plan and plan[-1][1] is None else None
 
 
 class TRPO(A2C):
@@ -39,9 +72,10 @@ class TRPO(A2C):
         self.residual_tol, self.v_opt_times = residual_tol, v_opt_times
         self.vf_sample_key = ["obs", "estimate_returns"]
         self.reference_quirks = bool(reference_quirks)
-        if not hasattr(self.pf, "logstd"):
-            raise NotImplementedError("TRPO here needs a Gaussian policy with a free log-std vector "
-                                      "(GuassianContPolicyBasicBias, what examples/trpo_continuous_vec.py builds)")
+        self._plan = layer_plan(self.pf)
+        if self._plan is None or not self._head.trpo_ok(self.pf):
+            raise NotImplementedError(self._head.trpo_unsupported)
+        self._obs_dims = 3 if isinstance(self.pf.base, CNNBase) else 1
 
     # ------------------------------------------------------------------ value-function sweeps (A2C loop, vf only)
     def _passes(self):
@@ -69,20 +103,15 @@ class TRPO(A2C):
         return {'Training/vf_loss': 0.5 * float(row[16]), 'grad_norm/vf': float(norms[1])}
 
     # ------------------------------------------------------------------ policy step
-    def _layers(self):
-        """Linear layers of the policy's mean network in forward order + the hidden activation code."""
-        pairs = self.pf.base._pairs
-        assert pairs is not None and len(self.pf.append_fcs) == 1, "TRPO needs an MLPBase trunk + one linear head"
-        kinds = {type(a) for _, a in pairs}
-        assert len(kinds) == 1 and next(iter(kinds)) in fused.ACT_CODES, "one activation type (Tanh / ReLU)"
-        return [fc for fc, _ in pairs] + [self.pf.append_fcs[0]], fused.ACT_CODES[next(iter(kinds))]
-
     def _forward_cache(self, obs):
-        """Activations of every hidden layer (no grad): what the tangent forward pass needs."""
+        """The output of every layer with an activation (no grad): what the tangent forward pass needs."""
         ys, x = [], obs
         with torch.no_grad():
-            for fc, act in self.pf.base._pairs:
-                x = self.pf.base._pair(x, fc, act)
+            for layer, act in self._plan[:-1]:
+                if isinstance(layer, nn.Linear):
+                    x = MLPBase._pair(x.reshape(x.shape[0], -1), layer, act)
+                else:
+                    x = act(layer(x))
                 ys.append(x)
         return ys
 
@@ -93,76 +122,95 @@ class TRPO(A2C):
         return vec[o:o + p.numel()].view(p.shape)
 
     def _tangent_forward(self, obs, ys, v):
-        """J v: directional derivative of (mean, std) along the parameter direction v (flat, pf-segment layout)."""
-        fcs, code = self._layers()
+        """J v: directional derivative of the net's output along the parameter direction v (flat, pf-segment
+        layout).  Per layer x dW^T + t W^T (conv(x, dW) + conv(t, W)), then (t + db) * act'(y) in one launch."""
         x, t = obs, None
-        for li, fc in enumerate(fcs):
-            dW, db = self._view(v, fc.weight), self._view(v, fc.bias)
-            tz = x @ dW.t() + db
-            if t is not None:
-                tz = tz + t @ fc.weight.t()
-            if li < len(fcs) - 1:
-                y = ys[li]
-                t = tz * (1.0 - y * y) if code == 1 else tz * (y > 0).to(tz.dtype)
-                x = y
+        for li, (layer, act) in enumerate(self._plan):
+            W, dW, db = layer.weight, self._view(v, layer.weight), self._view(v, layer.bias)
+            if isinstance(layer, nn.Conv2d):
+                conv = lambda inp, w: F.conv2d(inp, w, None, layer.stride, layer.padding, layer.dilation,  # noqa: E731
+                                               layer.groups)
+                tz = conv(x, dW)
+                if t is not None:
+                    tz.add_(conv(t, W))
             else:
-                t = tz
-        ls = self.pf.logstd
-        inside = ((ls > -20.0) & (ls < 2.0)).to(ls.dtype)                # derivative of the clamp
-        dstd = torch.exp(torch.clamp(ls, -20.0, 2.0)) * inside * self._view(v, ls)
-        return t, dstd
+                x = x.reshape(x.shape[0], -1)
+                tz = torch.mm(x, dW.t())
+                if t is not None:
+                    tz.addmm_(t.reshape(t.shape[0], -1), W.t())
+            y = ys[li] if act is not None else None
+            t = ops.tangent_bias_act(tz, db, y, fused.ACT_CODES[type(act)] if act is not None else 0)
+            x = y
+        return t
 
-    def _fvp(self, v, obs, ys, mean, std_vec, kl_scale):
+    def _fvp(self, v, obs, ys, outs, kl_scale):
         """(H_KL + damping I) v with H_KL = J^T D J (see module docstring); v and the result in pf-segment layout."""
         with torch.no_grad():
-            dmean, dstd = self._tangent_forward(obs, ys, v)
-            B = mean.shape[0]
-            u_mean = (dmean / (std_vec * std_vec)) * (kl_scale / B)
-            u_std = (2.0 * dstd / (std_vec * std_vec)) * kl_scale
+            dout = self._tangent_forward(obs, ys, v)
         seg = self.opt.grad[self.opt.seg_begin[0]:self.opt.seg_begin[1]]
         seg.zero_()
-        std_param = torch.exp(torch.clamp(self.pf.logstd, -20.0, 2.0))
-        torch.autograd.backward([mean, std_param], [u_mean, u_std], retain_graph=True)
+        self._head.trpo_fisher_backward(self.pf, outs, dout, lambda p: self._view(v, p), kl_scale)
         out = seg.clone() + self.cg_damping * v
         seg.zero_()
         return out
 
-    def _log_probs(self, obs, acts, out=None):
-        with torch.no_grad():
-            mean, log_std = self._policy_outputs(self.pf, obs)
-            return ops.gaussian_log_prob(mean, log_std, acts, self.tanh_action, out=out)
+    def _kl_scale(self, env_axis):
+        """N / act_dim (N / A) for a (T, N) batch under reference_quirks, else 1 (module docstring)."""
+        if not self.reference_quirks or env_axis is None:
+            return 1.0
+        return float(env_axis) / self._plan[-1][0].out_features
+
+    def _policy_batch(self, batch):
+        """(obs (B, ...), acts, advs (B,), env-axis size or None) of an explicit whole batch: flat (B, .) or the
+        (T, N, .) whole-rollout layout; uint8 frames are scaled once (OnRLAlgo._prep_obs), not merely cast."""
+        o = batch['obs']
+        if torch.is_tensor(o) and o.dtype == torch.uint8:
+            obs = self._prep_obs(o.to(self.device))
+        else:
+            obs, = self._minibatch(batch, ('obs',))
+        acts, advs = self._minibatch(batch, ('acts', 'advs'))
+        lead = tuple(obs.shape[:obs.dim() - self._obs_dims])
+        obs = obs.reshape((-1,) + tuple(obs.shape[len(lead):]))
+        return obs, acts.reshape(obs.shape[0], -1), advs.reshape(-1), (lead[1] if len(lead) >= 2 else None)
+
+    @fused.presplit_scope
+    def fisher_vector_product(self, batch, v):
+        """(H_KL + cg_damping I) v on an explicit whole batch at the current policy (trpo.py:65-86, the reference's
+        hessian_vector_product); v and the result are flat vectors in the order of pf.parameters()
+        (parameters_to_vector), not the padded layout of the flat buffer."""
+        obs, acts, advs, env_axis = self._policy_batch(batch)
+        outs = self._head.trpo_forward(self.pf, obs)
+        params = list(self.pf.parameters())
+        seg = torch.zeros(self.opt.seg_begin[1] - self.opt.seg_begin[0], dtype=torch.float32, device=self.device)
+        o = 0
+        for p in params:
+            self._view(seg, p).copy_(v[o:o + p.numel()].view(p.shape))
+            o += p.numel()
+        out = self._fvp(seg, obs, self._forward_cache(obs), outs, self._kl_scale(env_axis))
+        return torch.cat([self._view(out, p).reshape(-1) for p in params])
 
     @fused.presplit_scope
     def update(self, batch):
-        """The natural-gradient policy step on an explicit whole batch (trpo.py:153-230): obs (..., o), acts (..., a),
-        advs (..., 1) as arrays or device tensors.  Returns the reference's info dict."""
+        """The natural-gradient policy step on an explicit whole batch (trpo.py:153-230): obs (..., obs shape),
+        acts (..., a) -- action indices for a categorical policy --, advs (..., 1) as arrays or device tensors.
+        Returns the reference's info dict."""
         self.training_update_num += 1
-        obs_in = batch['obs']
-        lead = tuple(obs_in.shape[:-1])
-        env_axis = lead[1] if len(lead) >= 2 else 1
-        obs, acts, advs = self._minibatch(batch, ('obs', 'acts', 'advs'))
-        obs = obs.reshape(-1, obs.shape[-1])
+        obs, acts, advs, env_axis = self._policy_batch(batch)
         B = obs.shape[0]
-        acts = acts.reshape(B, -1)
-        advs = advs.reshape(-1)
-        a = acts.shape[1]
-        kl_scale = float(env_axis) / a if (self.reference_quirks and len(lead) >= 2) else 1.0
+        kl_scale = self._kl_scale(env_axis)
         info32 = torch.zeros(32, dtype=torch.float32, device=self.device)
         st = ops.vec_stats(advs, out=info32[20:24])
         advn = ((advs - st[0]) / (st[1] + 1e-4)).contiguous()                       # trpo.py:171 (1e-4, not 1e-5)
         # trpo.py:177-180: ratio = p / (p.detach() + 1e-8) with p = exp(log_prob): its value AND its gradient carry
         # the factor w = p / (p + 1e-8) (1 for any action the policy could have taken, 0 for log-probs below ~ -18)
-        logp_old = self._log_probs(obs, acts)
+        logp_old = self._head.trpo_log_prob(self.pf, obs, acts)
         p_old = torch.exp(logp_old)
         advw = (advn * (p_old / (p_old + 1e-8))).contiguous()
         seg0 = slice(self.opt.seg_begin[0], self.opt.seg_begin[1])
         # ---- surrogate gradient (ratio = 1): policy-gradient mode of the actor kernel + one backward --------------
         self.opt.grad[seg0].zero_()
-        scratch = ops.LossScratch(B, a, self.device)
-        mean, log_std = self._policy_outputs(self.pf, obs)
-        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, log_std, acts, None, advw, None, 0.0, self.entropy_coeff,
-                                             self.tanh_action, scratch, info=info32[0:16])
-        torch.autograd.backward([mean, log_std], [g_mean, g_ls], retain_graph=True)
+        outs = self._head.trpo_forward(self.pf, obs)
+        self._head.trpo_actor(outs, acts, advw, self.entropy_coeff, info32[0:16])
         g = self.opt.grad[seg0].clone()
         self.opt.grad[seg0].zero_()
         ops.vec_stats(logp_old, out=info32[24:28])
@@ -170,21 +218,22 @@ class TRPO(A2C):
         surrogate = -(advw.mean()) - self.entropy_coeff * ent_mean
         if bool((g != 0).any()):
             ys = self._forward_cache(obs)
-            std_vec = torch.exp(torch.clamp(self.pf.logstd.detach(), -20.0, 2.0))
-            fvp = lambda v: self._fvp(v, obs, ys, mean, std_vec, kl_scale)
+            fvp = lambda v: self._fvp(v, obs, ys, outs, kl_scale)                  # noqa: E731
             step_dir = self._conjugate_gradient(fvp, -g)
             shs = 0.5 * torch.dot(step_dir, fvp(step_dir))
             lm = torch.sqrt(shs / self.max_kl)
             fullstep = step_dir / lm
             gdotstepdir = -torch.dot(g, step_dir)
             theta0 = self.opt.data[seg0].clone()
-            theta = self._linesearch(theta0, fullstep, gdotstepdir / lm, obs, acts, advn, logp_old)
+            del ys
+            score = self._scorer(obs, acts, advn, logp_old)
+            theta = self._linesearch(theta0, fullstep, gdotstepdir / lm, score)
             if bool(torch.isnan(theta).any()):
                 self.opt.data[seg0].copy_(theta0)                                 # "NaN detected. Skipping update..."
             else:
                 self.opt.data[seg0].copy_(theta)
             self.opt.refresh_split()
-        del mean, log_std
+        del outs
         row = info32.cpu().numpy()
         info = atu.four_stats('advs', row[20:24])
         info['Training/policy_loss'] = float(surrogate.item())
@@ -209,20 +258,25 @@ class TRPO(A2C):
             alive = alive * (rdotr >= self.residual_tol).to(torch.float64)
         return x
 
-    def _surrogate_at(self, theta, obs, acts, advn, logp_old):
+    def _scorer(self, obs, acts, advn, logp_old):
+        """theta -> the surrogate at theta (trpo.py:113-129), a device scalar: theta is written into the flat buffer
+        and the policy head scores the candidate."""
         seg0 = slice(self.opt.seg_begin[0], self.opt.seg_begin[1])
-        self.opt.data[seg0].copy_(theta)
-        self.opt.refresh_split()
-        logp = self._log_probs(obs, acts)
-        return -torch.mean(torch.exp(logp - logp_old) * advn)
+        scratch = self._head.trpo_scratch(obs.shape[0], self.device)
 
-    def _linesearch(self, x, fullstep, expected_improve_rate, obs, acts, advn, logp_old):
+        def score(theta):
+            self.opt.data[seg0].copy_(theta)
+            self.opt.refresh_split()
+            return self._head.trpo_score(self.pf, obs, acts, logp_old, advn, scratch)
+        return score
+
+    def _linesearch(self, x, fullstep, expected_improve_rate, score):
         """trpo.py:131-151: backtracking on the surrogate; returns the accepted parameter vector (or x)."""
-        fval = self._surrogate_at(x, obs, acts, advn, logp_old)
+        fval = score(x)
         for stepfrac in .5 ** np.arange(10):
             stepfrac = float(stepfrac)
             xnew = x + stepfrac * fullstep
-            newfval = self._surrogate_at(xnew, obs, acts, advn, logp_old)
+            newfval = score(xnew)
             actual_improve = fval - newfval
             ratio = actual_improve / (expected_improve_rate * stepfrac)
             if bool((ratio > 0.1) & (actual_improve > 0)):
@@ -250,7 +304,7 @@ class TRPO(A2C):
         atu.update_linear_schedule(self.pf_optimizer, self.current_epoch, self.num_epochs, self.plr)
         atu.update_linear_schedule(self.vf_optimizer, self.current_epoch, self.num_epochs, self.vlr)
         rb = self.replay_buffer
-        info = self.update({"obs": rb._obs, "acts": rb._acts, "advs": rb._advs})
+        info = self.update({"obs": rb._obs, "acts": rb._acts, "advs": rb._advs})     # uint8 frames scaled once
         self._last_policy_info = info
         if self.logger is not None:
             self.logger.add_update_info(info)

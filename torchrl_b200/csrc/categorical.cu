@@ -8,6 +8,8 @@
 //   and of A2C.update                                  /root/reference/torchrl/algo/on_policy/a2c.py:45-112
 //   VMPO.update_actor for this policy (top-half selection, loss, dual gradients)
 //                                                      /root/reference/torchrl/algo/on_policy/v_mpo.py:57-133
+//   TRPO's Fisher-vector product, the bias / activation step of its tangent pass and its line-search score
+//                                                      /root/reference/torchrl/algo/on_policy/trpo.py:29-151
 // The distribution is torch's Categorical(probs=softmax(x)): p = softmax(x) (maximum subtracted, then renormalised as
 // Categorical does), l_j = log(clamp(p_j, eps, 1-eps)) (probs_to_logits, NOT log_softmax), log_prob(a) = l_a,
 // entropy = -sum_j p_j l_j.  Gradients wrt x, with m_j = 1 where the clamp passes (eps <= p_j <= 1-eps):
@@ -507,6 +509,124 @@ __global__ void __launch_bounds__(kCatThreads) vmpo_categorical_loss_kernel(cons
   }
 }
 
+// ------------------------------------------------------------------------------------ TRPO
+// The Fisher-vector product in logit space (trpo.py:29-86 with the KL over probs, trpo.py:53-61): at theta0 the
+// Hessian of sum_a p_a log(p_a / (p_a.detach() + 1e-8)) wrt the logits z is diag(p) - p p^T up to O(1e-8) terms
+// (DESIGN §6 deviation 20), so with t = J v the row's product is g = scale * (p * t - p <p, t>).  One thread per row;
+// p is a max-subtracted softmax of the row's logits.
+__global__ void __launch_bounds__(kCatThreads) categorical_fisher_vp_kernel(const float* __restrict__ logits,
+                                                                            const float* __restrict__ tangent,
+                                                                            long long M, int A, float scale,
+                                                                            float* __restrict__ g) {
+  const long long m = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  const float* x = logits + m * A;
+  const float* t = tangent + m * A;
+  float p[kCatMaxA];
+  float mx = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < kCatMaxA; ++j) {
+    if (j < A) {
+      p[j] = x[j];
+      mx = fmaxf(mx, p[j]);
+    }
+  }
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCatMaxA; ++j) {
+    if (j < A) {
+      p[j] = expf(p[j] - mx);
+      s += p[j];
+    }
+  }
+  const float inv = 1.0f / s;
+  float pt = 0.f;
+#pragma unroll
+  for (int j = 0; j < kCatMaxA; ++j) {
+    if (j < A) {
+      p[j] *= inv;
+      pt += p[j] * t[j];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kCatMaxA; ++j)
+    if (j < A) g[m * A + j] = scale * (p[j] * (t[j] - pt));
+}
+
+// The bias and activation step of the tangent forward pass, in place: t <- (t + db[c]) * act'(y) over (M, C, S)
+// (NCHW conv outputs with S = H * W, or (M, H) linear outputs with S = 1), with act'(y) from the cached output y:
+// 1 - y*y (tanh, act 1), y > 0 (ReLU, act 2), 1 (no activation, act 0: the output layer, y unused).  Every operation
+// is rounded on its own, so the result is bit for bit torch's (t + db) * (1 - y * y) / (t + db) * (y > 0).  VEC
+// elements per thread (float4 loads when the caller checked alignment); the channel of the first element costs one
+// division and one remainder, the others step from it.
+template <int VEC, typename Idx>
+__global__ void __launch_bounds__(256) tangent_bias_act_kernel(float* __restrict__ t, const float* __restrict__ db,
+                                                               const float* __restrict__ y, Idx n, Idx C, Idx S,
+                                                               int act) {
+  const Idx stride = static_cast<Idx>(gridDim.x) * blockDim.x * VEC;
+  for (Idx i = (static_cast<Idx>(blockIdx.x) * blockDim.x + threadIdx.x) * VEC; i < n; i += stride) {
+    float tv[VEC], yv[VEC];
+    if constexpr (VEC == 4) {
+      const float4 a = *reinterpret_cast<const float4*>(t + i);
+      tv[0] = a.x; tv[1] = a.y; tv[2] = a.z; tv[3] = a.w;
+      if (act != 0) {
+        const float4 b = __ldg(reinterpret_cast<const float4*>(y + i));
+        yv[0] = b.x; yv[1] = b.y; yv[2] = b.z; yv[3] = b.w;
+      }
+    } else {
+      tv[0] = t[i];
+      if (act != 0) yv[0] = __ldg(y + i);
+    }
+    const Idx q = i / S;
+    Idx s = i - q * S, c = q % C;
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) {
+      float v = __fadd_rn(tv[k], __ldg(db + c));
+      if (act == 1) v = __fmul_rn(v, __fsub_rn(1.0f, __fmul_rn(yv[k], yv[k])));
+      else if (act == 2) v = __fmul_rn(v, yv[k] > 0.f ? 1.0f : 0.0f);
+      tv[k] = v;
+      if (++s == S) {
+        s = 0;
+        c = c + 1 == C ? 0 : c + 1;
+      }
+    }
+    if constexpr (VEC == 4) {
+      *reinterpret_cast<float4*>(t + i) = make_float4(tv[0], tv[1], tv[2], tv[3]);
+    } else {
+      t[i] = tv[0];
+    }
+  }
+}
+
+// The line search's score of one candidate (trpo.py:113-129): -mean(exp(logp - logp_old) * advn) with logp the
+// clamped log-probability of trl_categorical_log_prob.  Each row's term in fp32 as torch forms it, the sum in fp64:
+// per-CTA block sums, then the last CTA folds them in a fixed order (cat_fold_partials) -- deterministic, one launch.
+__global__ void __launch_bounds__(kCatThreads) categorical_surrogate_kernel(const float* __restrict__ logits,
+                                                                            const float* __restrict__ actions,
+                                                                            const float* __restrict__ logp_old,
+                                                                            const float* __restrict__ advn,
+                                                                            long long M, int A,
+                                                                            float* __restrict__ out,
+                                                                            double* __restrict__ partial,
+                                                                            unsigned* __restrict__ ticket) {
+  __shared__ double sh[32];
+  const long long m = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  double term = 0.0;
+  if (m < M) {
+    float p[kCatMaxA], l[kCatMaxA];
+    unsigned pass;
+    cat_row(logits + m * A, A, p, l, pass);
+    const float logp = cat_pick(l, A, cat_action(actions[m], A));
+    term = static_cast<double>(__fmul_rn(expf(__fsub_rn(logp, logp_old[m])), advn[m]));
+  }
+  term = block_reduce_sum<false>(term, sh);
+  if (threadIdx.x == 0) partial[blockIdx.x] = term;
+  if (!last_cta(ticket, gridDim.x)) return;
+  __shared__ double tot[1];
+  cat_fold_partials<1, 1>(partial, tot);
+  if (threadIdx.x == 0) out[0] = static_cast<float>(-tot[0] / static_cast<double>(M));
+}
+
 }  // namespace trl
 
 TRL_API int trl_categorical_sample(const float* logits, const float* u, uint64_t seed, const uint64_t* rng_counter,
@@ -593,4 +713,57 @@ TRL_API int trl_vmpo_categorical_loss(const float* logits, const float* target_l
   vmpo_categorical_loss_kernel<<<static_cast<unsigned>(ceil_div<long long>(k, kCatThreads)), kCatThreads, 0,
                                  static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("vmpo_categorical_loss_kernel");
+}
+
+TRL_API int trl_categorical_fisher_vp(const float* logits, const float* tangent, int64_t M, int num_actions,
+                                      float scale, float* g_logits, void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(M >= 0 && num_actions >= 1 && num_actions <= kCatMaxA,
+              "trl_categorical_fisher_vp: bad sizes M=%lld A=%d (1 <= A <= %d)", (long long)M, num_actions, kCatMaxA);
+  TRL_REQUIRE(logits && tangent && g_logits, "trl_categorical_fisher_vp: null pointer");
+  if (M == 0) return TRL_OK;
+  categorical_fisher_vp_kernel<<<static_cast<unsigned>(ceil_div<long long>(M, kCatThreads)), kCatThreads, 0,
+                                 static_cast<cudaStream_t>(stream)>>>(logits, tangent, M, num_actions, scale, g_logits);
+  return check_launch("categorical_fisher_vp_kernel");
+}
+
+TRL_API int trl_tangent_bias_act(float* t, const float* bias_tangent, const float* y, int64_t M, int C, int64_t S,
+                                 int act, void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(M >= 0 && C >= 1 && S >= 1 && act >= 0 && act <= 2,
+              "trl_tangent_bias_act: bad sizes M=%lld C=%d S=%lld act=%d (act 0 none, 1 tanh, 2 relu)", (long long)M,
+              C, (long long)S, act);
+  TRL_REQUIRE(t && bias_tangent && (y || act == 0), "trl_tangent_bias_act: null pointer");
+  const long long n = M * C * S;
+  if (n == 0) return TRL_OK;
+  const bool vec = n % 4 == 0 && reinterpret_cast<uintptr_t>(t) % 16 == 0 &&
+                   (act == 0 || reinterpret_cast<uintptr_t>(y) % 16 == 0);
+  const int V = vec ? 4 : 1;
+  const long long blocks = ceil_div<long long>(n, 256LL * V);
+  const unsigned grid = static_cast<unsigned>(blocks < 132LL * 16 ? blocks : 132LL * 16);  // grid-stride beyond
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n < (1LL << 31)) {
+    const unsigned nn = static_cast<unsigned>(n), cc = static_cast<unsigned>(C), ss = static_cast<unsigned>(S);
+    if (vec) tangent_bias_act_kernel<4, unsigned><<<grid, 256, 0, st>>>(t, bias_tangent, y, nn, cc, ss, act);
+    else tangent_bias_act_kernel<1, unsigned><<<grid, 256, 0, st>>>(t, bias_tangent, y, nn, cc, ss, act);
+  } else {
+    const unsigned long long nn = n, cc = C, ss = S;
+    if (vec) tangent_bias_act_kernel<4, unsigned long long><<<grid, 256, 0, st>>>(t, bias_tangent, y, nn, cc, ss, act);
+    else tangent_bias_act_kernel<1, unsigned long long><<<grid, 256, 0, st>>>(t, bias_tangent, y, nn, cc, ss, act);
+  }
+  return check_launch("tangent_bias_act_kernel");
+}
+
+TRL_API int trl_categorical_surrogate(const float* logits, const float* actions, const float* logp_old,
+                                      const float* advn, int64_t M, int num_actions, float* out, double* scratch,
+                                      unsigned* ticket, void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(M >= 1 && num_actions >= 1 && num_actions <= kCatMaxA,
+              "trl_categorical_surrogate: bad sizes M=%lld A=%d (1 <= A <= %d)", (long long)M, num_actions, kCatMaxA);
+  TRL_REQUIRE(logits && actions && logp_old && advn && out && scratch && ticket,
+              "trl_categorical_surrogate: null pointer");
+  categorical_surrogate_kernel<<<static_cast<unsigned>(ceil_div<long long>(M, kCatThreads)), kCatThreads, 0,
+                                 static_cast<cudaStream_t>(stream)>>>(logits, actions, logp_old, advn, M, num_actions,
+                                                                     out, scratch, ticket);
+  return check_launch("categorical_surrogate_kernel");
 }

@@ -424,6 +424,66 @@ def vmpo_categorical_loss(logits, target_logits, actions, advs, adv_stats, dual,
     return g_logits
 
 
+def categorical_fisher_vp(logits, tangent, scale, out=None):
+    """TRPO's Fisher-vector product in logit space (trpo.py:29-86): scale * (p * t - p <p, t>) per row of (M, A)
+    logits and their tangent t = J v, p = softmax(logits).  Back-propagating the result through the logits gives
+    J^T (diag p - p p^T) J v * scale."""
+    A = logits.shape[-1]
+    M = logits.numel() // A
+    if tangent.shape != logits.shape:
+        raise ValueError("categorical_fisher_vp: tangent must have the shape of logits")
+    if out is None:
+        out = torch.empty_like(logits)
+    if out.shape != logits.shape:
+        raise ValueError("categorical_fisher_vp: out must have the shape of logits")
+    _lib.call("trl_categorical_fisher_vp", _chk(logits, F32, "logits"), _chk(tangent, F32, "tangent"), M, A,
+              float(scale), _chk(out, F32, "g_logits"), _stream())
+    return out
+
+
+def tangent_bias_act(t, bias_tangent, y, act):
+    """In place t <- (t + bias_tangent[c]) * act'(y) (act 0 none, 1 tanh, 2 ReLU; act'(y) from the layer's cached
+    output y) on (M, C, H, W) conv outputs or (M, C) linear outputs: the bias and activation step of TRPO's tangent
+    forward pass.  Returns t."""
+    if t.dim() < 2:
+        raise ValueError("tangent_bias_act: t must be (M, C) or (M, C, H, W)")
+    M, C = t.shape[0], t.shape[1]
+    S = t.numel() // max(M * C, 1) if M * C else 1
+    if bias_tangent.numel() != C:
+        raise ValueError("tangent_bias_act: bias_tangent must hold one value per channel (%d)" % C)
+    if act != 0 and (y is None or y.shape != t.shape):
+        raise ValueError("tangent_bias_act: y must have the shape of t")
+    _lib.call("trl_tangent_bias_act", _chk(t, F32, "t"), _chk(bias_tangent, F32, "bias_tangent"),
+              _opt(y if act != 0 else None, F32, "y"), M, C, S, int(act), _stream())
+    return t
+
+
+class SurrogateScratch:
+    """Scratch + ticket of trl_categorical_surrogate for up to M rows (allocated once)."""
+
+    def __init__(self, M, device):
+        self.partial = torch.zeros(max((int(M) + 255) // 256, 1), dtype=F64, device=device)
+        self.ticket = torch.zeros(1, dtype=I32, device=device)
+        self.M = int(M)
+
+
+def categorical_surrogate(logits, actions, logp_old, advn, scratch, out=None):
+    """TRPO's line-search score of one candidate (trpo.py:113-129): -mean(exp(logp - logp_old) * advn) as a (1,)
+    device tensor, logp the clamped log-probability of categorical_log_prob.  Deterministic, one launch."""
+    A = logits.shape[-1]
+    M = logits.numel() // A
+    if actions.numel() != M or logp_old.numel() != M or advn.numel() != M:
+        raise ValueError("categorical_surrogate: (M) actions, logp_old and advn")
+    if scratch.M < M:
+        raise ValueError("categorical_surrogate: scratch sized for %d rows, got %d" % (scratch.M, M))
+    if out is None:
+        out = torch.empty(1, dtype=F32, device=logits.device)
+    _lib.call("trl_categorical_surrogate", _chk(logits, F32, "logits"), _chk(actions, F32, "actions"),
+              _chk(logp_old, F32, "logp_old"), _chk(advn, F32, "advn"), M, A, _chk(out, F32, "out"),
+              _chk(scratch.partial, F64, "scratch"), _chk(scratch.ticket, I32, "ticket"), _stream())
+    return out
+
+
 def row_group_moments(x, idx, groups, b, out=None):
     """out (groups,4) f64 = sum, sum of squares, max, -min over the rows idx[u*b:(u+1)*b] of x (rows, n)."""
     n = x.numel() // x.shape[0]
