@@ -419,6 +419,20 @@ int trl_synth_atari_step(uint8_t* obs, int* latent, const float* actions, int* e
 int trl_synth_atari_reset(uint8_t* obs, int* latent, int* elapsed, unsigned* episode, const unsigned* seeds,
                           const uint8_t* mask, const int* zero_is_mask, int episode_bias, int bump, int64_t N,
                           void* stream);
+/* ---- K1 for CartPole-v0 / CartPole-v1: gym.make(env_id) (torchrl/env/get_env.py:53) with TimeLimitAugment.step
+ * (env/base_wrapper.py:152-156), RewardShift.reward (env/base_wrapper.py:37-41) and VecEnv.step (env/vecenv.py:53-61)
+ * fused in; gym's closed-form dynamics and Euler step in fp64 from the fp32 state (N,4), rounded once (defined in
+ * oracle/cartpole.py).  actions (N) are 0.0 or 1.0 (force -10 / +10); any other value sets *action_error = 1 and
+ * leaves that env's state unchanged.  reward = reward_scale on every step.  partial ((trl_cartpole_num_ctas(N), 8)
+ * doubles) / batch_sums (8) / norm_*: the NormObs batch moments, as in trl_synth_env_step.  Resets go through
+ * trl_synth_env_reset with obs_dim 4 and init_scale 0.05. */
+int trl_cartpole_num_ctas(int64_t N);
+int trl_cartpole_step(float* state, const float* actions, int* elapsed, const int* step_count, float* reward,
+                      uint8_t* done, uint8_t* time_limit, int* action_error, double* partial, double* batch_sums,
+                      double* norm_mean, double* norm_var, double* norm_count, unsigned* ticket, int* any_reset,
+                      const int* t_ptr, int64_t N, float reward_scale, int max_episode_steps, int max_episode_frames,
+                      int merge_stats, void* stream);
+
 /* ScaledFloatFrame (env/atari_wrapper.py:171-180): out = in * scale */
 int trl_u8_to_f32(const uint8_t* in, float* out, int64_t n, float scale, void* stream);
 

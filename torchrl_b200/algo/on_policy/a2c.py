@@ -32,10 +32,12 @@ class A2C(OnRLAlgo):
         self.plr = plr
         self.vlr = vlr
         self.optimizer_class = optimizer_class
-        # segment 0 = policy, segment 1 = value net, then whatever a subclass optimises besides (unclipped)
+        # segment 0 = policy, segment 1 = value net (each clipped to 0.5), then whatever a subclass optimises besides
+        # (unclipped)
+        nets = self._net_segments(plr, vlr)
         extra = self._extra_opt_segments()
-        self._init_optimizer(optimizer_class, [("pf", self.pf, plr), ("vf", self.vf, vlr)] + extra, eps=1e-5,
-                             max_norms=[0.5, 0.5] + [0.0] * len(extra))
+        self._init_optimizer(optimizer_class, nets + extra, eps=self.adam_eps,
+                             max_norms=[0.5] * len(nets) + [0.0] * len(extra))
         self.entropy_coeff = entropy_coeff
         self.vf_criterion = torch.nn.MSELoss()
         self.sample_key = ["obs", "acts", "advs", "estimate_returns"]
@@ -48,6 +50,12 @@ class A2C(OnRLAlgo):
         self._side_stream = torch.cuda.Stream(device=self.device)
 
     # ------------------------------------------------------------------ what subclasses specialise
+    adam_eps = 1e-5
+
+    def _net_segments(self, plr, vlr):
+        """[(name, network, lr)] of the networks the agent trains, each clipped to a gradient norm of 0.5."""
+        return [("pf", self.pf, plr), ("vf", self.vf, vlr)]
+
     def _extra_opt_segments(self):
         """[(name or None, parameter list, lr)] optimised without clipping by the same fused step besides pf and vf."""
         return []

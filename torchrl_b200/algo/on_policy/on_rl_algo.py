@@ -3,6 +3,7 @@ advantages / returns on the device (K6), then hand minibatches of whole time-row
 (API of /root/reference/torchrl/algo/on_policy/on_rl_algo.py:6-48)."""
 import torch
 
+from ...networks.nets import ZeroNet
 from ..rl_algo import RLAlgo
 
 _KEYS = ("obs", "acts", "advs", "estimate_returns")
@@ -23,7 +24,9 @@ class OnRLAlgo(RLAlgo):
 
     def _bootstrap_value(self):
         """V(next_obs[T-1]) * (1 - terminals[T-1]) as a contiguous (N,) device vector (on_rl_algo.py:23-27); no
-        host copy."""
+        host copy.  A ZeroNet value function (REINFORCE) bootstraps with zeros and launches nothing."""
+        if isinstance(self.vf, ZeroNet):
+            return torch.zeros(self.replay_buffer.env_nums, dtype=torch.float32, device=self.device)
         tail = self.replay_buffer.last_sample(['next_obs', 'terminals', 'time_limits'])
         alive = 1.0 - tail['terminals'].reshape(-1).float()
         with torch.no_grad():

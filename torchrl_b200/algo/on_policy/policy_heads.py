@@ -35,7 +35,8 @@ class GaussianHead:
     def loss_scratch(self, B, acts, device):
         return ops.LossScratch(B, acts.shape[-1], device)
 
-    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info):
+    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info,
+                        logp_out=None):
         """Device minibatch path: the mean, the raw log-std parameter with the policy's clamp applied inside the loss
         kernel, which writes the parameter's gradient straight into its slice of the flat gradient buffer (this removes
         the clamp / exp / clamp-backward / accumulate launches on six-element tensors from every minibatch)."""
@@ -45,7 +46,8 @@ class GaussianHead:
             mean = mean.contiguous()
         g_mean, _, _ = ops.ppo_actor_loss(mean, pf.logstd.detach(), acts.reshape(mean.shape[0], -1), old_logp, advs,
                                           adv_table, clip, ent_coef, self.tanh_action, scratch, g_log_std=pf.logstd.grad,
-                                          info=info[0:16], stats_pos=stats_pos, ls_clamp=(LOG_SIG_MIN, LOG_SIG_MAX))
+                                          info=info[0:16], logp_out=logp_out, stats_pos=stats_pos,
+                                          ls_clamp=(LOG_SIG_MIN, LOG_SIG_MAX))
         with fused.backward_fork():
             torch.autograd.backward([mean], [g_mean])
 
@@ -63,13 +65,14 @@ class GaussianHead:
         return {'std/mean': float(m), 'std/std': float(np.sqrt(var)), 'std/max': float(sd.max()),
                 'std/min': float(sd.min())}
 
-    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False):
+    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False,
+                    logp_out=None):
         """One eager actor step (loss kernel + autograd); returns the extra scalars A2C logs (std/*)."""
         mean, std, ls = gaussian_outputs(pf, obs)
         if ls.dim() > 1 and ls.shape != mean.shape:
             ls = ls.expand_as(mean).contiguous()
         g_mean, g_ls, _ = ops.ppo_actor_loss(mean, ls, acts.reshape(mean.shape[0], -1), old_logp, advs, adv_stats,
-                                             clip, ent_coef, self.tanh_action, scratch, info=info)
+                                             clip, ent_coef, self.tanh_action, scratch, info=info, logp_out=logp_out)
         if fork:
             with fused.backward_fork():
                 torch.autograd.backward([mean, ls], [g_mean, g_ls])
@@ -149,10 +152,11 @@ class CategoricalHead:
         z = pf.logits(obs)
         return z if z.is_contiguous() else z.contiguous()
 
-    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info):
+    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info,
+                        logp_out=None):
         logits = self._logits(pf, obs)
         g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1), old_logp, advs, adv_table, clip, ent_coef,
-                                              scratch, info=info[0:16], stats_pos=stats_pos)
+                                              scratch, info=info[0:16], logp_out=logp_out, stats_pos=stats_pos)
         with fused.backward_fork():
             torch.autograd.backward([logits], [g])
 
@@ -162,10 +166,11 @@ class CategoricalHead:
     def a2c_std_info(self, row, B, a):
         return {}                                           # a2c.py:90-94 logs std/* only `if 'std' in out`
 
-    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False):
+    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False,
+                    logp_out=None):
         logits = self._logits(pf, obs)
         g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1).contiguous(), old_logp, advs, adv_stats, clip,
-                                              ent_coef, scratch, info=info)
+                                              ent_coef, scratch, info=info, logp_out=logp_out)
         if fork:
             with fused.backward_fork():
                 torch.autograd.backward([logits], [g])

@@ -14,6 +14,7 @@ import torch
 from .. import ops
 from ..env import synth_spec
 from ..networks import fused
+from ..networks.nets import ZeroNet
 from ..policies import distribution as D
 from ..spaces import is_box
 
@@ -57,6 +58,8 @@ class VecCollector:
         self.max_episode_frames = max_episode_frames
         self.use_cuda_graph = bool(use_cuda_graph)
         self.reference_quirks = bool(reference_quirks)
+        # REINFORCE's value function is a ZeroNet: V = 0 needs no launches, `_values` rows stay zero
+        self._has_vf = self.on_policy and not isinstance(getattr(self, "vf", None), ZeroNet)
 
         N = self.env.env_nums
         o = int(np.prod(self.env.observation_space.shape))
@@ -77,6 +80,7 @@ class VecCollector:
         self._value = torch.zeros(N, dtype=F32, device=dev) if self.on_policy else None
         self._v_next = torch.zeros(N, dtype=F32, device=dev) if self.on_policy else None
         self._eps = None
+        self._eps_dev = None
         self._host_step = 0
         self._host_steps = np.zeros(N, dtype=np.int64)      # host mirror of current_step (host envs only)
         self._graphs = {}
@@ -99,6 +103,11 @@ class VecCollector:
                 rb.allocate(k, shp)
         rb._ensure_device()
         self._T = rb._max_replay_buffer_size
+        # epsilon-greedy Q policies on a device env: the host schedule ticks outside the captured step and hands the
+        # rate over in a device scalar
+        if not self._host_env and not self.continuous and hasattr(self.pf, "tick") and not hasattr(self.pf, "act_only"):
+            self._eps_dev = torch.zeros(1, dtype=F32, device=self.device)
+            self._eps_host = torch.zeros(1, dtype=F32).pin_memory()
 
     # ------------------------------------------------------------------ one step
     def _policy_action(self, ob):
@@ -106,7 +115,8 @@ class VecCollector:
         if hasattr(self.pf, "act_only"):
             self.pf.act_only(ob, eps=self._eps, action_out=self._act, nan_flag=self._nan_flag)
         else:
-            out = self.pf.explore(ob.unsqueeze(0) if not self.on_policy else ob)
+            kw = {} if self._eps_dev is None else {"epsilon": self._eps_dev}
+            out = self.pf.explore(ob.unsqueeze(0) if not self.on_policy else ob, **kw)
             act = out["action"]
             self._act.copy_(act.reshape(self._act.shape).to(F32))
 
@@ -122,14 +132,14 @@ class VecCollector:
                              None if nrm is None else nrm._var, self.current_ob, rb._obs, rb._next_obs, rb._acts,
                              rb._values if self.on_policy else None, rb._rewards, rb._terminals, rb._time_limits,
                              rb._top_dev, self.max_episode_frames, getattr(self, "discount", 0.99),
-                             synth_spec.INIT_SCALE, nrm.clip if nrm is not None else 10.0, self.on_policy,
-                             self.reference_quirks)
+                             getattr(env, "init_scale", synth_spec.INIT_SCALE), nrm.clip if nrm is not None else 10.0,
+                             self.on_policy, self.reference_quirks)
 
     def _step_body(self, bootstrap):
         with torch.no_grad():
             ob = self.current_ob
             side = None
-            if self.on_policy:
+            if self._has_vf:
                 # V(ob) is only needed by the finalize kernel: evaluate it on a second stream (a parallel branch of the
                 # captured step graph) while the policy forward, the sampling and the env step run on this one
                 main = torch.cuda.current_stream(self.device)
@@ -142,7 +152,7 @@ class VecCollector:
             if not getattr(self.env, "obs_norm", False):
                 self.env.obs_out.copy_(self.env.state)
             v_next = None
-            if bootstrap:
+            if bootstrap and self._has_vf:
                 if side is not None:
                     main.wait_stream(side)          # one value net, one set of per-stream scratch: V(ob) first
                     side = None
@@ -163,14 +173,14 @@ class VecCollector:
         with torch.no_grad():
             ob = self.current_ob
             self._policy_action(ob)
-            if self.on_policy:
+            if self._has_vf:
                 self._value.copy_(self.vf(ob).reshape(-1))
             env.launch_step(self._act)
             sc = self._host_steps + 1
             mask = env.host_done | (sc >= self.max_episode_frames)
             reset = bool(mask.any())
             v_next = None
-            if self.on_policy and reset:
+            if self._has_vf and reset:
                 self._v_next.copy_(self.vf(env.obs_out).reshape(-1))
                 v_next = self._v_next
             self._finalize(v_next)
@@ -219,6 +229,10 @@ class VecCollector:
                 self._eps.copy_(D.draw_reference_noise((self._N, self._a), self.device))
             return self._step_host()
         boot = self._need_bootstrap()
+        if self._eps_dev is not None:
+            self.pf.tick()
+            self._eps_host[0] = float(self.pf.epsilon)
+            self._eps_dev.copy_(self._eps_host, non_blocking=True)
         if D.get_noise_mode() == "reference_cpu" and self.continuous and hasattr(self.pf, "act_only"):
             eps = D.draw_reference_noise((self._N, self._a), self.device)
             if self._eps is None:
@@ -258,6 +272,8 @@ class VecCollector:
         n_done = int(self._n_done.item())                   # the epoch's only sync
         if int(self._nan_flag.item()) != 0:
             raise FloatingPointError("NaN detected in sampled actions (reference: 'NaN detected. BOOM')")
+        if hasattr(self.env, "check_actions"):
+            self.env.check_actions()
         self.train_rews = []
         if n_done > 0:
             # finished-episode returns in the reference's order (time-major, env ascending)

@@ -87,12 +87,13 @@ class PixelVecCollector(VecCollector):
             env.to_float(env.obs, self._obs_f)
             side = None
             if self.on_policy:
-                # V(obs) is only needed by the finalize kernel: a parallel branch of the captured step graph
-                main = torch.cuda.current_stream(self.device)
-                side = self._side_stream
-                side.wait_stream(main)
-                with torch.cuda.stream(side):
-                    self._value.copy_(self.vf(self._obs_f).reshape(-1))
+                if self._has_vf:
+                    # V(obs) is only needed by the finalize kernel: a parallel branch of the captured step graph
+                    main = torch.cuda.current_stream(self.device)
+                    side = self._side_stream
+                    side.wait_stream(main)
+                    with torch.cuda.stream(side):
+                        self._value.copy_(self.vf(self._obs_f).reshape(-1))
                 self.pf.act_only(self._obs_f, action_out=self._act, nan_flag=self._nan_flag)
             elif self._boot:
                 self.pf.act(self._obs_f, self.current_step, self._act, rb._masks, rb._top_dev)

@@ -89,6 +89,9 @@ class SynthVecEnv:
     over ranks equals the single-process env set).
     """
 
+    # half-width of the uniform reset distribution (the collector's in-kernel partial reset reads it too)
+    init_scale = spec.INIT_SCALE
+
     def __init__(self, env_id, env_nums, env_param=None, device="cuda", first_env=0, total_envs=None,
                  max_episode_steps=spec.MAX_EPISODE_STEPS):
         env_param = dict(env_param or {})
@@ -177,7 +180,7 @@ class SynthVecEnv:
         ops.synth_env_seed(self.seeds, self.episode, seed, self.total_envs, self.first_env)
 
     def _reset_kernel(self, mask):
-        ops.synth_env_reset(self.state, self.elapsed, self.episode, self.seeds, mask, spec.INIT_SCALE)
+        ops.synth_env_reset(self.state, self.elapsed, self.episode, self.seeds, mask, self.init_scale)
 
     def _observe(self, update):
         """NormObs.observation (/root/reference/torchrl/env/base_wrapper.py:118-121)."""
@@ -239,7 +242,7 @@ class SynthVecEnv:
         return self.obs_out, self.reward.unsqueeze(-1), self.done.bool().unsqueeze(-1), infos
 
     def __deepcopy__(self, memo):
-        new = SynthVecEnv.__new__(SynthVecEnv)
+        new = type(self).__new__(type(self))
         for k, v in self.__dict__.items():
             if k == "_dist":
                 new.__dict__[k] = v                       # the job's communicator is shared, never copied

@@ -1009,6 +1009,30 @@ def synth_env_step(state, actions, A, B, c, lb, ub, elapsed, step_count, reward,
               int(bool(merge_stats)), _stream())
 
 
+def cartpole_num_ctas(N):
+    return int(_lib.load().trl_cartpole_num_ctas(int(N)))
+
+
+def cartpole_step(state, actions, elapsed, step_count, reward, done, time_limit, action_error, partial, batch_sums,
+                  norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale, max_episode_steps,
+                  max_episode_frames, merge_stats):
+    """One CartPole step of all N envs (csrc/cartpole.cu): state (N, 4) in place, actions (N) 0.0 / 1.0 (anything else
+    sets action_error (1) int32).  partial / batch_sums / norm_*: the observation-normaliser moments (all None: not
+    estimated); step_count / t_ptr: the collector's step counters and ring row (None outside a collector)."""
+    N = state.shape[0]
+    if state.dim() != 2 or state.shape[1] != 4:
+        raise ValueError("cartpole_step: state must be (N, 4), got %s" % (tuple(state.shape),))
+    if actions.numel() != N:
+        raise ValueError("cartpole_step: one action per env expected, got %d for %d envs" % (actions.numel(), N))
+    _lib.call("trl_cartpole_step", _chk(state, F32, "state"), _chk(actions, F32, "actions"),
+              _chk(elapsed, I32, "elapsed"), _opt(step_count, I32, "step_count"), _chk(reward, F32, "reward"),
+              _chk(done, U8, "done"), _chk(time_limit, U8, "time_limit"), _chk(action_error, I32, "action_error"),
+              _opt(partial, F64, "partial"), _opt(batch_sums, F64, "batch_sums"), _opt(norm_mean, F64, "norm_mean"),
+              _opt(norm_var, F64, "norm_var"), _opt(norm_count, F64, "norm_count"), _chk(ticket, I32, "ticket"),
+              _chk(any_reset, I32, "any_reset"), _opt(t_ptr, I32, "t_ptr"), N, float(reward_scale),
+              int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream(), kernels=int(N > 0))
+
+
 def synth_atari_reset(obs, latent, elapsed, episode, seeds, mask=None, zero_is_mask=None, episode_bias=0, bump=1):
     """New episodes for every env, the envs of the uint8 `mask`, or those whose int32 `zero_is_mask` entry is 0."""
     _lib.call("trl_synth_atari_reset", _chk(obs, U8, "obs"), _chk(latent, I32, "latent"), _chk(elapsed, I32, "elapsed"),
