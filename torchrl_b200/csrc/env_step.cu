@@ -217,10 +217,18 @@ __global__ void synth_env_seed_kernel(unsigned* seeds, unsigned* episode, long l
 
 }  // namespace trl
 
+namespace trl {
+// dynamic shared memory of synth_env_step_kernel in bytes, in double so that no obs_dim / act_dim overflows it
+static double synth_env_smem(int obs_dim, int act_dim) {
+  const double o = obs_dim, a = act_dim, E = kEnvsPerCta;
+  return sizeof(float) * (o * o + a * o + o + 2 * a + 2 * E * o + E * a);
+}
+}  // namespace trl
+
+// saturates at INT_MAX, far above anything that fits
 TRL_API int trl_synth_env_smem_bytes(int obs_dim, int act_dim) {
-  const int E = trl::kEnvsPerCta;
-  return static_cast<int>(sizeof(float)) *
-         (obs_dim * obs_dim + act_dim * obs_dim + obs_dim + 2 * act_dim + 2 * E * obs_dim + E * act_dim);
+  const double b = trl::synth_env_smem(obs_dim, act_dim);
+  return b > 2147483647.0 ? 2147483647 : static_cast<int>(b);
 }
 
 TRL_API int trl_synth_env_num_ctas(int64_t N) {
@@ -246,15 +254,28 @@ TRL_API int trl_synth_env_step(float* state, const float* actions, const float* 
   EnvParams p{state, actions, A, B, c, lb, ub, elapsed, step_count, reward, done, time_limit, partial, batch_sums,
               norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, obs_dim, act_dim, rho, eta, ctrl_cost,
               term_thr, reward_scale, max_episode_steps, max_episode_frames, merge_stats};
-  const int smem = trl_synth_env_smem_bytes(obs_dim, act_dim);
-  TRL_REQUIRE(smem <= 227 * 1024, "trl_synth_env_step: obs_dim %d needs %d B of shared memory (> 227 KB)", obs_dim,
-              smem);
-  static int s_attr_smem = 0;  // set the opt-in once (outside of any stream capture: first call is eager)
-  if (smem > 48 * 1024 && smem > s_attr_smem) {
-    s_attr_smem = smem;
+  const double smem_bytes = synth_env_smem(obs_dim, act_dim);
+  TRL_REQUIRE(smem_bytes <= 227 * 1024, "trl_synth_env_step: obs_dim %d act_dim %d need %.0f B of shared memory "
+              "(> 227 KB)", obs_dim, act_dim, smem_bytes);
+  const int smem = static_cast<int>(smem_bytes);
+  // Both shared-memory limits, 48 KB without the opt-in and 227 KB with it, cover dynamic plus static shared memory.
+  // The kernel's static size is read once and the opt-in set once per size increase (outside of any stream capture:
+  // the first call is eager).
+  static int s_static_smem = -1, s_attr_smem = 0;
+  if (s_static_smem < 0) {
+    cudaFuncAttributes fa;
+    const cudaError_t e = cudaFuncGetAttributes(&fa, synth_env_step_kernel);
+    if (e != cudaSuccess) { set_error("cudaFuncGetAttributes: %s", cudaGetErrorString(e)); return (int)e; }
+    s_static_smem = static_cast<int>(fa.sharedSizeBytes);
+  }
+  TRL_REQUIRE(smem + s_static_smem <= 227 * 1024,
+              "trl_synth_env_step: obs_dim %d act_dim %d need %d B of shared memory + %d B static (> 227 KB)", obs_dim,
+              act_dim, smem, s_static_smem);
+  if (smem + s_static_smem > 48 * 1024 && smem > s_attr_smem) {
     const cudaError_t e =
         cudaFuncSetAttribute(synth_env_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
+    s_attr_smem = smem;
   }
   synth_env_step_kernel<<<trl_synth_env_num_ctas(N), kEnvThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("synth_env_step_kernel");

@@ -13,7 +13,7 @@
 //                 (the carry x_{t0} flows to the earlier tile through shared memory);
 //   CTA         = 16 warps: warp w scans the 4 timesteps [t0 + 4w, t0 + 4w + 4), lane = 4 consecutive envs
 //                 (LDS.128 rows of 512 B: conflict-free), composition of the 16 chunk maps through shared memory;
-//   grid        = min(#groups, 148) persistent CTAs, group g -> CTA g % grid.
+//   grid        = min(#groups, kNumSM = 132) persistent CTAs, group g -> CTA g % grid.
 // Algorithmic traffic is unchanged: 10 B read + 8 B written per (t, n) element, + 4 B per env for last_value.
 #include "gae_common.cuh"
 #include <cuda.h>
