@@ -9,6 +9,7 @@ Per minibatch (one captured CUDA graph, replayed T/b times per pass):
 The advantage statistics of every minibatch of the epoch are computed once up-front (`_epoch_adv_stats`).  Nothing
 syncs with the host inside the loop: the reference's 12 `.item()` calls per update (a2c.py:82-98) become one device
 log fetched per epoch.  The constructor re-homes pf and vf into one flat buffer (flat.FlatAdam).
+`update(batch)` runs the same minibatch step (`_step`) on an explicit batch, with that batch's own advantage statistics.
 """
 import numpy as np
 import torch
@@ -18,9 +19,7 @@ from ... import ops
 from ...networks import fused
 from ..utils import four_stats
 from .on_rl_algo import OnRLAlgo
-from .policy_heads import gaussian_outputs, policy_head
-
-_HALF_LOG_2PI = 0.5 * float(np.log(2.0 * np.pi))
+from .policy_heads import policy_head
 
 
 class A2C(OnRLAlgo):
@@ -71,41 +70,54 @@ class A2C(OnRLAlgo):
     def _gather_keys(self):
         return ["obs", "acts", "advs", "estimate_returns"]
 
-    def _critic_step(self, batch, info):
+    def _critic_step(self, batch, st, info):
         v = self.vf(batch["obs"])
         g_v, _ = ops.ppo_critic_loss(v.reshape(-1), batch["estimate_returns"].reshape(-1), None, False, 0.0,
-                                     self._mb_state["scratch"], info=info[16:17])
+                                     st["scratch"], info=info[16:17])
         with fused.backward_fork():
             torch.autograd.backward([v], [g_v.reshape(v.shape)])
         ops.vec_stats(v.detach().reshape(-1), out=info[24:28])          # v_pred/* (a2c.py:85-88)
 
-    def _actor_step(self, batch, info):
-        st = self._mb_state
-        self._head.minibatch_actor(self.pf, batch["obs"], batch["acts"], None, batch["advs"].reshape(-1),
-                                   st["adv_table"], st["upd"], 0.0, self.entropy_coeff, st["scratch"], info)
-        self._head.log_std_row(self.pf, info)
+    def _actor_step(self, batch, st, info):
+        std = self._head.actor(self.pf, batch["obs"], batch["acts"], None, batch["advs"].reshape(-1), st["adv_table"],
+                               st["upd"], 0.0, self.entropy_coeff, st["scratch"], info)
+        self._head.std_row(self.pf, std, info)
 
     def _pre_update(self):
         """Host-side work of an epoch before the minibatch loop (schedules, target copies)."""
 
-    def _decode_info(self, row, norms, gs):
+    def _prepare_batch(self, batch, st):
+        """For an explicit batch, what the epoch computes once for all of its minibatches (`_epoch_adv_stats`): the
+        advantage statistics, here of this batch alone (a2c.py:62)."""
+        ops.vec_stats(batch["advs"].reshape(-1), out=st["adv_table"][0])
+
+    def _decode_info(self, row, norms, st):
         info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16])}
         info.update(four_stats('v_pred', row[24:28]))
-        info.update(self._head.a2c_std_info(row, self._mb_state["B"], self.replay_buffer._acts.shape[-1]))
+        info.update(self._head.a2c_std_info(row, st["B"], st["a"]))
         info['ent'] = float(row[11])
         info['log_prob'] = float(row[1])
         return info
 
     # ------------------------------------------------------------------ helpers
-    def _policy_outputs(self, pf, obs):
-        mean, _, log_std = gaussian_outputs(pf, obs)
-        return mean, log_std
-
     def _device_path_ok(self):
         """The fused minibatch loop needs a policy its head supports (a Gaussian policy with a shared log-std vector,
-        or a categorical policy) over a device rollout buffer; anything else takes the eager `update(batch)` route."""
+        or a categorical policy) over a device rollout buffer; anything else runs `update(batch)` on each minibatch."""
         rb = self.replay_buffer
         return self._head.fused_ok(self.pf) and rb is not None and hasattr(rb, "gather_rows") and hasattr(rb, "_rewards")
+
+    def _step_state(self, B, U, a):
+        """What a minibatch step of B samples (a action components) runs against: the loss kernels' scratch, the info
+        row, and the (U, 4) advantage statistics table (mean, std, max, min per row) read at row `upd`."""
+        dev = self.device
+        return {
+            "B": B, "U": U, "a": a,
+            "n": B,                                                 # samples behind one row of the table
+            "upd": torch.zeros(1, dtype=torch.int32, device=dev),
+            "info": torch.zeros(1, 64, dtype=torch.float32, device=dev),
+            "scratch": self._head.loss_scratch(B, a, dev),
+            "adv_table": torch.zeros(U, 4, dtype=torch.float32, device=dev),
+        }
 
     def _mb_setup(self):
         rb = self.replay_buffer
@@ -118,36 +130,38 @@ class A2C(OnRLAlgo):
         passes = self._passes()
         U = passes * n_mb
         dev = self.device
-        st = {
-            "b": b, "n_mb": n_mb, "U": U, "B": b * N, "passes": passes,
+        W = self.dist.world_size if (self.dist is not None and self.dist.active) else 1
+        # one step state for all U minibatches of the epoch: `upd` is the gather position, the statistics row and the
+        # log row of minibatch u
+        st = self._step_state(b * N, U, int(np.prod(rb._acts.shape[2:])))
+        st.update({
+            "b": b, "n_mb": n_mb, "passes": passes, "n": b * N * W,     # the table spans every rank's rows
             # every pass' row order is uploaded up-front: (passes, T) indices, minibatch u of the epoch reads
-            # perm[u*b : (u+1)*b] -- `upd` is the gather position, the statistics row and the log row
+            # perm[u*b : (u+1)*b]
             "perm": torch.zeros(passes * T, dtype=torch.int64, device=dev),
             "perm_host": torch.zeros(passes * T, dtype=torch.int64).pin_memory(),
-            "upd": torch.zeros(1, dtype=torch.int32, device=dev),
-            "info": torch.zeros(1, 64, dtype=torch.float32, device=dev),
             "log_ticket": torch.zeros(1, dtype=torch.int32, device=dev),
             "log32": torch.zeros(U, 64, dtype=torch.float32, device=dev),
             "log64": torch.zeros(U, self.opt.sumsq3.numel(), dtype=torch.float64, device=dev),
-            "scratch": self._head.loss_scratch(b * N, rb._acts, dev),
-            # advantage statistics of all U minibatches, computed once per epoch (mean, std, max, min per row)
-            "adv_table": torch.zeros(U, 4, dtype=torch.float32, device=dev),
             "keys": self._gather_keys(),
-        }
+        })
         st["log_plan"] = ops.RowCopyPlan([st["info"], self.opt.sumsq3.view(1, -1)], [st["log32"], st["log64"]],
                                          [64 * 4, self.opt.sumsq3.numel() * 8])
         self._mb_state = st
         return st
 
-    def _mb_body(self):
-        """One minibatch update reading its row indices at device position `upd`.  Layer gradients go straight into
-        the flat gradient buffer (networks.fused.direct_grad): every parameter gets exactly one contribution per
-        minibatch and the optimizer step left the buffer zeroed.  The dgrad GEMMs read transposed weight planes,
-        rewritten from the previous optimizer step's planes beside the gather and the forward passes."""
+    def _step(self, batch, st):
+        """One minibatch update against the step state `st`; returns the gradient scale of the optimizer step.
+        `batch` None: the epoch's minibatch, whose row indices are read at device position `upd` and whose log row is
+        written before `upd` advances.  Layer gradients go straight into the flat gradient buffer
+        (networks.fused.direct_grad): every parameter gets exactly one contribution per minibatch and the optimizer step
+        left the buffer zeroed.  The dgrad GEMMs read transposed weight planes, rewritten from the previous optimizer
+        step's planes beside the gather and the forward passes."""
         with fused.direct_grad(), fused.deferred_reduces(), fused.transposed_planes(self.opt):
-            st, rb = self._mb_state, self.replay_buffer
-            batch = rb.gather_rows(st["perm"], st["keys"], pos_ptr=st["upd"], rows=st["b"])
-            batch["obs"] = self._prep_obs(batch["obs"])
+            epoch = batch is None
+            if epoch:
+                batch = self.replay_buffer.gather_rows(st["perm"], st["keys"], pos_ptr=st["upd"], rows=st["b"])
+                batch["obs"] = self._prep_obs(batch["obs"])
             info = st["info"][0]
             # the critic and the actor branch share nothing but their (read-only) inputs: run them on two streams --
             # under capture this becomes two parallel branches of the graph -- so that their many latency-bound
@@ -156,12 +170,19 @@ class A2C(OnRLAlgo):
             side = self._side_stream
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                self._critic_step(batch, info)
-            self._actor_step(batch, info)
+                self._critic_step(batch, st, info)
+            self._actor_step(batch, st, info)
             main.wait_stream(side)
             fused.flush_reduces()              # the slab sums of both networks' skinny gradients, one launch
-            self._optimizer_step(self._step_mask())
-            ops.ring_write_advance(st["log_plan"], st["upd"], st["U"], st["log_ticket"])   # log row, then upd += 1
+            scale = self._optimizer_step(self._step_mask())
+            if epoch:
+                # the log row, then upd += 1
+                ops.ring_write_advance(st["log_plan"], st["upd"], st["U"], st["log_ticket"])
+            return scale
+
+    def _mb_body(self):
+        """One minibatch update of the epoch (what the captured graph holds)."""
+        self._step(None, self._mb_state)
 
     def _run_minibatch(self):
         if not self.use_cuda_graph:
@@ -201,7 +222,7 @@ class A2C(OnRLAlgo):
             else:
                 import torch.distributed as tdist
                 tdist.all_gather_into_tensor(st["mom_all"].view(-1), st["mom"].view(-1))
-        ops.group_stats_from_moments(st["mom_all"], W, U, float(b * rb.env_nums * W), out=st["adv_table"])
+        ops.group_stats_from_moments(st["mom_all"], W, U, float(st["n"]), out=st["adv_table"])
 
     def _flush_infos(self, n_updates):
         """One D2H copy of the epoch's per-update scalars -> list of the reference's info dicts."""
@@ -211,7 +232,7 @@ class A2C(OnRLAlgo):
         log64 = st["log64"][:n_updates].cpu().numpy()
         # the flat gradient holds the SUM over ranks; the averaged gradient's norm is what one process sees
         gs = 1.0 / self.dist.world_size if (self.dist is not None and self.dist.active) else 1.0
-        return [self._decode_info(log32[u], np.sqrt(log64[u][:self.opt.nseg]) * gs, gs) for u in range(n_updates)]
+        return [self._decode_info(log32[u], np.sqrt(log64[u][:self.opt.nseg]) * gs, st) for u in range(n_updates)]
 
     # ------------------------------------------------------------------ reference API
     @fused.presplit_scope
@@ -242,35 +263,32 @@ class A2C(OnRLAlgo):
         if flush_infos:
             self._record_infos(self._flush_infos(n))
 
-    def _minibatch(self, batch, keys):
-        return [torch.as_tensor(np.asarray(batch[k]) if not torch.is_tensor(batch[k]) else batch[k],
-                                dtype=torch.float32, device=self.device).contiguous() for k in keys]
+    def _device_batch(self, batch, keys):
+        """The `keys` present in an explicit batch as contiguous device tensors: float32, except uint8 frames, which
+        `_prep_obs` then scales as the epoch's gather does."""
+        out = {}
+        for k in keys:
+            if k in batch:
+                v = batch[k] if torch.is_tensor(batch[k]) else torch.as_tensor(np.asarray(batch[k]))
+                dt = torch.uint8 if (k == "obs" and v.dtype == torch.uint8) else torch.float32
+                out[k] = v.to(device=self.device, dtype=dt).contiguous()
+        out["obs"] = self._prep_obs(out["obs"])
+        return out
 
     @fused.presplit_scope
     def update(self, batch):
-        """One A2C minibatch update on an explicit batch (a2c.py:45-112), eagerly, through the same loss kernels and
-        the fused optimizer step; returns the reference's info dict (this entry point syncs; the epoch loop does not
-        use it)."""
+        """One minibatch update on an explicit batch (a2c.py:45-112; PPO, V-MPO and REINFORCE likewise): the epoch's
+        `_step` against a one-row step state whose advantage statistics are the batch's own.  Syncs to return the
+        reference's info dict."""
         self.training_update_num += 1
-        obs, acts, advs, est_rets = self._minibatch(batch, ('obs', 'acts', 'advs', 'estimate_returns'))
-        B = obs.shape[0]
-        scratch = self._head.loss_scratch(B, acts.reshape(B, -1), self.device)
-        info32 = torch.zeros(32, dtype=torch.float32, device=self.device)
-        adv_stats = ops.vec_stats(advs.reshape(-1), out=info32[20:24])
-        values = self.vf(obs)
-        g_v, _ = ops.ppo_critic_loss(values.reshape(-1), est_rets.reshape(-1), None, False, 0.0, scratch, info=info32[16:17])
-        torch.autograd.backward([values], [g_v.reshape(values.shape)])
-        std = self._head.eager_actor(self.pf, obs, acts, None, advs.reshape(-1), adv_stats, 0.0, self.entropy_coeff,
-                                     scratch, info32[0:16])
-        self._optimizer_step()
-        row = info32.cpu().numpy()
-        info = {'Training/policy_loss': float(row[0]), 'Training/vf_loss': float(row[16])}
-        for prefix, t in (('v_pred', values.detach()), ('std', std)):
-            if t is not None:
-                info.update(four_stats(prefix, (t.mean(), t.std(), t.max(), t.min())))
-        info['ent'] = float(row[11])
-        info['log_prob'] = float(row[1])
-        return info
+        batch = self._device_batch(batch, self._gather_keys())
+        B = batch["obs"].shape[0]
+        st = self._step_state(B, 1, int(np.prod(batch["acts"].shape[1:])) if "acts" in batch else 1)
+        self._prepare_batch(batch, st)
+        scale = self._step(batch, st)
+        row = st["info"][0].cpu().numpy()
+        row[20:24] = st["adv_table"][0].cpu().numpy()                   # where _flush_infos puts the epoch's table
+        return self._decode_info(row, self.opt.grad_norms().cpu().numpy() * scale, st)
 
     @property
     def snapshot_networks(self):

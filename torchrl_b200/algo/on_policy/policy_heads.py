@@ -1,6 +1,6 @@
-"""What the on-policy algorithms (A2C, PPO, V-MPO, TRPO) need to know about the policy's action distribution, in one
-place: how the fused minibatch loop and the eager `update` compute the actor loss and its gradient, the old log-probs,
-TRPO's surrogate gradient, KL weighting and line-search score, and which distribution-specific scalars are logged.
+"""What the on-policy algorithms (A2C, PPO, V-MPO, TRPO, REINFORCE) need to know about the policy's action distribution,
+in one place: how the minibatch step computes the actor loss and its gradient, the old log-probs, TRPO's surrogate
+gradient, KL weighting and line-search score, and which distribution-specific scalars are logged.
 `policy_head(pf)` picks the helper once, at construction.
 
   GaussianHead     -- the (tanh-)Gaussian policies of policies/continuous_policy.py (csrc/ppo_loss.cu);
@@ -11,6 +11,7 @@ import torch
 
 from ... import ops
 from ...networks import fused
+from ..utils import four_stats
 
 
 def gaussian_outputs(pf, obs):
@@ -27,58 +28,61 @@ class GaussianHead:
 
     def __init__(self, pf):
         self.tanh_action = bool(getattr(pf, "tanh_action", False))
+        self.shared_logstd = hasattr(pf, "logstd")
 
     def fused_ok(self, pf):
         """The fused minibatch loop needs a shared log-std PARAMETER (GuassianContPolicyBasicBias)."""
         return hasattr(pf, "logstd")
 
-    def loss_scratch(self, B, acts, device):
-        return ops.LossScratch(B, acts.shape[-1], device)
+    def loss_scratch(self, B, a, device):
+        return ops.LossScratch(B, a, device)
 
-    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info,
-                        logp_out=None):
-        """Device minibatch path: the mean, the raw log-std parameter with the policy's clamp applied inside the loss
-        kernel, which writes the parameter's gradient straight into its slice of the flat gradient buffer (this removes
-        the clamp / exp / clamp-backward / accumulate launches on six-element tensors from every minibatch)."""
+    def actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info, logp_out=None):
+        """The actor loss kernel, then autograd through the policy.  With a shared log-std parameter the kernel takes
+        the mean and the raw parameter, applies the policy's clamp itself and writes the parameter's gradient straight
+        into its slice of the flat gradient buffer (this removes the clamp / exp / clamp-backward / accumulate launches
+        on six-element tensors from every minibatch); otherwise autograd runs through the (mean, log_std) of the
+        policy's forward.  Returns the std that `std_row` logs: None with a shared log-std parameter."""
         from ...policies.continuous_policy import LOG_SIG_MIN, LOG_SIG_MAX
-        mean = pf.mean_net(obs)
-        if not mean.is_contiguous():
-            mean = mean.contiguous()
-        g_mean, _, _ = ops.ppo_actor_loss(mean, pf.logstd.detach(), acts.reshape(mean.shape[0], -1), old_logp, advs,
-                                          adv_table, clip, ent_coef, self.tanh_action, scratch, g_log_std=pf.logstd.grad,
-                                          info=info[0:16], logp_out=logp_out, stats_pos=stats_pos,
-                                          ls_clamp=(LOG_SIG_MIN, LOG_SIG_MAX))
+        if self.shared_logstd:
+            mean = pf.mean_net(obs)
+            if not mean.is_contiguous():
+                mean = mean.contiguous()
+            ls, g_ls, ls_clamp, std = pf.logstd.detach(), pf.logstd.grad, (LOG_SIG_MIN, LOG_SIG_MAX), None
+        else:
+            mean, std, ls = gaussian_outputs(pf, obs)
+            if ls.dim() > 1 and ls.shape != mean.shape:
+                ls = ls.expand_as(mean).contiguous()
+            g_ls, ls_clamp, std = None, None, std.detach().expand_as(mean)
+        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, ls, acts.reshape(mean.shape[0], -1), old_logp, advs, adv_table, clip,
+                                             ent_coef, self.tanh_action, scratch, g_log_std=g_ls, info=info[0:16],
+                                             logp_out=logp_out, stats_pos=stats_pos, ls_clamp=ls_clamp)
         with fused.backward_fork():
-            torch.autograd.backward([mean], [g_mean])
+            if self.shared_logstd:
+                torch.autograd.backward([mean], [g_mean])
+            else:
+                torch.autograd.backward([mean, ls], [g_mean, g_ls])
+        return std
 
-    def log_std_row(self, pf, info):
-        """A2C's std/* (a2c.py:90-94) are derived at flush from the clamped log-std written here."""
+    def std_row(self, pf, std, info):
+        """What A2C's std/* (a2c.py:90-94) are derived from at decode: the clamped shared log-std, or the four
+        statistics of the autograd route's std."""
+        if std is not None:
+            ops.vec_stats(std.contiguous().reshape(-1), out=info[28:32])
+            return
         from ...policies.continuous_policy import LOG_SIG_MIN, LOG_SIG_MAX
         n = pf.logstd.numel()
         torch.clamp(pf.logstd.detach(), LOG_SIG_MIN, LOG_SIG_MAX, out=info[28:28 + n])
 
     def a2c_std_info(self, row, B, a):
+        if not self.shared_logstd:
+            return four_stats('std', row[28:32])
         ls = row[28:28 + a].astype(np.float64)
         sd = np.exp(ls)
         m = sd.mean()
         var = B * ((sd - m) ** 2).sum() / (B * a - 1.0)              # torch.std() of the (B, a) expanded tensor
         return {'std/mean': float(m), 'std/std': float(np.sqrt(var)), 'std/max': float(sd.max()),
                 'std/min': float(sd.min())}
-
-    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False,
-                    logp_out=None):
-        """One eager actor step (loss kernel + autograd); returns the extra scalars A2C logs (std/*)."""
-        mean, std, ls = gaussian_outputs(pf, obs)
-        if ls.dim() > 1 and ls.shape != mean.shape:
-            ls = ls.expand_as(mean).contiguous()
-        g_mean, g_ls, _ = ops.ppo_actor_loss(mean, ls, acts.reshape(mean.shape[0], -1), old_logp, advs, adv_stats,
-                                             clip, ent_coef, self.tanh_action, scratch, info=info, logp_out=logp_out)
-        if fork:
-            with fused.backward_fork():
-                torch.autograd.backward([mean, ls], [g_mean, g_ls])
-        else:
-            torch.autograd.backward([mean, ls], [g_mean, g_ls])
-        return std.detach().expand_as(mean)
 
     def old_log_prob(self, pf, obs, acts, out):
         mean, _, ls = gaussian_outputs(pf, obs)
@@ -144,7 +148,7 @@ class CategoricalHead:
     def fused_ok(self, pf):
         return True
 
-    def loss_scratch(self, B, acts, device):
+    def loss_scratch(self, B, a, device):
         return ops.LossScratch(B, 1, device, categorical=True)
 
     @staticmethod
@@ -152,31 +156,18 @@ class CategoricalHead:
         z = pf.logits(obs)
         return z if z.is_contiguous() else z.contiguous()
 
-    def minibatch_actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info,
-                        logp_out=None):
+    def actor(self, pf, obs, acts, old_logp, advs, adv_table, stats_pos, clip, ent_coef, scratch, info, logp_out=None):
         logits = self._logits(pf, obs)
         g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1), old_logp, advs, adv_table, clip, ent_coef,
                                               scratch, info=info[0:16], logp_out=logp_out, stats_pos=stats_pos)
         with fused.backward_fork():
             torch.autograd.backward([logits], [g])
 
-    def log_std_row(self, pf, info):
+    def std_row(self, pf, std, info):
         pass
 
     def a2c_std_info(self, row, B, a):
         return {}                                           # a2c.py:90-94 logs std/* only `if 'std' in out`
-
-    def eager_actor(self, pf, obs, acts, old_logp, advs, adv_stats, clip, ent_coef, scratch, info, fork=False,
-                    logp_out=None):
-        logits = self._logits(pf, obs)
-        g, _ = ops.ppo_categorical_actor_loss(logits, acts.reshape(-1).contiguous(), old_logp, advs, adv_stats, clip,
-                                              ent_coef, scratch, info=info, logp_out=logp_out)
-        if fork:
-            with fused.backward_fork():
-                torch.autograd.backward([logits], [g])
-        else:
-            torch.autograd.backward([logits], [g])
-        return None
 
     def old_log_prob(self, pf, obs, acts, out):
         return ops.categorical_log_prob(self._logits(pf, obs), acts.reshape(-1).contiguous(), out=out)
@@ -186,7 +177,7 @@ class CategoricalHead:
         return ops.VMPOScratch(B - B // 2, device)
 
     def vmpo_actor(self, pf, target_pf, obs, acts, advs, adv_stats, stats_pos, dual, eta_eps, alpha_eps, per_row_kl,
-                   scratch, info, fork=False):
+                   scratch, info):
         """The actor step on the k selected rows: both policies' logits on those rows only, one loss kernel that writes
         dL/d[eta, alpha] straight into the duals' slice of the flat gradient, autograd through the policy's logits."""
         logits = self._logits(pf, obs)
@@ -194,10 +185,7 @@ class CategoricalHead:
             tlogits = self._logits(target_pf, obs)
         g = ops.vmpo_categorical_loss(logits, tlogits, acts.reshape(-1), advs.reshape(-1), adv_stats, dual.detach(),
                                       eta_eps, alpha_eps, per_row_kl, scratch, dual.grad, info, stats_pos=stats_pos)
-        if fork:
-            with fused.backward_fork():
-                torch.autograd.backward([logits], [g])
-        else:
+        with fused.backward_fork():
             torch.autograd.backward([logits], [g])
 
     # ---- TRPO (trpo.py:29-230 with the KL over probs, trpo.py:53-61)

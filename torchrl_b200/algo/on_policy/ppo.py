@@ -1,9 +1,9 @@
 """PPO on the device (API of /root/reference/torchrl/algo/on_policy/ppo.py:10-160).
 
 The per-minibatch loop (gather -> critic loss -> actor loss -> [gradient exchange] -> clip + Adam -> log row, one
-captured CUDA graph replayed opt_epochs * T/b times per epoch, no host sync inside) lives in a2c.A2C; PPO adds the
-clipped surrogate (the actor kernel's ratio mode), the optional clipped value loss, the linear LR decay and the
-target policy.
+captured CUDA graph replayed opt_epochs * T/b times per epoch, no host sync inside) and the explicit-batch `update` live
+in a2c.A2C; PPO adds the clipped surrogate (the actor kernel's ratio mode), the optional clipped value loss, the linear
+LR decay and the target policy.
 
 Exactness notes (SURVEY.md section 7):
   * old log-probs are computed once per epoch and gathered with the minibatch -- the reference recomputes
@@ -48,19 +48,17 @@ class PPO(A2C):
     def _device_path_ok(self):
         return True
 
-    def _critic_step(self, batch, info):
+    def _critic_step(self, batch, st, info):
         v = self.vf(batch["obs"])
         g_v, _ = ops.ppo_critic_loss(v.reshape(-1), batch["estimate_returns"].reshape(-1),
                                      batch["values"].reshape(-1), self.clipped_value_loss, self.clip_para,
-                                     self._mb_state["scratch"], info=info[16:17])
+                                     st["scratch"], info=info[16:17])
         with fused.backward_fork():
             torch.autograd.backward([v], [g_v.reshape(v.shape)])
 
-    def _actor_step(self, batch, info):
-        st = self._mb_state
-        self._head.minibatch_actor(self.pf, batch["obs"], batch["acts"], batch["old_logp"].reshape(-1),
-                                   batch["advs"].reshape(-1), st["adv_table"], st["upd"], self.clip_para,
-                                   self.entropy_coeff, st["scratch"], info)
+    def _actor_step(self, batch, st, info):
+        self._head.actor(self.pf, batch["obs"], batch["acts"], batch["old_logp"].reshape(-1), batch["advs"].reshape(-1),
+                         st["adv_table"], st["upd"], self.clip_para, self.entropy_coeff, st["scratch"], info)
 
     def _cache_old_logp(self):
         """log pi_old(a|s) for every stored transition, once per epoch (see module docstring).  Chunks of whole time
@@ -87,7 +85,15 @@ class PPO(A2C):
         self._hard_update_targets()                              # copy_model_params_from_to(pf, target_pf)
         self._cache_old_logp()
 
-    def _decode_info(self, row, norms, gs):
+    def _prepare_batch(self, batch, st):
+        """The batch's advantage statistics, and its old log-probs from the target policy when it brings none
+        (ppo.py:54-56)."""
+        super()._prepare_batch(batch, st)
+        if "old_logp" not in batch:
+            with torch.no_grad():
+                batch["old_logp"] = self._head.old_log_prob(self.target_pf, batch["obs"], batch["acts"], None)
+
+    def _decode_info(self, row, norms, st):
         info = atu.four_stats('advs', row[20:24])
         info['Training/vf_loss'] = float(row[16])
         info['grad_norm/vf'] = float(norms[1])
@@ -97,36 +103,6 @@ class PPO(A2C):
             info[k] = float(row[7 + i])
         info['grad_norm/pf'] = float(norms[0])
         return info
-
-    # ------------------------------------------------------------------ reference API
-    @fused.presplit_scope
-    def update(self, batch):
-        """Eager single-minibatch update with the reference's signature (ppo.py:124-152): `batch`
-        holds (B,D) arrays for obs, acts, advs, estimate_returns, values; returns the info dict of
-        Python floats (this entry point syncs; the epoch loop does not use it)."""
-        self.training_update_num += 1
-        dev = self.device
-        obs, acts, advs, rets, old_v = self._minibatch(batch, ('obs', 'acts', 'advs', 'estimate_returns', 'values'))
-        B = obs.shape[0]
-        scratch = self._head.loss_scratch(B, acts.reshape(B, -1), dev)
-        info32 = torch.zeros(32, dtype=torch.float32, device=dev)
-        adv_stats = ops.vec_stats(advs.reshape(-1), out=info32[20:24])
-        if 'old_logp' in batch:
-            old_logp = self._minibatch(batch, ('old_logp',))[0].reshape(-1)
-        else:
-            with torch.no_grad():
-                old_logp = self._head.old_log_prob(self.target_pf, obs, acts, None)
-        v = self.vf(obs)
-        g_v, _ = ops.ppo_critic_loss(v.reshape(-1), rets.reshape(-1), old_v.reshape(-1), self.clipped_value_loss,
-                                     self.clip_para, scratch, info=info32[16:17])
-        with fused.backward_fork():
-            torch.autograd.backward([v], [g_v.reshape(v.shape)])
-        self._head.eager_actor(self.pf, obs, acts, old_logp, advs.reshape(-1), adv_stats, self.clip_para,
-                               self.entropy_coeff, scratch, info32[0:16], fork=True)
-        scale = self._optimizer_step()
-        row = info32.cpu().numpy()
-        norms = self.opt.grad_norms().cpu().numpy() * scale
-        return self._decode_info(row, norms, scale)
 
     @property
     def networks(self):

@@ -9,14 +9,14 @@ The device epoch is A2C's minibatch machinery without the critic branch: the epo
 captured graph per minibatch (row gather -> policy forward -> actor loss kernel, which also writes every row's log-prob
 -> statistics of those log-probs (1) -> autograd -> clip + Adam -> info row) and one info read-back per epoch.  Both
 policy heads are served: the Gaussian policies of the continuous envs and CategoricalDisPolicy (CartPole's MLP, the
-SynthAtari CNN).  `update(batch)` is the eager form and returns the reference's info dict.
+SynthAtari CNN).  `update(batch)` runs the same minibatch step on an explicit batch and returns the reference's info
+dict.
 """
 import numpy as np
 import torch
 import torch.optim as optim
 
 from ... import ops
-from ...networks import fused
 from ...networks.nets import ZeroNet
 from ..utils import four_stats
 from .a2c import A2C
@@ -38,52 +38,28 @@ class Reinforce(A2C):
     def _gather_keys(self):
         return ["obs", "acts", "advs"]
 
-    def _mb_setup(self):
-        st = super()._mb_setup()
-        st["logp"] = torch.zeros(st["B"], dtype=torch.float32, device=self.device)
+    def _step_state(self, B, U, a):
+        st = super()._step_state(B, U, a)
+        st["logp"] = torch.zeros(B, dtype=torch.float32, device=self.device)
         return st
 
-    def _critic_step(self, batch, info):
+    def _critic_step(self, batch, st, info):
         pass
 
-    def _actor_step(self, batch, info):
-        st = self._mb_state
-        self._head.minibatch_actor(self.pf, batch["obs"], batch["acts"], None, batch["advs"].reshape(-1),
-                                   st["adv_table"], st["upd"], 0.0, self.entropy_coeff, st["scratch"], info,
-                                   logp_out=st["logp"])
+    def _actor_step(self, batch, st, info):
+        self._head.actor(self.pf, batch["obs"], batch["acts"], None, batch["advs"].reshape(-1), st["adv_table"],
+                         st["upd"], 0.0, self.entropy_coeff, st["scratch"], info, logp_out=st["logp"])
         ops.vec_stats(st["logp"], out=info[32:36])                     # logprob/* (reinforce.py:70-73)
 
-    @staticmethod
-    def _info(adv_stats, n, policy_loss, ent, logp_stats):
+    def _decode_info(self, row, norms, st):
         """The reference's info dict.  Its advs/* are NumPy statistics of the batch (reinforce.py:42-45), so advs/std
-        is the population std; the kernels' table holds torch's unbiased std of the same moments."""
-        mean, std, mx, mn = (float(v) for v in adv_stats)
+        is the population std; the kernels' table holds torch's unbiased std of the same n samples."""
+        mean, std, mx, mn = (float(v) for v in row[20:24])
+        n = float(st["n"])
         info = {'advs/mean': mean, 'advs/std': float(np.float64(std) * np.sqrt((n - 1.0) / n)), 'advs/max': mx,
-                'advs/min': mn, 'Training/policy_loss': float(policy_loss), 'ent': float(ent)}
-        info.update(four_stats('logprob', logp_stats))
+                'advs/min': mn, 'Training/policy_loss': float(row[0]), 'ent': float(row[11])}
+        info.update(four_stats('logprob', row[32:36]))
         return info
-
-    def _decode_info(self, row, norms, gs):
-        W = self.dist.world_size if (self.dist is not None and self.dist.active) else 1
-        return self._info(row[20:24], float(self._mb_state["B"] * W), row[0], row[11], row[32:36])
-
-    @fused.presplit_scope
-    def update(self, batch):
-        """One REINFORCE update on an explicit batch (reinforce.py:33-75), eagerly, through the same loss kernel and
-        the fused optimizer step; returns the reference's info dict (this entry point syncs)."""
-        self.training_update_num += 1
-        obs, acts, advs = self._minibatch(batch, ('obs', 'acts', 'advs'))
-        B = obs.shape[0]
-        scratch = self._head.loss_scratch(B, acts.reshape(B, -1), self.device)
-        info32 = torch.zeros(24, dtype=torch.float32, device=self.device)
-        logp = torch.empty(B, dtype=torch.float32, device=self.device)
-        adv_stats = ops.vec_stats(advs.reshape(-1), out=info32[16:20])
-        self._head.eager_actor(self.pf, obs, acts, None, advs.reshape(-1), adv_stats, 0.0, self.entropy_coeff,
-                               scratch, info32[0:16], logp_out=logp)
-        ops.vec_stats(logp, out=info32[20:24])
-        self._optimizer_step()
-        row = info32.cpu().numpy()
-        return self._info(row[16:20], float(advs.numel()), row[0], row[11], row[20:24])
 
     @property
     def snapshot_networks(self):

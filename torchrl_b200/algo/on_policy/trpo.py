@@ -87,19 +87,22 @@ class TRPO(A2C):
     def _step_mask(self):
         return 0b10
 
-    def _critic_step(self, batch, info):
+    def _critic_step(self, batch, st, info):
         v = self.vf(batch["obs"])
         g_v, _ = ops.ppo_critic_loss(v.reshape(-1), batch["estimate_returns"].reshape(-1), None, False, 0.0,
-                                     self._mb_state["scratch"], info=info[16:17])
+                                     st["scratch"], info=info[16:17])
         torch.autograd.backward([v], [0.5 * g_v.reshape(v.shape)])       # 0.5 * mean((V - R)^2), trpo.py:244
 
-    def _actor_step(self, batch, info):
+    def _actor_step(self, batch, st, info):
         pass
 
     def _epoch_adv_stats(self):
         pass                                                             # the value sweeps use no advantages
 
-    def _decode_info(self, row, norms, gs):
+    def _prepare_batch(self, batch, st):
+        pass
+
+    def _decode_info(self, row, norms, st):
         return {'Training/vf_loss': 0.5 * float(row[16]), 'grad_norm/vf': float(norms[1])}
 
     # ------------------------------------------------------------------ policy step
@@ -163,12 +166,8 @@ class TRPO(A2C):
     def _policy_batch(self, batch):
         """(obs (B, ...), acts, advs (B,), env-axis size or None) of an explicit whole batch: flat (B, .) or the
         (T, N, .) whole-rollout layout; uint8 frames are scaled once (OnRLAlgo._prep_obs), not merely cast."""
-        o = batch['obs']
-        if torch.is_tensor(o) and o.dtype == torch.uint8:
-            obs = self._prep_obs(o.to(self.device))
-        else:
-            obs, = self._minibatch(batch, ('obs',))
-        acts, advs = self._minibatch(batch, ('acts', 'advs'))
+        b = self._device_batch(batch, ('obs', 'acts', 'advs'))
+        obs, acts, advs = b['obs'], b['acts'], b['advs']
         lead = tuple(obs.shape[:obs.dim() - self._obs_dims])
         obs = obs.reshape((-1,) + tuple(obs.shape[len(lead):]))
         return obs, acts.reshape(obs.shape[0], -1), advs.reshape(-1), (lead[1] if len(lead) >= 2 else None)
@@ -284,19 +283,8 @@ class TRPO(A2C):
         return x
 
     def update_vf(self, batch):
-        """One eager value-function minibatch (trpo.py:232-261)."""
-        self.training_update_num += 1
-        obs, rets = self._minibatch(batch, ('obs', 'estimate_returns'))
-        B = obs.shape[0]
-        scratch = ops.LossScratch(B, 1, self.device)
-        info32 = torch.zeros(32, dtype=torch.float32, device=self.device)
-        with fused.presplit():
-            v = self.vf(obs)
-            g_v, _ = ops.ppo_critic_loss(v.reshape(-1), rets.reshape(-1), None, False, 0.0, scratch, info=info32[16:17])
-            torch.autograd.backward([v], [0.5 * g_v.reshape(v.shape)])
-            scale = self._optimizer_step(0b10)
-        return {'Training/vf_loss': 0.5 * float(info32[16].item()),
-                'grad_norm/vf': float(self.opt.grad_norms()[1].item()) * scale}
+        """One value-function minibatch on an explicit batch (trpo.py:232-261): the value sweeps' step."""
+        return A2C.update(self, batch)
 
     def update_per_epoch(self, flush_infos=True):
         """trpo.py:263-279: returns, LR decay, one whole-rollout policy step, v_opt_times value sweeps."""

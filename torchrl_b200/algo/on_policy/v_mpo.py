@@ -1,13 +1,13 @@
 """V-MPO on the device (API of /root/reference/torchrl/algo/on_policy/v_mpo.py:11-185).
 
-Same minibatch loop as A2C / PPO (a2c.A2C: row gather, per-epoch advantage statistics, fused clip + Adam for every
-optimised tensor in one step, one captured CUDA graph per minibatch, no host sync inside).  The actor step is the
-reference's (v_mpo.py:59-125): keep the half of the minibatch with the largest normalised advantages, weight the
-log-likelihood by softmax(adv / eta), add alpha * KL(pi || pi_target), learn the temperature eta and the KL
-multiplier alpha by their dual losses, clamp both at 1e-8.  The MLPs run on the library's fused layers; the
-per-sample loss assembly (sort, softmax, KL) is a handful of elementwise torch ops inside the captured graph.
-eta and alpha live in one 2-element parameter optimised by a third segment of the flat Adam (lr = plr, eps = 1e-5,
-no clipping: v_mpo.py:33-37).
+Same minibatch loop and explicit-batch `update` as A2C / PPO (a2c.A2C: row gather, per-epoch advantage statistics,
+fused clip + Adam for every optimised tensor in one step, one captured CUDA graph per minibatch, no host sync inside).
+The actor step is the reference's (v_mpo.py:59-125): keep the half of the minibatch with the largest normalised
+advantages, weight the log-likelihood by softmax(adv / eta), add alpha * KL(pi || pi_target), learn the temperature
+eta and the KL multiplier alpha by their dual losses, clamp both at 1e-8.  The MLPs run on the library's fused
+layers; the per-sample loss assembly (sort, softmax, KL) is a handful of elementwise torch ops inside the captured
+graph.  eta and alpha live in one 2-element parameter optimised by a third segment of the flat Adam (lr = plr,
+eps = 1e-5, no clipping: v_mpo.py:33-37).
 
 With a CategoricalDisPolicy the actor step runs on the library's kernels instead (csrc/categorical.cu): one launch per
 epoch selects the top half of every minibatch (`_epoch_adv_stats`), and one launch per minibatch computes the loss,
@@ -59,10 +59,10 @@ class VMPO(A2C):
     def _pre_update(self):
         self._hard_update_targets()                              # copy_model_params_from_to(pf, target_pf)
 
-    def _critic_step(self, batch, info):
+    def _critic_step(self, batch, st, info):
         v = self.vf(batch["obs"])
         g_v, _ = ops.ppo_critic_loss(v.reshape(-1), batch["estimate_returns"].reshape(-1), None, False, 0.0,
-                                     self._mb_state["scratch"], info=info[16:17])
+                                     st["scratch"], info=info[16:17])
         torch.autograd.backward([v], [g_v.reshape(v.shape)])
 
     def _actor_loss(self, obs, acts, advn, info):
@@ -87,15 +87,14 @@ class VMPO(A2C):
         ops.vec_stats(kl.detach().reshape(-1).contiguous(), out=info[40:44])
         return policy_loss + eta_loss.sum() + alpha_loss.sum()
 
-    def _actor_step(self, batch, info):
-        st = self._mb_state
+    def _actor_step(self, batch, st, info):
         if self._categorical:
             sel = st["sel"].index_select(0, st["upd"].long()).reshape(-1)        # this minibatch's top half
             self._head.vmpo_actor(self.pf, self.target_pf, batch["obs"].index_select(0, sel),
                                   batch["acts"].reshape(-1).index_select(0, sel),
                                   batch["advs"].reshape(-1).index_select(0, sel), st["adv_table"], st["upd"], self.dual,
                                   self.eta_eps, self.alpha_eps, not self.reference_quirks, st["vmpo_scratch"],
-                                  info[32:44], fork=True)
+                                  info[32:44])
             return
         row = st["adv_table"].index_select(0, st["upd"].long())                  # this minibatch's statistics
         advn = (batch["advs"].reshape(-1, 1) - row[:, 0:1]) / (row[:, 1:2] + 1e-5)
@@ -103,10 +102,15 @@ class VMPO(A2C):
         loss = self._actor_loss(batch["obs"], acts, advn, info)
         loss.backward()
 
+    def _step(self, batch, st):
+        scale = super()._step(batch, st)
+        with torch.no_grad():
+            self.dual.clamp_(min=1e-8)                                           # v_mpo.py:101-103
+        return scale
+
     def _mb_body(self):
         super()._mb_body()
         with torch.no_grad():
-            self.dual.clamp_(min=1e-8)                                           # v_mpo.py:101-103
             self._mb_state["dual_log"].index_copy_(0, self._dual_pos(), self.dual.detach().reshape(1, 2))
 
     def _dual_pos(self):
@@ -114,14 +118,23 @@ class VMPO(A2C):
         st = self._mb_state
         return ((st["upd"].long() - 1) % st["U"]).reshape(1)
 
+    def _step_state(self, B, U, a):
+        st = super()._step_state(B, U, a)
+        if self._categorical:
+            st["sel"] = torch.zeros(U, B - B // 2, dtype=torch.int64, device=self.device)
+            st["vmpo_scratch"] = self._head.vmpo_scratch(B, self.device)
+        return st
+
     def _mb_setup(self):
         st = super()._mb_setup()
         st["dual_log"] = torch.zeros(st["U"], 2, dtype=torch.float32, device=self.device)
-        if self._categorical:
-            B = st["B"]
-            st["sel"] = torch.zeros(st["U"], B - B // 2, dtype=torch.int64, device=self.device)
-            st["vmpo_scratch"] = self._head.vmpo_scratch(B, self.device)
         return st
+
+    def _prepare_batch(self, batch, st):
+        """The batch's advantage statistics and, for a categorical policy, its top half."""
+        super()._prepare_batch(batch, st)
+        if self._categorical:
+            ops.vmpo_select(batch["advs"].reshape(-1), st["adv_table"], 1, st["B"], out=st["sel"])
 
     def _epoch_adv_stats(self):
         super()._epoch_adv_stats()
@@ -137,48 +150,22 @@ class VMPO(A2C):
             info['Training/eta'], info['Training/alpha'] = float(self._dual_rows[u][0]), float(self._dual_rows[u][1])
         return infos
 
-    def _decode_info(self, row, norms, gs):
+    def _decode_info(self, row, norms, st):
         info = four_stats('advs', row[20:24])
         info['Training/vf_loss'] = float(row[16])
         info['grad_norm/vf'] = float(norms[1])
         info['Training/policy_loss'] = float(row[32])
         info['Training/alpha_loss'] = float(row[33])
-        info['Training/alpha'] = info['Training/eta'] = float("nan")             # filled by _flush_infos
+        info['Training/alpha'] = info['Training/eta'] = float("nan")             # filled by the caller
         info.update(four_stats('logprob', row[36:40]))
         info.update(four_stats('KL', row[40:44]))
         info['grad_norm/pf'] = float(norms[0])
         return info
 
     def update(self, batch):
-        """Eager single-minibatch update with the reference's signature (v_mpo.py:145-175); syncs to return floats."""
-        from ...networks import fused
-        with fused.presplit():
-            self.training_update_num += 1
-            obs, acts, advs, rets = self._minibatch(batch, ('obs', 'acts', 'advs', 'estimate_returns'))
-            B = obs.shape[0]
-            acts = acts.reshape(B, -1)
-            scratch = ops.LossScratch(B, acts.shape[1], self.device)
-            info = torch.zeros(64, dtype=torch.float32, device=self.device)
-            stats = ops.vec_stats(advs.reshape(-1), out=info[20:24])
-            v = self.vf(obs)
-            g_v, _ = ops.ppo_critic_loss(v.reshape(-1), rets.reshape(-1), None, False, 0.0, scratch, info=info[16:17])
-            torch.autograd.backward([v], [g_v.reshape(v.shape)])
-            if self._categorical:
-                a = advs.reshape(-1)
-                sel = ops.vmpo_select(a, stats, 1, B).reshape(-1)
-                self._head.vmpo_actor(self.pf, self.target_pf, obs.index_select(0, sel),
-                                      acts.reshape(-1).index_select(0, sel), a.index_select(0, sel), stats, None,
-                                      self.dual, self.eta_eps, self.alpha_eps, not self.reference_quirks,
-                                      self._head.vmpo_scratch(B, self.device), info[32:44])
-            else:
-                advn = (advs.reshape(-1, 1) - stats[0]) / (stats[1] + 1e-5)
-                self._actor_loss(obs, acts, advn, info).backward()
-            scale = self._optimizer_step()
-            with torch.no_grad():
-                self.dual.clamp_(min=1e-8)
-            out = self._decode_info(info.cpu().numpy(), self.opt.grad_norms().cpu().numpy() * scale, scale)
-            out['Training/eta'], out['Training/alpha'] = float(self.dual[0].item()), float(self.dual[1].item())
-            return out
+        info = super().update(batch)
+        info['Training/eta'], info['Training/alpha'] = (float(v) for v in self.dual.detach().cpu().numpy())
+        return info
 
     @property
     def networks(self):
