@@ -124,6 +124,9 @@ TRL_API int trl_transpose_f32(const float* in, float* out, int64_t rows, int col
   using namespace trl;
   TRL_REQUIRE(rows >= 1 && cols >= 1, "trl_transpose_f32: bad sizes");
   TRL_REQUIRE(in && out, "trl_transpose_f32: null pointer");
+  // the row tiles run on grid.y (at most 65535 blocks)
+  TRL_REQUIRE(ceil_div<long long>(rows, 32) <= 65535LL,
+              "trl_transpose_f32: bad sizes rows=%lld (at most 65535 * 32 rows)", (long long)rows);
   const dim3 grid(static_cast<unsigned>(ceil_div(cols, 32)), static_cast<unsigned>(ceil_div<long long>(rows, 32)));
   transpose_kernel<<<grid, dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(in, out, rows, cols);
   return check_launch("transpose_kernel");

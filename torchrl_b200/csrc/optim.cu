@@ -122,7 +122,9 @@ __global__ void polyak_kernel(float* __restrict__ target, const float* __restric
                               float* __restrict__ t_hi, float* __restrict__ t_lo) {
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float w = target[i] * (1.0f - tau) + source[i] * tau;
+    // target * (1 - tau) + source * tau with every operation rounded on its own, as torch evaluates the soft update
+    // (no contraction into an FFMA): the target and its TF32 planes equal torch's bit for bit
+    const float w = __fadd_rn(__fmul_rn(target[i], __fsub_rn(1.0f, tau)), __fmul_rn(source[i], tau));
     target[i] = w;
     if (t_hi) split_tf32_store(w, t_hi, t_lo, i);
   }
