@@ -432,6 +432,33 @@ int trl_cartpole_step(float* state, const float* actions, int* elapsed, const in
                       double* norm_mean, double* norm_var, double* norm_count, unsigned* ticket, int* any_reset,
                       const int* t_ptr, int64_t N, float reward_scale, int max_episode_steps, int max_episode_frames,
                       int merge_stats, void* stream);
+/* ---- K1 for Pendulum-v1: gym.make("Pendulum-v1") (torchrl/env/get_env.py:53) with NormAct.action
+ * (env/continuous_wrapper.py:18-20), TimeLimitAugment.step (env/base_wrapper.py:152-156), RewardShift.reward
+ * (env/base_wrapper.py:37-41) and VecEnv.step / partial_reset (env/vecenv.py:47-61) fused in (defined in
+ * oracle/pendulum.py).  phys (N,2) fp64 (theta, theta_dot) in place; obs (N,3) fp32 raw observation (cos, sin,
+ * theta_dot).  actions (N) in [-1, 1]: the torque is NormAct's map to [-2, 2] in fp32, widened exactly; the step is fp64
+ * in gym's order, the velocity clipped before it moves the angle (v1).  A non-finite action sets *action_error = 1 and
+ * leaves that env's state and observation unchanged (reward 0).  done = (elapsed >= max_episode_steps), time_limit =
+ * done && elapsed == max_episode_steps.
+ * partial ((trl_pendulum_num_ctas(N), 6) doubles) / batch_sums (6) / norm_*: the NormObs batch moments of the three
+ * observation columns, as in trl_cartpole_step. */
+int trl_pendulum_num_ctas(int64_t N);
+int trl_pendulum_step(double* phys, float* obs, const float* actions, int* elapsed, const int* step_count,
+                      float* reward, uint8_t* done, uint8_t* time_limit, int* action_error, double* partial,
+                      double* batch_sums, double* norm_mean, double* norm_var, double* norm_count, unsigned* ticket,
+                      int* any_reset, const int* t_ptr, int64_t N, float reward_scale, int max_episode_steps,
+                      int max_episode_frames, int merge_stats, void* stream);
+/* PendulumEnv.reset + VecEnv.partial_reset (env/vecenv.py:47-51), and for a collector the partial reset of
+ * collect_finalize (theta = pi (2U - 1), theta_dot = 2U - 1 in fp64 from the counter hash of trl_synth_env_reset).
+ * Selected envs: step_count[n] == 0 when step_count is given (after trl_collect_finalize with external-env arguments
+ * this holds exactly for the envs it cut), else mask[n] != 0, else all.  They get a new state and raw observation,
+ * elapsed = 0, episode += 1.  With cur_ob (needs step_count, next_norm, any_reset, t_ptr) it also writes the next
+ * observation as collect_finalize does: raw without norm_mean; raw for all envs when raw_obs_after_reset and
+ * any_reset[*t_ptr & 1]; otherwise clip((raw - mean) / (sqrt(var) + 1e-4)) on reset rows and next_norm on the rest. */
+int trl_pendulum_reset(double* phys, float* obs, int* elapsed, unsigned* episode, const unsigned* seeds,
+                       const uint8_t* mask, const int* step_count, const float* next_norm, float* cur_ob,
+                       const int* any_reset, const int* t_ptr, const double* norm_mean, const double* norm_var,
+                       int64_t N, double clip, int raw_obs_after_reset, void* stream);
 
 /* ScaledFloatFrame (env/atari_wrapper.py:171-180): out = in * scale */
 int trl_u8_to_f32(const uint8_t* in, float* out, int64_t n, float scale, void* stream);

@@ -116,6 +116,9 @@ SIGNATURES = {
     "trl_u8_to_f32": [vp, vp, i64, f32, vp],
     "trl_cartpole_num_ctas": [i64],
     "trl_cartpole_step": [vp] * 16 + [i64, f32, i32, i32, i32, vp],
+    "trl_pendulum_num_ctas": [i64],
+    "trl_pendulum_step": [vp] * 17 + [i64, f32, i32, i32, i32, vp],
+    "trl_pendulum_reset": [vp] * 13 + [i64, f64, i32, vp],
     "trl_offpolicy_scratch_doubles": [i64],
     "trl_td_target": [vp, vp, vp, vp, vp, vp, f32, f32, i64, vp, vp, vp, vp, vp],
     "trl_td3_smooth_action": [vp, vp, f32, f32, u64, vp, i64, vp, vp],
@@ -135,7 +138,7 @@ _RESTYPES = {"trl_last_error": ctypes.c_char_p, "trl_ppo_actor_scratch_doubles":
              "trl_skinny_dgrad_act_scratch_floats": ctypes.c_int64, "trl_comm_ll_recv_bytes": ctypes.c_int64}
 # entry points that return a value rather than an error code
 _VALUE_FUNCS = ("trl_abi_version", "trl_synth_env_smem_bytes", "trl_synth_env_num_ctas", "trl_cartpole_num_ctas",
-                "trl_comm_flag_bytes",
+                "trl_pendulum_num_ctas", "trl_comm_flag_bytes",
                 "trl_comm_ipc_handle_bytes", "trl_comm_scratch_doubles", "trl_comm_ll_recv_bytes",
                 "trl_ppo_actor_scratch_doubles", "trl_ppo_categorical_actor_scratch_doubles", "trl_vmpo_categorical_scratch_doubles",
                 "trl_grad_sumsq_blocks")

@@ -123,7 +123,10 @@ class VecCollector:
     def _finalize(self, v_next):
         env, rb = self.env, self.replay_buffer
         nrm = env._obs_normalizer if getattr(env, "obs_norm", False) else None
-        ext = self._host_env            # host envs: the kernel stores rows / counters, the host env resets
+        # host envs, and device envs whose observation is not their state (`resets_itself`): the kernel stores rows and
+        # the collector's counters and carries the stepped observation forward; the env resets the envs it cut
+        own = getattr(env, "resets_itself", False)
+        ext = self._host_env or own
         ops.collect_finalize(self.current_ob, env.obs_out, None if ext else env.state, self._act, self._value, v_next,
                              env.reward, env.done, env.time_limit, None if ext else env.elapsed,
                              None if ext else env.episode, None if ext else env.seeds, self.current_step,
@@ -134,6 +137,8 @@ class VecCollector:
                              rb._top_dev, self.max_episode_frames, getattr(self, "discount", 0.99),
                              getattr(env, "init_scale", synth_spec.INIT_SCALE), nrm.clip if nrm is not None else 10.0,
                              self.on_policy, self.reference_quirks)
+        if own:
+            env.collector_reset(self.current_step, self.current_ob, rb._top_dev, self.reference_quirks)
 
     def _step_body(self, bootstrap):
         with torch.no_grad():

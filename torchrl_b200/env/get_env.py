@@ -1,13 +1,15 @@
 """Env factories with the reference's names (/root/reference/torchrl/env/get_env.py:32-87).
 
 Synthetic ids ("SynthHalfCheetah-v0", "SynthAnt-v0") build the device-resident
-SynthVecEnv, "SynthAtari-v0" the pixel env and "CartPole-v0" / "CartPole-v1" the device CartPole; any other id needs a real gym + the host-env bridge (SURVEY.md section 8(f).1), which is
-outside this round's hot path and raises.
+SynthVecEnv, "SynthAtari-v0" the pixel env, "CartPole-v0" / "CartPole-v1" the device CartPole and "Pendulum-v1" the
+device Pendulum; any other id (Pendulum-v0 included: its dynamics differ from v1's) needs a real gym + the host-env
+bridge (SURVEY.md section 8(f).1), which is outside this round's hot path and raises.
 """
 import torch
 
 from . import synth_spec
 from .cartpole import CartPoleVecEnv, is_cartpole
+from .pendulum import PendulumVecEnv, is_pendulum
 from .synth import SynthVecEnv
 from .synth_atari import SynthAtariVecEnv, ENV_ID as ATARI_ID
 
@@ -27,6 +29,8 @@ def get_vec_env(env_id, env_param, vec_env_nums, device=None, **kwargs):
         return SynthAtariVecEnv(vec_env_nums, env_param, device=_device(device), **kwargs)
     if is_cartpole(env_id):
         return CartPoleVecEnv(env_id, vec_env_nums, env_param, device=_device(device), **kwargs)
+    if is_pendulum(env_id):
+        return PendulumVecEnv(vec_env_nums, env_param, device=_device(device), **kwargs)
     raise NotImplementedError("only the synthetic device envs are built in this round: %r" % (env_id,))
 
 

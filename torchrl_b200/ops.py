@@ -1033,6 +1033,53 @@ def cartpole_step(state, actions, elapsed, step_count, reward, done, time_limit,
               int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream(), kernels=int(N > 0))
 
 
+def pendulum_num_ctas(N):
+    return int(_lib.load().trl_pendulum_num_ctas(int(N)))
+
+
+def pendulum_step(phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error, partial, batch_sums,
+                  norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale, max_episode_steps,
+                  max_episode_frames, merge_stats):
+    """One Pendulum-v1 step of all N envs (csrc/pendulum.cu): phys (N, 2) fp64 and obs (N, 3) in place, actions (N) in
+    [-1, 1] (a non-finite one sets action_error (1) int32).  partial / batch_sums / norm_*: the observation-normaliser
+    moments (all None: not estimated); step_count / t_ptr: the collector's step counters and ring row (None outside a
+    collector)."""
+    N = phys.shape[0]
+    if phys.dim() != 2 or phys.shape[1] != 2 or tuple(obs.shape) != (N, 3):
+        raise ValueError("pendulum_step: phys must be (N, 2) and obs (N, 3), got %s and %s"
+                         % (tuple(phys.shape), tuple(obs.shape)))
+    if actions.numel() != N:
+        raise ValueError("pendulum_step: one action per env expected, got %d for %d envs" % (actions.numel(), N))
+    _lib.call("trl_pendulum_step", _chk(phys, F64, "phys"), _chk(obs, F32, "obs"), _chk(actions, F32, "actions"),
+              _chk(elapsed, I32, "elapsed"), _opt(step_count, I32, "step_count"), _chk(reward, F32, "reward"),
+              _chk(done, U8, "done"), _chk(time_limit, U8, "time_limit"), _chk(action_error, I32, "action_error"),
+              _opt(partial, F64, "partial"), _opt(batch_sums, F64, "batch_sums"), _opt(norm_mean, F64, "norm_mean"),
+              _opt(norm_var, F64, "norm_var"), _opt(norm_count, F64, "norm_count"), _chk(ticket, I32, "ticket"),
+              _chk(any_reset, I32, "any_reset"), _opt(t_ptr, I32, "t_ptr"), N, float(reward_scale),
+              int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream(), kernels=int(N > 0))
+
+
+def pendulum_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=None, next_norm=None, cur_ob=None,
+                   any_reset=None, t_ptr=None, norm_mean=None, norm_var=None, clip=10.0, raw_obs_after_reset=True):
+    """New Pendulum episodes for every env (mask and step_count None), the envs of the uint8 `mask`, or those whose
+    int32 `step_count` is 0 (the collector's path).  With `cur_ob` the next observation of every env is written there
+    as collect_finalize writes it (next_norm / any_reset / t_ptr / norm_* / clip / raw_obs_after_reset)."""
+    N = phys.shape[0]
+    if phys.dim() != 2 or phys.shape[1] != 2 or tuple(obs.shape) != (N, 3):
+        raise ValueError("pendulum_reset: phys must be (N, 2) and obs (N, 3), got %s and %s"
+                         % (tuple(phys.shape), tuple(obs.shape)))
+    if mask is not None and step_count is not None:
+        raise ValueError("pendulum_reset: select envs by mask or by step_count, not both")
+    if cur_ob is not None and (step_count is None or next_norm is None or any_reset is None or t_ptr is None):
+        raise ValueError("pendulum_reset: cur_ob needs step_count, next_norm, any_reset and t_ptr")
+    _lib.call("trl_pendulum_reset", _chk(phys, F64, "phys"), _chk(obs, F32, "obs"), _chk(elapsed, I32, "elapsed"),
+              _chk(episode, I32, "episode"), _chk(seeds, I32, "seeds"), _opt(mask, U8, "mask"),
+              _opt(step_count, I32, "step_count"), _opt(next_norm, F32, "next_norm"), _opt(cur_ob, F32, "cur_ob"),
+              _opt(any_reset, I32, "any_reset"), _opt(t_ptr, I32, "t_ptr"), _opt(norm_mean, F64, "norm_mean"),
+              _opt(norm_var, F64, "norm_var"), N, float(clip), int(bool(raw_obs_after_reset)), _stream(),
+              kernels=int(N > 0))
+
+
 def synth_atari_reset(obs, latent, elapsed, episode, seeds, mask=None, zero_is_mask=None, episode_bias=0, bump=1):
     """New episodes for every env, the envs of the uint8 `mask`, or those whose int32 `zero_is_mask` entry is 0."""
     _lib.call("trl_synth_atari_reset", _chk(obs, U8, "obs"), _chk(latent, I32, "latent"), _chk(elapsed, I32, "elapsed"),
