@@ -5,20 +5,13 @@
 // oracle/synth_atari.py (pure integer arithmetic => the CUDA env is BIT-EXACT against it).  One CTA per env:
 // shift the 4-frame stack by one frame, render the new 84x84 frame, advance the latent state.  HBM traffic
 // per env-step: 21 KB read + 28 KB written (uint8) -- HBM-bound at large N.
-#include "common.cuh"
+#include "env_common.cuh"
 
 namespace trl {
 
 constexpr int kAH = 84, kAW = 84, kFrame = kAH * kAW;      // 7056 bytes = 441 x 16
 constexpr int kPaddleY = 78, kPaddleW = 12, kBall = 4;
 
-__device__ __forceinline__ uint32_t amix32(uint32_t x) {
-  x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ uint32_t ahash(uint32_t seed, uint32_t episode, uint32_t j) {
-  return amix32(seed * 0x9E3779B1u + episode * 0x85EBCA77u + j * 0xC2B2AE3Du + 0x27D4EB2Fu);
-}
 __device__ __forceinline__ uint8_t apixel(int x, int y, int bx, int by, int px) {
   if (x >= bx && x < bx + kBall && y >= by && y < by + kBall) return 255;
   if (y >= kPaddleY && y < kPaddleY + 2 && x >= px && x < px + kPaddleW) return 200;
@@ -86,12 +79,13 @@ __global__ void __launch_bounds__(256) synth_atari_reset_kernel(uint8_t* __restr
   if (mask && !mask[n]) return;
   if (zero_is_mask && zero_is_mask[n] != 0) return;
   const unsigned seed = seeds[n], ep = episode[n] - static_cast<unsigned>(episode_bias);
-  const int h0 = static_cast<int>(ahash(seed, ep, 0) % 72u), h1 = static_cast<int>(ahash(seed, ep, 1) % 40u);
-  const unsigned h2 = ahash(seed, ep, 2), h3 = ahash(seed, ep, 3);
+  const int h0 = static_cast<int>(counter_hash(seed, ep, 0) % 72u);
+  const int h1 = static_cast<int>(counter_hash(seed, ep, 1) % 40u);
+  const unsigned h2 = counter_hash(seed, ep, 2), h3 = counter_hash(seed, ep, 3);
   const int bx = 4 + h0, by = 4 + h1;
   const int vx = ((h2 & 1u) ? 1 : -1) * (1 + static_cast<int>((h2 >> 1) & 1u));
   const int vy = 1 + static_cast<int>(h3 & 1u);
-  const int px = static_cast<int>(ahash(seed, ep, 4) % 73u);
+  const int px = static_cast<int>(counter_hash(seed, ep, 4) % 73u);
   uint8_t* o = obs + n * 4 * kFrame;
   for (int c = 0; c < 4; ++c) arender(o + c * kFrame, bx, by, px);     // FrameStack.reset repeats the first frame
   if (threadIdx.x == 0) {

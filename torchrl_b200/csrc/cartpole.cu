@@ -14,12 +14,11 @@
 // -fmad=true would otherwise allow) and rounded to fp32 once.  Thresholds are compared on the rounded state.
 //
 // Layout: state (N,4) fp32 row-major == the raw observation; one thread per env, kCartThreads envs per CTA.
-#include "reduce.cuh"
+#include "env_common.cuh"
 
 namespace trl {
 
 constexpr int kCartThreads = 256;
-constexpr int kCartWarps = kCartThreads / 32;
 
 // gym's CartPoleEnv constants (classic_control/cartpole.py), derived quantities computed as gym computes them
 constexpr double kGravity = 9.8;
@@ -37,24 +36,8 @@ constexpr double kXThreshold = 2.4;
 struct CartPoleParams {
   float* __restrict__ state;            // (N,4) in/out: x, x_dot, theta, theta_dot
   const float* __restrict__ actions;    // (N) 0.0 or 1.0
-  int* __restrict__ elapsed;            // (N) env-side step counter (TimeLimit._elapsed_steps)
-  const int* __restrict__ step_count;   // (N) collector-side counter or nullptr
-  float* __restrict__ reward;           // (N)
-  uint8_t* __restrict__ done;           // (N)
-  uint8_t* __restrict__ time_limit;     // (N)
   int* __restrict__ action_error;       // (1) set to 1 when an action is neither 0 nor 1
-  double* __restrict__ partial;         // (grid, 8) per-CTA column sums / sums of squares, or nullptr
-  double* __restrict__ batch_sums;      // (8) reduced sums (written by the last CTA) or nullptr
-  double* __restrict__ norm_mean;       // (4) running mean   (merged in-kernel if merge != 0)
-  double* __restrict__ norm_var;        // (4)
-  double* __restrict__ norm_count;      // (1)
-  unsigned* __restrict__ ticket;        // (1) zero-initialised
-  int* __restrict__ any_reset;          // (2) double-buffered "some env needs a reset" flag, or nullptr
-  const int* __restrict__ t_ptr;        // (1) device step index (selects the flag slot), or nullptr
-  long long N;
-  float reward_scale;
-  int max_episode_steps, max_episode_frames;
-  int merge;                            // 1: Chan-merge batch moments into norm_* in the last CTA
+  EnvStepFields env;                    // D = 4
 };
 
 // One Euler step of gym's CartPoleEnv.step in fp64, every operation rounded once, in gym's evaluation order.
@@ -75,14 +58,11 @@ __device__ __forceinline__ void cartpole_dynamics(const float s[4], double force
 }
 
 __global__ void __launch_bounds__(kCartThreads) cartpole_step_kernel(const CartPoleParams p) {
-  __shared__ double sh[kCartWarps][8];
-  __shared__ double sred[8];
-  const int tid = threadIdx.x;
-  const long long n = static_cast<long long>(blockIdx.x) * kCartThreads + tid;
-  const bool live = n < p.N;
+  const EnvStepFields& f = p.env;
+  const long long n = static_cast<long long>(blockIdx.x) * kCartThreads + threadIdx.x;
   float s2[4] = {0.f, 0.f, 0.f, 0.f};
-  int local_reset = 0;
-  if (live) {
+  bool local_reset = false;
+  if (n < f.N) {
     float s[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) s[j] = p.state[n * 4 + j];
@@ -97,57 +77,13 @@ __global__ void __launch_bounds__(kCartThreads) cartpole_step_kernel(const CartP
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) p.state[n * 4 + j] = s2[j];
-    const int el = p.elapsed[n] + 1;
-    p.elapsed[n] = el;
-    const bool done_dyn = fabs(static_cast<double>(s2[0])) > kXThreshold ||
+    const bool terminal = fabs(static_cast<double>(s2[0])) > kXThreshold ||
                           fabs(static_cast<double>(s2[2])) > kThetaThreshold;
-    const bool done = done_dyn || el >= p.max_episode_steps;
-    p.reward[n] = p.reward_scale;                     // 1.0 on every step, the terminating one included
-    p.done[n] = done ? 1 : 0;
-    p.time_limit[n] = (done && el == p.max_episode_steps) ? 1 : 0;
-    const bool surpass = p.step_count ? (p.step_count[n] + 1 >= p.max_episode_frames) : false;
-    local_reset = (done || surpass) ? 1 : 0;
+    // reward 1.0 on every step, the terminating one included
+    local_reset = env_row_end(f, n, terminal, f.reward_scale);
   }
-  if (p.any_reset) {
-    const int t = p.t_ptr ? *p.t_ptr : 0;
-    if (blockIdx.x == 0 && tid == 0) p.any_reset[(t + 1) & 1] = 0;  // slot of the *next* step
-    if (__syncthreads_or(local_reset) && tid == 0) atomicOr(&p.any_reset[t & 1], 1);
-  }
-
-  if (p.partial) {
-    // per-feature batch moments of this CTA's envs: warp shuffles, then thread k folds the warps in order
-    const int lane = tid & 31, wid = tid >> 5;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const double x = static_cast<double>(s2[j]);
-      const double ws = warp_sum(x), wq = warp_sum(x * x);
-      if (lane == 0) { sh[wid][j] = ws; sh[wid][4 + j] = wq; }
-    }
-    __syncthreads();
-    if (tid < 8) {
-      double t = 0.0;
-#pragma unroll
-      for (int w = 0; w < kCartWarps; ++w) t += sh[w][tid];
-      p.partial[static_cast<long long>(blockIdx.x) * 8 + tid] = t;
-    }
-    if (last_cta(p.ticket, gridDim.x)) {
-      // warp k folds quantity k over the CTAs: lanes stride over CTAs, then one shuffle reduction (fixed order)
-      if (wid < 8) {
-        double acc = 0.0;
-        for (unsigned b = lane; b < gridDim.x; b += 32) acc += __ldcg(p.partial + static_cast<long long>(b) * 8 + wid);
-        acc = warp_sum(acc);
-        if (lane == 0) sred[wid] = acc;
-      }
-      __syncthreads();
-      if (tid < 4) {
-        const double s = sred[tid], q = sred[4 + tid];
-        if (p.batch_sums) { p.batch_sums[tid] = s; p.batch_sums[4 + tid] = q; }
-        if (p.merge) chan_merge(s, q, static_cast<double>(p.N), *p.norm_count, p.norm_mean[tid], p.norm_var[tid]);
-      }
-      __syncthreads();   // every thread has read *norm_count
-      if (tid == 0 && p.merge) *p.norm_count = *p.norm_count + static_cast<double>(p.N);
-    }
-  }
+  update_any_reset(f, local_reset);
+  if (f.partial) env_moments<4, kCartThreads>(f, s2);
 }
 
 }  // namespace trl
@@ -167,13 +103,10 @@ TRL_API int trl_cartpole_step(float* state, const float* actions, int* elapsed, 
   if (N == 0) return TRL_OK;
   TRL_REQUIRE(state && actions && elapsed && reward && done && time_limit && action_error,
               "trl_cartpole_step: null pointer");
-  TRL_REQUIRE(!partial || ticket, "trl_cartpole_step: statistics requested without a ticket counter");
-  TRL_REQUIRE(!(merge_stats && partial) || (norm_mean && norm_var && norm_count),
-              "trl_cartpole_step: merge_stats needs norm_mean/var/count");
-  TRL_REQUIRE(!t_ptr || any_reset, "trl_cartpole_step: t_ptr given without the any_reset flag");
-  CartPoleParams p{state, actions, elapsed, step_count, reward, done, time_limit, action_error, partial, batch_sums,
-                   norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps,
-                   max_episode_frames, merge_stats};
+  CartPoleParams p{state, actions, action_error,
+                   {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean, norm_var, norm_count,
+                    ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps, max_episode_frames, merge_stats}};
+  if (const int e = check_env_step("trl_cartpole_step", p.env)) return e;
   cartpole_step_kernel<<<trl_cartpole_num_ctas(N), kCartThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("cartpole_step_kernel");
 }

@@ -9,21 +9,11 @@
 //   BaseReplayBuffer.add_sample       /root/reference/torchrl/replay_buffers/base.py:19-37
 // The time row `t` is read from device memory so that one captured CUDA graph of the whole
 // step can be replayed for every row of the epoch (pointers in the graph never change).
-#include "common.cuh"
+#include "env_common.cuh"
 
 namespace trl {
 
 constexpr float kLogSqrt2Pi = 0.9189385332046727f;  // 0.5*log(2*pi)
-
-__host__ __device__ __forceinline__ uint32_t mix32b(uint32_t x) {
-  x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
-  return x;
-}
-__host__ __device__ __forceinline__ float reset_value_b(uint32_t seed, uint32_t episode, uint32_t j, double init_scale) {
-  const uint32_t key = seed * 0x9E3779B1u + episode * 0x85EBCA77u + j * 0xC2B2AE3Du + 0x27D4EB2Fu;
-  const float u = float(mix32b(key) >> 8) * (1.0f / 16777216.0f);
-  return float(init_scale * (2.0 * double(u) - 1.0));
-}
 
 // ------------------------------------------------------------------------------------ K3
 struct SampleParams {
@@ -220,29 +210,20 @@ __global__ void __launch_bounds__(256) collect_finalize_kernel(const FinalizePar
     for (int i = tid; i < ne * o; i += nthr) p.cur_ob_out[env_base * o + i] = p.next_norm[env_base * o + i];
     return;
   }
-  // partial reset + next current_ob
+  // partial reset + next current_ob; under quirk A.1 no row is normalised, so a reset without the flag carries over
+  const bool all_raw = !p.norm_mean || (p.raw_obs_after_reset && any_reset);
   for (int i = tid; i < ne * o; i += nthr) {
     const int e = i / o, j = i - e * o;
     const long long n = env_base + e;
     float raw;
     if (s_mask[e]) {
-      raw = reset_value_b(p.seeds[n], p.episode[n], j, p.init_scale);
+      raw = reset_value(p.seeds[n], p.episode[n], j, p.init_scale);
       p.state[n * o + j] = raw;
     } else {
       raw = p.state[n * o + j];
     }
-    float ob;
-    if (!p.norm_mean) {
-      ob = raw;                                   // no NormObs: observations are raw throughout
-    } else if (p.raw_obs_after_reset) {
-      ob = any_reset ? raw : p.next_norm[n * o + j];
-    } else if (s_mask[e]) {
-      double y = (static_cast<double>(raw) - p.norm_mean[j]) / (sqrt(p.norm_var[j]) + 1e-4);
-      ob = static_cast<float>(fmin(fmax(y, -p.clip), p.clip));
-    } else {
-      ob = p.next_norm[n * o + j];
-    }
-    p.cur_ob_out[n * o + j] = ob;
+    p.cur_ob_out[n * o + j] = next_observation(all_raw, s_mask[e] && !p.raw_obs_after_reset, raw,
+                                               p.next_norm + n * o + j, p.norm_mean, p.norm_var, j, p.clip);
   }
   __syncthreads();
   if (tid < ne && s_mask[tid]) p.episode[env_base + tid] += 1u;

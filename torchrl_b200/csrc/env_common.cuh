@@ -1,0 +1,138 @@
+// env_common.cuh -- what the device env kernels share: the reset counter hash, the fields and bookkeeping of a step
+// (TimeLimitAugment, the collector's reset flag, NormObs's batch moments) and the collector's next-observation rule.
+// Each env's .cu file keeps its physics, its parameter struct and its launch.
+#pragma once
+#include "reduce.cuh"
+
+namespace trl {
+
+// ---- the reset counter hash (oracle/synth_env.py:hash_uniform) ------------------------------------------------------
+__host__ __device__ __forceinline__ uint32_t counter_hash(uint32_t seed, uint32_t episode, uint32_t j) {
+  uint32_t x = seed * 0x9E3779B1u + episode * 0x85EBCA77u + j * 0xC2B2AE3Du + 0x27D4EB2Fu;
+  x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
+  return x;
+}
+// U(seed, episode, j): 24 random bits / 2^24 -- exact in fp32
+__host__ __device__ __forceinline__ float counter_uniform(uint32_t seed, uint32_t episode, uint32_t j) {
+  return float(counter_hash(seed, episode, j) >> 8) * (1.0f / 16777216.0f);
+}
+__host__ __device__ __forceinline__ float reset_value(uint32_t seed, uint32_t episode, uint32_t j, double init_scale) {
+  // INIT_SCALE * (2u - 1) evaluated in fp64 then rounded once, like the float64 oracle cast to fp32
+  return float(init_scale * (2.0 * double(counter_uniform(seed, episode, j)) - 1.0));
+}
+
+// ---- one step of N envs ---------------------------------------------------------------------------------------------
+// The fields every env step kernel has besides its physics; D below is the observation's feature count.
+struct EnvStepFields {
+  int* __restrict__ elapsed;            // (N) env-side step counter (TimeLimit._elapsed_steps)
+  const int* __restrict__ step_count;   // (N) collector-side counter or nullptr
+  float* __restrict__ reward;           // (N)
+  uint8_t* __restrict__ done;           // (N)
+  uint8_t* __restrict__ time_limit;     // (N)
+  double* __restrict__ partial;         // (grid, 2*D) per-CTA column sums / sums of squares, or nullptr
+  double* __restrict__ batch_sums;      // (2*D) reduced sums (written by the last CTA) or nullptr
+  double* __restrict__ norm_mean;       // (D) running mean   (merged in-kernel if merge != 0)
+  double* __restrict__ norm_var;        // (D)
+  double* __restrict__ norm_count;      // (1)
+  unsigned* __restrict__ ticket;        // (1) zero-initialised
+  int* __restrict__ any_reset;          // (2) double-buffered "some env needs a reset" flag, or nullptr
+  const int* __restrict__ t_ptr;        // (1) device step index (selects the flag slot), or nullptr
+  long long N;
+  float reward_scale;
+  int max_episode_steps, max_episode_frames;
+  int merge;                            // 1: Chan-merge batch moments into norm_* in the last CTA
+};
+
+// The step arguments' rules that every env step shares; `fn` names the entry point in the message.
+inline int check_env_step(const char* fn, const EnvStepFields& f) {
+  TRL_REQUIRE(!f.partial || f.ticket, "%s: statistics requested without a ticket counter", fn);
+  TRL_REQUIRE(!(f.merge && f.partial) || (f.norm_mean && f.norm_var && f.norm_count),
+              "%s: merge_stats needs norm_mean/var/count", fn);
+  TRL_REQUIRE(!f.t_ptr || f.any_reset, "%s: t_ptr given without the any_reset flag", fn);
+  return TRL_OK;
+}
+
+// The end of env n's step (TimeLimitAugment): counts the step and stores its reward (already scaled), done and
+// time_limit.  Returns whether the env needs a reset: done, or cut by the collector's max_episode_frames ("surpass").
+__device__ __forceinline__ bool env_row_end(const EnvStepFields& f, long long n, bool terminal, float reward) {
+  const int el = f.elapsed[n] + 1;
+  f.elapsed[n] = el;
+  const bool done = terminal || el >= f.max_episode_steps;
+  f.reward[n] = reward;
+  f.done[n] = done ? 1 : 0;
+  f.time_limit[n] = (done && el == f.max_episode_steps) ? 1 : 0;
+  const bool surpass = f.step_count ? (f.step_count[n] + 1 >= f.max_episode_frames) : false;
+  return done || surpass;
+}
+
+// any_reset[t & 1] |= "an env of this CTA needs a reset", and CTA 0 clears the slot of the next step.  Called by every
+// thread of the CTA (a barrier).
+__device__ __forceinline__ void update_any_reset(const EnvStepFields& f, bool local_reset) {
+  if (f.any_reset) {
+    const int t = f.t_ptr ? *f.t_ptr : 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) f.any_reset[(t + 1) & 1] = 0;  // slot of the *next* step
+    if (__syncthreads_or(local_reset) && threadIdx.x == 0) atomicOr(&f.any_reset[t & 1], 1);
+  }
+}
+
+// The last CTA's tail for feature j of D, given the batch's sum s and sum of squares q: batch_sums, then the merge.
+__device__ __forceinline__ void merge_feature(const EnvStepFields& f, int D, int j, double s, double q) {
+  if (f.batch_sums) { f.batch_sums[j] = s; f.batch_sums[D + j] = q; }
+  if (f.merge) chan_merge(s, q, static_cast<double>(f.N), *f.norm_count, f.norm_mean[j], f.norm_var[j]);
+}
+// After every merge_feature of the last CTA (called by all its threads): the count grows by the batch.
+__device__ __forceinline__ void merge_count(const EnvStepFields& f) {
+  __syncthreads();   // every thread has read *norm_count
+  if (threadIdx.x == 0 && f.merge) *f.norm_count = *f.norm_count + static_cast<double>(f.N);
+}
+
+// NormObs's batch moments for the envs that run one thread per env (kThreads per CTA): x is this thread's observation
+// (zeros past N).  Warp shuffles, then thread k folds the warps' value of quantity k in order into this CTA's partial;
+// the last CTA's warp k folds quantity k over the CTAs (lanes stride over them, then one shuffle reduction: a fixed
+// order) and merges.  Called by every thread.
+template <int D, int kThreads>
+__device__ __forceinline__ void env_moments(const EnvStepFields& f, const float (&x)[D]) {
+  constexpr int kWarps = kThreads / 32;
+  __shared__ double sh[kWarps][2 * D];
+  __shared__ double sred[2 * D];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+#pragma unroll
+  for (int j = 0; j < D; ++j) {
+    const double v = static_cast<double>(x[j]);
+    const double ws = warp_sum(v), wq = warp_sum(v * v);
+    if (lane == 0) { sh[wid][j] = ws; sh[wid][D + j] = wq; }
+  }
+  __syncthreads();
+  if (tid < 2 * D) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) t += sh[w][tid];
+    f.partial[static_cast<long long>(blockIdx.x) * 2 * D + tid] = t;
+  }
+  if (last_cta(f.ticket, gridDim.x)) {
+    if (wid < 2 * D) {
+      double acc = 0.0;
+      for (unsigned b = lane; b < gridDim.x; b += 32)
+        acc += __ldcg(f.partial + static_cast<long long>(b) * 2 * D + wid);
+      acc = warp_sum(acc);
+      if (lane == 0) sred[wid] = acc;
+    }
+    __syncthreads();
+    if (tid < D) merge_feature(f, D, tid, sred[tid], sred[D + tid]);
+    merge_count(f);
+  }
+}
+
+// ---- the collector's next observation -------------------------------------------------------------------------------
+// Feature j of the observation the policy acts on next: the raw one when `all_raw` (no NormObs, or reference quirk A.1
+// (SURVEY.md) after any reset), the raw one normalised and clipped in fp64 when `normalise` (a reset row), else the
+// observation the step returned (*carried).
+__device__ __forceinline__ float next_observation(bool all_raw, bool normalise, float raw, const float* carried,
+                                                  const double* norm_mean, const double* norm_var, int j, double clip) {
+  if (all_raw) return raw;
+  if (!normalise) return *carried;
+  const double y = (static_cast<double>(raw) - norm_mean[j]) / (sqrt(norm_var[j]) + 1e-4);
+  return static_cast<float>(fmin(fmax(y, -clip), clip));
+}
+
+}  // namespace trl

@@ -16,26 +16,12 @@
 // are staged in shared memory with flat coalesced loads; A (o x o), B (a x o), c live in
 // shared memory too (49 KB for o=111).  Thread (e, j) produces s'[e][j].  HBM traffic per
 // env-step: read 4(o+a), write 4o + 6 bytes -> HBM/latency-bound, no tensor-core work.
-#include "reduce.cuh"
+#include "env_common.cuh"
 
 namespace trl {
 
 constexpr int kEnvsPerCta = 32;
 constexpr int kEnvThreads = 256;
-
-__host__ __device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
-  return x;
-}
-// U(seed, episode, j): 24 random bits / 2^24 -- exact in fp32 (oracle/synth_env.py:hash_uniform)
-__host__ __device__ __forceinline__ float hash_uniform(uint32_t seed, uint32_t episode, uint32_t j) {
-  const uint32_t key = seed * 0x9E3779B1u + episode * 0x85EBCA77u + j * 0xC2B2AE3Du + 0x27D4EB2Fu;
-  return float(mix32(key) >> 8) * (1.0f / 16777216.0f);
-}
-__host__ __device__ __forceinline__ float reset_value(uint32_t seed, uint32_t episode, uint32_t j, double init_scale) {
-  // INIT_SCALE * (2u - 1) evaluated in fp64 then rounded once, like the float64 oracle cast to fp32
-  return float(init_scale * (2.0 * double(hash_uniform(seed, episode, j)) - 1.0));
-}
 
 struct EnvParams {
   float* __restrict__ state;            // (N,o) in/out: s -> s'
@@ -45,24 +31,9 @@ struct EnvParams {
   const float* __restrict__ c;          // (o)
   const float* __restrict__ lb;         // (a)
   const float* __restrict__ ub;         // (a)
-  int* __restrict__ elapsed;            // (N) env-side step counter (TimeLimit._elapsed_steps)
-  const int* __restrict__ step_count;   // (N) collector-side counter or nullptr
-  float* __restrict__ reward;           // (N)
-  uint8_t* __restrict__ done;           // (N)
-  uint8_t* __restrict__ time_limit;     // (N)
-  double* __restrict__ partial;         // (grid, 2*o) per-CTA column sums / sums of squares, or nullptr
-  double* __restrict__ batch_sums;      // (2*o) reduced sums (written by the last CTA) or nullptr
-  double* __restrict__ norm_mean;       // (o)  running mean   (merged in-kernel if merge != 0)
-  double* __restrict__ norm_var;        // (o)
-  double* __restrict__ norm_count;      // (1)
-  unsigned* __restrict__ ticket;        // (1) zero-initialised
-  int* __restrict__ any_reset;          // (2) double-buffered "some env needs a reset" flag, or nullptr
-  const int* __restrict__ t_ptr;        // (1) device step index (selects the flag slot), or nullptr
-  long long N;
+  EnvStepFields env;                    // D = o
   int o, a;
-  float rho, eta, ctrl_cost, term_thr, reward_scale;
-  int max_episode_steps, max_episode_frames;
-  int merge;                            // 1: Chan-merge batch moments into norm_* in the last CTA
+  float rho, eta, ctrl_cost, term_thr;
 };
 
 // dynamic smem: A[o*o] B[a*o] c[o] lbub[2a] | s[E*o] u[E*a] s2[E*o]
@@ -78,8 +49,9 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
   float* su = ss + E * o;
   float* s2 = su + E * a;
   const int tid = threadIdx.x, nthr = blockDim.x;
+  const EnvStepFields& f = p.env;
   const long long env_base = static_cast<long long>(blockIdx.x) * E;
-  const int ne = static_cast<int>(min(static_cast<long long>(E), p.N - env_base));
+  const int ne = static_cast<int>(min(static_cast<long long>(E), f.N - env_base));
 
   for (int i = tid; i < o * o; i += nthr) sA[i] = p.A[i];
   for (int i = tid; i < a * o; i += nthr) sB[i] = p.B[i];
@@ -111,33 +83,19 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
   float* gout = p.state + env_base * o;
   for (int i = tid; i < ne * o; i += nthr) gout[i] = s2[i];
 
-  int local_reset = 0;
+  bool local_reset = false;
   if (tid < ne) {
-    const long long n = env_base + tid;
     const float* ue = su + tid * a;
     float usq = 0.f;
     for (int k = 0; k < a; ++k) usq = fmaf(ue[k], ue[k], usq);
     const float r = s2[tid * o + 0] - p.ctrl_cost * usq;
-    const int el = p.elapsed[n] + 1;
-    p.elapsed[n] = el;
-    const bool done_dyn = fabsf(s2[tid * o + 1]) > p.term_thr;
-    const bool past = el >= p.max_episode_steps;
-    const bool done = done_dyn || past;
-    p.reward[n] = r * p.reward_scale;
-    p.done[n] = done ? 1 : 0;
-    p.time_limit[n] = (done && el == p.max_episode_steps) ? 1 : 0;
-    const bool surpass = p.step_count ? (p.step_count[n] + 1 >= p.max_episode_frames) : false;
-    local_reset = (done || surpass) ? 1 : 0;
+    local_reset = env_row_end(f, env_base + tid, fabsf(s2[tid * o + 1]) > p.term_thr, r * f.reward_scale);
   }
-  if (p.any_reset) {
-    const int t = p.t_ptr ? *p.t_ptr : 0;
-    if (blockIdx.x == 0 && tid == 0) p.any_reset[(t + 1) & 1] = 0;  // slot of the *next* step
-    if (__syncthreads_or(local_reset) && tid == 0) atomicOr(&p.any_reset[t & 1], 1);
-  }
+  update_any_reset(f, local_reset);
 
-  if (p.partial) {
+  if (f.partial) {
     // per-feature batch moments of this CTA's rows (fp64 accumulation)
-    double* pp = p.partial + static_cast<long long>(blockIdx.x) * 2 * o;
+    double* pp = f.partial + static_cast<long long>(blockIdx.x) * 2 * o;
     for (int j = tid; j < o; j += nthr) {
       double s = 0.0, q = 0.0;
       for (int e = 0; e < ne; ++e) {
@@ -148,7 +106,7 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
       pp[j] = s;
       pp[o + j] = q;
     }
-    if (last_cta(p.ticket, gridDim.x)) {
+    if (last_cta(f.ticket, gridDim.x)) {
       // fold the per-CTA partials with all threads: thread (part, c) sums CTAs b = part, part+P, ... of
       // column c (c < 2*o), then `part` results are combined in fixed order (deterministic); the previous
       // version walked all CTAs serially in `o` threads and dominated the kernel's latency
@@ -159,7 +117,7 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
         const int part = tid / C, c = tid - part * C;
         if (part < P) {
           double acc = 0.0;
-          for (unsigned b = part; b < gridDim.x; b += P) acc += p.partial[static_cast<long long>(b) * C + c];
+          for (unsigned b = part; b < gridDim.x; b += P) acc += f.partial[static_cast<long long>(b) * C + c];
           sred[part * C + c] = acc;
         }
       }
@@ -170,15 +128,13 @@ __global__ void __launch_bounds__(kEnvThreads) synth_env_step_kernel(const EnvPa
           for (int part = 0; part < P; ++part) { s += sred[part * C + j]; q += sred[part * C + o + j]; }
         } else {
           for (unsigned b = 0; b < gridDim.x; ++b) {
-            s += p.partial[static_cast<long long>(b) * C + j];
-            q += p.partial[static_cast<long long>(b) * C + o + j];
+            s += f.partial[static_cast<long long>(b) * C + j];
+            q += f.partial[static_cast<long long>(b) * C + o + j];
           }
         }
-        if (p.batch_sums) { p.batch_sums[j] = s; p.batch_sums[o + j] = q; }
-        if (p.merge) chan_merge(s, q, static_cast<double>(p.N), *p.norm_count, p.norm_mean[j], p.norm_var[j]);
+        merge_feature(f, o, j, s, q);
       }
-      __syncthreads();   // every thread has read *norm_count
-      if (tid == 0 && p.merge) *p.norm_count = *p.norm_count + static_cast<double>(p.N);
+      merge_count(f);
     }
   }
 }
@@ -248,12 +204,11 @@ TRL_API int trl_synth_env_step(float* state, const float* actions, const float* 
   if (N == 0) return TRL_OK;
   TRL_REQUIRE(state && actions && A && B && c && lb && ub && elapsed && reward && done && time_limit,
               "trl_synth_env_step: null pointer");
-  TRL_REQUIRE(!partial || ticket, "trl_synth_env_step: statistics requested without a ticket counter");
-  TRL_REQUIRE(!(merge_stats && partial) || (norm_mean && norm_var && norm_count),
-              "trl_synth_env_step: merge_stats needs norm_mean/var/count");
-  EnvParams p{state, actions, A, B, c, lb, ub, elapsed, step_count, reward, done, time_limit, partial, batch_sums,
-              norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, obs_dim, act_dim, rho, eta, ctrl_cost,
-              term_thr, reward_scale, max_episode_steps, max_episode_frames, merge_stats};
+  EnvParams p{state, actions, A, B, c, lb, ub,
+              {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean, norm_var, norm_count,
+               ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps, max_episode_frames, merge_stats},
+              obs_dim, act_dim, rho, eta, ctrl_cost, term_thr};
+  if (const int e = check_env_step("trl_synth_env_step", p.env)) return e;
   const double smem_bytes = synth_env_smem(obs_dim, act_dim);
   TRL_REQUIRE(smem_bytes <= 227 * 1024, "trl_synth_env_step: obs_dim %d act_dim %d need %.0f B of shared memory "
               "(> 227 KB)", obs_dim, act_dim, smem_bytes);

@@ -16,12 +16,11 @@
 //
 // Layout: phys (N,2) fp64, obs (N,3) fp32 raw observation; one thread per env, kPendThreads envs per CTA.  The reset
 // has its own kernel because the observation is not the state: collect_finalize's in-kernel reset cannot serve it.
-#include "reduce.cuh"
+#include "env_common.cuh"
 
 namespace trl {
 
 constexpr int kPendThreads = 256;
-constexpr int kPendWarps = kPendThreads / 32;
 
 // gym's PendulumEnv constants (classic_control/pendulum.py)
 constexpr double kPendG = 10.0;
@@ -34,13 +33,6 @@ constexpr double kPi = 3.141592653589793;
 constexpr double kTwoPi = 2.0 * 3.141592653589793;
 constexpr double kGravTerm = 3.0 * kPendG / (2.0 * kPendL);            // 15.0, exact
 constexpr double kTorqueTerm = 3.0 / (kPendM * kPendL * kPendL);       // 3.0, exact
-
-// U(seed, episode, j): the synthetic envs' 24-bit counter hash (oracle/synth_env.py:hash_uniform), exact in fp32/fp64
-__device__ __forceinline__ double pend_hash_uniform(uint32_t seed, uint32_t episode, uint32_t j) {
-  uint32_t x = seed * 0x9E3779B1u + episode * 0x85EBCA77u + j * 0xC2B2AE3Du + 0x27D4EB2Fu;
-  x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
-  return static_cast<double>(static_cast<float>(x >> 8) * (1.0f / 16777216.0f));
-}
 
 // NormAct (continuous_wrapper.py:18-20) with lb = -2, ub = 2, in fp32: clip(lb + (a + 1) * 0.5 * (ub - lb), lb, ub)
 __device__ __forceinline__ float pend_torque(float a) {
@@ -60,35 +52,16 @@ struct PendulumParams {
   double* __restrict__ phys;            // (N,2) in/out: theta, theta_dot
   float* __restrict__ obs;              // (N,3) out: cos theta, sin theta, theta_dot
   const float* __restrict__ actions;    // (N) policy-space actions, [-1, 1] after NormAct's clip
-  int* __restrict__ elapsed;            // (N) env-side step counter (TimeLimit._elapsed_steps)
-  const int* __restrict__ step_count;   // (N) collector-side counter or nullptr
-  float* __restrict__ reward;           // (N)
-  uint8_t* __restrict__ done;           // (N)
-  uint8_t* __restrict__ time_limit;     // (N)
   int* __restrict__ action_error;       // (1) set to 1 when an action is not finite
-  double* __restrict__ partial;         // (grid, 6) per-CTA column sums / sums of squares, or nullptr
-  double* __restrict__ batch_sums;      // (6) reduced sums (written by the last CTA) or nullptr
-  double* __restrict__ norm_mean;       // (3) running mean   (merged in-kernel if merge != 0)
-  double* __restrict__ norm_var;        // (3)
-  double* __restrict__ norm_count;      // (1)
-  unsigned* __restrict__ ticket;        // (1) zero-initialised
-  int* __restrict__ any_reset;          // (2) double-buffered "some env needs a reset" flag, or nullptr
-  const int* __restrict__ t_ptr;        // (1) device step index (selects the flag slot), or nullptr
-  long long N;
-  float reward_scale;
-  int max_episode_steps, max_episode_frames;
-  int merge;                            // 1: Chan-merge batch moments into norm_* in the last CTA
+  EnvStepFields env;                    // D = 3
 };
 
 __global__ void __launch_bounds__(kPendThreads) pendulum_step_kernel(const PendulumParams p) {
-  __shared__ double sh[kPendWarps][6];
-  __shared__ double sred[6];
-  const int tid = threadIdx.x;
-  const long long n = static_cast<long long>(blockIdx.x) * kPendThreads + tid;
-  const bool live = n < p.N;
+  const EnvStepFields& f = p.env;
+  const long long n = static_cast<long long>(blockIdx.x) * kPendThreads + threadIdx.x;
   float ob[3] = {0.f, 0.f, 0.f};
-  int local_reset = 0;
-  if (live) {
+  bool local_reset = false;
+  if (n < f.N) {
     const double th = p.phys[n * 2], thdot = p.phys[n * 2 + 1];
     const float a = p.actions[n];
     float r = 0.f;
@@ -106,7 +79,7 @@ __global__ void __launch_bounds__(kPendThreads) pendulum_step_kernel(const Pendu
       ob[0] = static_cast<float>(cos(nth));
       ob[1] = static_cast<float>(sin(nth));
       ob[2] = static_cast<float>(nthdot);
-      r = static_cast<float>(__dmul_rn(-cost, static_cast<double>(p.reward_scale)));
+      r = static_cast<float>(__dmul_rn(-cost, static_cast<double>(f.reward_scale)));
     } else {
       // not an action: flag it for the host and leave this env's state and observation where they were
       atomicOr(p.action_error, 1);
@@ -115,55 +88,10 @@ __global__ void __launch_bounds__(kPendThreads) pendulum_step_kernel(const Pendu
     }
 #pragma unroll
     for (int j = 0; j < 3; ++j) p.obs[n * 3 + j] = ob[j];
-    const int el = p.elapsed[n] + 1;
-    p.elapsed[n] = el;
-    const bool done = el >= p.max_episode_steps;      // no terminal state: only the time limit ends an episode
-    p.reward[n] = r;
-    p.done[n] = done ? 1 : 0;
-    p.time_limit[n] = (done && el == p.max_episode_steps) ? 1 : 0;
-    const bool surpass = p.step_count ? (p.step_count[n] + 1 >= p.max_episode_frames) : false;
-    local_reset = (done || surpass) ? 1 : 0;
+    local_reset = env_row_end(f, n, false, r);       // no terminal state: only the time limit ends an episode
   }
-  if (p.any_reset) {
-    const int t = p.t_ptr ? *p.t_ptr : 0;
-    if (blockIdx.x == 0 && tid == 0) p.any_reset[(t + 1) & 1] = 0;  // slot of the *next* step
-    if (__syncthreads_or(local_reset) && tid == 0) atomicOr(&p.any_reset[t & 1], 1);
-  }
-
-  if (p.partial) {
-    // per-feature batch moments of this CTA's envs: warp shuffles, then thread k folds the warps in order
-    const int lane = tid & 31, wid = tid >> 5;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double x = static_cast<double>(ob[j]);
-      const double ws = warp_sum(x), wq = warp_sum(x * x);
-      if (lane == 0) { sh[wid][j] = ws; sh[wid][3 + j] = wq; }
-    }
-    __syncthreads();
-    if (tid < 6) {
-      double t = 0.0;
-#pragma unroll
-      for (int w = 0; w < kPendWarps; ++w) t += sh[w][tid];
-      p.partial[static_cast<long long>(blockIdx.x) * 6 + tid] = t;
-    }
-    if (last_cta(p.ticket, gridDim.x)) {
-      // warp k folds quantity k over the CTAs: lanes stride over CTAs, then one shuffle reduction (fixed order)
-      if (wid < 6) {
-        double acc = 0.0;
-        for (unsigned b = lane; b < gridDim.x; b += 32) acc += __ldcg(p.partial + static_cast<long long>(b) * 6 + wid);
-        acc = warp_sum(acc);
-        if (lane == 0) sred[wid] = acc;
-      }
-      __syncthreads();
-      if (tid < 3) {
-        const double s = sred[tid], q = sred[3 + tid];
-        if (p.batch_sums) { p.batch_sums[tid] = s; p.batch_sums[3 + tid] = q; }
-        if (p.merge) chan_merge(s, q, static_cast<double>(p.N), *p.norm_count, p.norm_mean[tid], p.norm_var[tid]);
-      }
-      __syncthreads();   // every thread has read *norm_count
-      if (tid == 0 && p.merge) *p.norm_count = *p.norm_count + static_cast<double>(p.N);
-    }
-  }
+  update_any_reset(f, local_reset);
+  if (f.partial) env_moments<3, kPendThreads>(f, ob);
 }
 
 struct PendulumResetParams {
@@ -194,8 +122,8 @@ __global__ void __launch_bounds__(kPendThreads) pendulum_reset_kernel(const Pend
   if (sel) {
     // theta ~ U(-pi, pi), theta_dot ~ U(-1, 1) from the counter hash of (seed, episode, component)
     const unsigned seed = p.seeds[n], ep = p.episode[n];
-    const double th = __dmul_rn(kPi, __dadd_rn(__dmul_rn(2.0, pend_hash_uniform(seed, ep, 0)), -1.0));
-    const double thdot = __dadd_rn(__dmul_rn(2.0, pend_hash_uniform(seed, ep, 1)), -1.0);
+    const double th = __dmul_rn(kPi, __dadd_rn(__dmul_rn(2.0, double(counter_uniform(seed, ep, 0))), -1.0));
+    const double thdot = __dadd_rn(__dmul_rn(2.0, double(counter_uniform(seed, ep, 1))), -1.0);
     p.phys[n * 2] = th;
     p.phys[n * 2 + 1] = thdot;
     raw[0] = static_cast<float>(cos(th));
@@ -213,16 +141,8 @@ __global__ void __launch_bounds__(kPendThreads) pendulum_reset_kernel(const Pend
   const bool all_raw = !p.norm_mean || (p.raw_obs_after_reset && p.any_reset[*p.t_ptr & 1]);
 #pragma unroll
   for (int j = 0; j < 3; ++j) {
-    float ob;
-    if (all_raw) {
-      ob = raw[j];
-    } else if (sel) {
-      const double y = (static_cast<double>(raw[j]) - p.norm_mean[j]) / (sqrt(p.norm_var[j]) + 1e-4);
-      ob = static_cast<float>(fmin(fmax(y, -p.clip), p.clip));
-    } else {
-      ob = p.next_norm[n * 3 + j];
-    }
-    p.cur_ob[n * 3 + j] = ob;
+    p.cur_ob[n * 3 + j] =
+        next_observation(all_raw, sel, raw[j], p.next_norm + n * 3 + j, p.norm_mean, p.norm_var, j, p.clip);
   }
 }
 
@@ -243,13 +163,10 @@ TRL_API int trl_pendulum_step(double* phys, float* obs, const float* actions, in
   if (N == 0) return TRL_OK;
   TRL_REQUIRE(phys && obs && actions && elapsed && reward && done && time_limit && action_error,
               "trl_pendulum_step: null pointer");
-  TRL_REQUIRE(!partial || ticket, "trl_pendulum_step: statistics requested without a ticket counter");
-  TRL_REQUIRE(!(merge_stats && partial) || (norm_mean && norm_var && norm_count),
-              "trl_pendulum_step: merge_stats needs norm_mean/var/count");
-  TRL_REQUIRE(!t_ptr || any_reset, "trl_pendulum_step: t_ptr given without the any_reset flag");
-  PendulumParams p{phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error, partial,
-                   batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, reward_scale,
-                   max_episode_steps, max_episode_frames, merge_stats};
+  PendulumParams p{phys, obs, actions, action_error,
+                   {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean, norm_var, norm_count,
+                    ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps, max_episode_frames, merge_stats}};
+  if (const int e = check_env_step("trl_pendulum_step", p.env)) return e;
   pendulum_step_kernel<<<trl_pendulum_num_ctas(N), kPendThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("pendulum_step_kernel");
 }

@@ -1,4 +1,5 @@
-"""Device-resident vectorised synthetic env with the reference's vec-env API.
+"""Device-resident vectorised envs with the reference's vec-env API: `DeviceVecEnv`, the base of the state-vector
+device envs (synthetic, CartPole, Pendulum), and the synthetic env itself.
 
 Stands where ``NormObs(VecEnv(...))`` / ``NormObs(SubProcVecEnv(...))`` stand in the reference
 (/root/reference/torchrl/env/get_env.py:70-87): same methods and attributes
@@ -80,44 +81,39 @@ class DeviceNormalizer:
         return new
 
 
-class SynthVecEnv:
-    """N synthetic envs on one GPU.
+class DeviceVecEnv:
+    """What the state-vector device envs share: N envs whose raw observation is the fp32 `state` (N, obs_dim), stepped
+    by one kernel launch that also keeps the TimeLimit counters, the collector's reset flag and NormObs's batch moments.
 
     env_param: {"reward_scale": float, "obs_norm": bool} (the reference's "env" config section).
     first_env / total_envs: global index range of this shard (multi-GPU: rank g owns
     [g*N, (g+1)*N) of total_envs; seeds follow VecEnv.seed with the GLOBAL index so the union
     over ranks equals the single-process env set).
+    A subclass sets its spaces and launches its kernels in `_step_kernel` (and `_reset_kernel` unless the default reset
+    below is its own).
     """
 
     # half-width of the uniform reset distribution (the collector's in-kernel partial reset reads it too)
     init_scale = spec.INIT_SCALE
+    # host mirror of `elapsed` valid (read while lockstep; reset() restores it, partial_reset() invalidates it)
+    _host_mirror_ok = True
+    # check_actions' message (%s: env_id) for an env whose kernel flags the actions it refuses in `action_error`
+    action_error_msg = None
 
-    def __init__(self, env_id, env_nums, env_param=None, device="cuda", first_env=0, total_envs=None,
-                 max_episode_steps=spec.MAX_EPISODE_STEPS):
+    def __init__(self, env_id, env_nums, env_param, device, first_env, total_envs, max_episode_steps, obs_dim, act_dim,
+                 num_ctas):
         env_param = dict(env_param or {})
         self.env_id = env_id
         self.env_nums = int(env_nums)
         self.device = torch.device(device)
-        self.obs_dim, self.act_dim, self.term_thr = spec.SPECS[env_id]
+        self.obs_dim, self.act_dim = obs_dim, act_dim
         self.first_env = int(first_env)
         self.total_envs = int(total_envs) if total_envs is not None else self.env_nums
         self._max_episode_steps = int(max_episode_steps)
         self._reward_scale = env_param.get("reward_scale", 1)
         self.obs_norm = bool(env_param.get("obs_norm", False))
         self.training = True
-        hi = np.full((self.obs_dim,), np.inf)
-        self.observation_space = Box(-hi, hi)
-        ub = np.ones((self.act_dim,))
-        self.action_space = Box(-ub, ub)
-        # True when episode boundaries are a deterministic function of the step count
-        self.lockstep = not np.isfinite(self.term_thr)
-        N, o, a, dev = self.env_nums, self.obs_dim, self.act_dim, self.device
-        A, B, c = spec.make_params(o, a)
-        self.A = torch.from_numpy(A).to(dev)
-        self.B = torch.from_numpy(B).to(dev)
-        self.c = torch.from_numpy(c).to(dev)
-        self.lb = torch.full((a,), -1.0, dtype=F32, device=dev)
-        self.ub = torch.full((a,), 1.0, dtype=F32, device=dev)
+        N, o, dev = self.env_nums, obs_dim, self.device
         self.state = torch.zeros(N, o, dtype=F32, device=dev)       # raw observation
         self.elapsed = torch.zeros(N, dtype=I32, device=dev)
         self.episode = torch.zeros(N, dtype=I32, device=dev)
@@ -125,16 +121,16 @@ class SynthVecEnv:
         self.reward = torch.zeros(N, dtype=F32, device=dev)
         self.done = torch.zeros(N, dtype=U8, device=dev)
         self.time_limit = torch.zeros(N, dtype=U8, device=dev)
+        if self.action_error_msg is not None:
+            self.action_error = torch.zeros(1, dtype=I32, device=dev)
         self.obs_out = torch.zeros(N, o, dtype=F32, device=dev)     # what step() returns (normalised if obs_norm)
-        self._nblk = ops.synth_env_num_ctas(N)
-        self._partial = torch.zeros(self._nblk, 2 * o, dtype=F64, device=dev)
+        self._partial = torch.zeros(num_ctas, 2 * o, dtype=F64, device=dev)
         self.batch_sums = torch.zeros(2 * o, dtype=F64, device=dev)
         self._ticket = torch.zeros(1, dtype=I32, device=dev)
         self.any_reset = torch.zeros(2, dtype=I32, device=dev)
         self._obs_normalizer = DeviceNormalizer((o,), device=dev) if self.obs_norm else None
         self._obs = None
-        self._host_elapsed = 0          # host mirror of `elapsed` (valid while lockstep and unperturbed)
-        self._host_mirror_ok = True
+        self._host_elapsed = 0
         # stats merge happens in-kernel; with a DataParallelContext the batch sums are all-reduced
         # over ranks first and merged by a separate launch (global statistics, SURVEY.md 8(e))
         self._dist = None
@@ -180,6 +176,7 @@ class SynthVecEnv:
         ops.synth_env_seed(self.seeds, self.episode, seed, self.total_envs, self.first_env)
 
     def _reset_kernel(self, mask):
+        """Every state component from U(-init_scale, init_scale) by the counter hash, as collect_finalize resets."""
         ops.synth_env_reset(self.state, self.elapsed, self.episode, self.seeds, mask, self.init_scale)
 
     def _observe(self, update):
@@ -213,31 +210,37 @@ class SynthVecEnv:
         return self.state
 
     def launch_step(self, actions, step_count=None, max_episode_frames=0, t_ptr=None):
-        """Advance all envs one step: state/reward/done/time_limit staging buffers are updated and
-        `obs_out` receives what env.step would return.  No host sync."""
-        update = self.obs_norm and self.training and self._obs_normalizer.should_estimate
+        """Advance all envs one step: the staging buffers (state, reward, done, time_limit) are updated and, with
+        obs_norm, `obs_out` receives what env.step would return.  No host sync; an action the kernel refuses is
+        reported by `check_actions`."""
         nrm = self._obs_normalizer
+        update = self.obs_norm and self.training and nrm.should_estimate
         distributed = self.dist is not None and self.dist.active
-        rs = float(self._reward_scale) if self.training else 1.0
         moments = (self._partial, self.batch_sums, nrm._mean, nrm._var, nrm._count) if update else (None,) * 5
-        ops.synth_env_step(self.state, actions, self.A, self.B, self.c, self.lb, self.ub, self.elapsed, step_count,
-                           self.reward, self.done, self.time_limit, *moments, self._ticket, self.any_reset, t_ptr,
-                           spec.RHO, spec.ETA, spec.CTRL_COST,
-                           float(self.term_thr) if np.isfinite(self.term_thr) else 3.0e38, rs, self._max_episode_steps,
-                           int(max_episode_frames) if step_count is not None else (1 << 30),
-                           update and not distributed)
+        self._step_kernel(actions, step_count, moments, t_ptr, float(self._reward_scale) if self.training else 1.0,
+                          int(max_episode_frames) if step_count is not None else (1 << 30), update and not distributed)
         if update and distributed:
             ops.obs_norm_merge(self._reduce_sums(), self.total_envs, nrm._mean, nrm._var, nrm._count)
         if self.obs_norm:
             ops.obs_norm_filt(self.state, nrm._mean, nrm._var, nrm.clip, self.obs_out)
         return self.obs_out
 
+    def check_actions(self):
+        """Raise if any step since the last check received an action the kernel refuses (one host sync, none for an
+        env whose kernel accepts every action)."""
+        if self.action_error_msg is not None and int(self.action_error.item()) != 0:
+            self.action_error.zero_()
+            raise ValueError(self.action_error_msg % self.env_id)
+
     def step(self, actions):
         """obs (N,o), reward (N,1), done (N,1) bool, {'time_limit': (N,) bool} -- device tensors."""
-        actions = torch.as_tensor(actions, dtype=F32, device=self.device).reshape(self.env_nums, self.act_dim).contiguous()
-        self.launch_step(actions)
+        actions = torch.as_tensor(actions, dtype=F32, device=self.device).reshape(-1)
+        if actions.numel() != self.env_nums * self.act_dim:
+            raise ValueError("%s.step: %d actions for %d envs" % (self.env_id, actions.numel(), self.env_nums))
+        self.launch_step(actions.reshape(self.env_nums, self.act_dim).contiguous())
         if not self.obs_norm:
             self.obs_out.copy_(self.state)
+        self.check_actions()
         infos = {"time_limit": self.time_limit.bool()}
         return self.obs_out, self.reward.unsqueeze(-1), self.done.bool().unsqueeze(-1), infos
 
@@ -251,3 +254,32 @@ class SynthVecEnv:
             else:
                 new.__dict__[k] = copy.deepcopy(v, memo)
         return new
+
+
+class SynthVecEnv(DeviceVecEnv):
+    """N synthetic envs on one GPU: s' = rho * s + eta * tanh(s A + NormAct(u) B + c) (csrc/env_step.cu)."""
+
+    def __init__(self, env_id, env_nums, env_param=None, device="cuda", first_env=0, total_envs=None,
+                 max_episode_steps=spec.MAX_EPISODE_STEPS):
+        o, a, self.term_thr = spec.SPECS[env_id]
+        super().__init__(env_id, env_nums, env_param, device, first_env, total_envs, max_episode_steps, o, a,
+                         ops.synth_env_num_ctas(int(env_nums)))
+        hi = np.full((o,), np.inf)
+        self.observation_space = Box(-hi, hi)
+        ub = np.ones((a,))
+        self.action_space = Box(-ub, ub)
+        # True when episode boundaries are a deterministic function of the step count
+        self.lockstep = not np.isfinite(self.term_thr)
+        A, B, c = spec.make_params(o, a)
+        self.A = torch.from_numpy(A).to(self.device)
+        self.B = torch.from_numpy(B).to(self.device)
+        self.c = torch.from_numpy(c).to(self.device)
+        self.lb = torch.full((a,), -1.0, dtype=F32, device=self.device)
+        self.ub = torch.full((a,), 1.0, dtype=F32, device=self.device)
+
+    def _step_kernel(self, actions, step_count, moments, t_ptr, reward_scale, max_episode_frames, merge):
+        ops.synth_env_step(self.state, actions, self.A, self.B, self.c, self.lb, self.ub, self.elapsed, step_count,
+                           self.reward, self.done, self.time_limit, *moments, self._ticket, self.any_reset, t_ptr,
+                           spec.RHO, spec.ETA, spec.CTRL_COST,
+                           float(self.term_thr) if np.isfinite(self.term_thr) else 3.0e38, reward_scale,
+                           self._max_episode_steps, max_episode_frames, merge)
