@@ -246,6 +246,12 @@ int trl_sac_v_loss(const float* logp, const float* qn1, const float* qn2, const 
 /* MSE of one or two critics against the same target (twin_sac_q.py:142-143, td3.py:96-97) */
 int trl_twin_mse_loss(const float* q1, const float* q2, const float* y, int64_t B, float* g1, float* g2,
                       float* info2, double* scratch, unsigned* ticket, void* stream);
+/* The same with importance weights (prioritised replay; no reference counterpart): loss_k = mean_b w_b (q_k - y)^2,
+ * g_k = ((2 (q_k - y)) w_b) / B, td_out (B, 1 or 2 critics) = the unweighted |q_k - y|.  weights and td_out may be
+ * NULL; weights NULL gives trl_twin_mse_loss's bits. */
+int trl_twin_mse_loss_weighted(const float* q1, const float* q2, const float* y, const float* weights, int64_t B,
+                               float* g1, float* g2, float* td_out, float* info2, double* scratch, unsigned* ticket,
+                               void* stream);
 /* fused QR-DQN / DQN loss incl. greedy target selection; info3 = [loss, mean q_s_a, mean reward] */
 int trl_qr_dqn_loss(const float* pred, const float* next, const float* actions, const float* rewards,
                     const uint8_t* terminals, const float* weights, int B, int n_actions, int n_quantiles,
@@ -286,6 +292,14 @@ int trl_split_tf32(const float* x, int64_t n, float* hi, float* lo, void* stream
  * oracle/ref_numpy.py:per_sample/per_update.  u: device doubles in [0,1) (host np.random for parity). */
 int trl_per_sample(const float* prio, int size, const double* u, int b, float beta, int64_t* idx,
                    float* weights, void* stream);
+/* The same draw for rings of up to 2^24 rows, graph-safe: the live size is *size_ptr (clamped to 1..capacity) and
+ * the uniforms are u[*pos_ptr * b ..][0..b), both read on the device.  Two launches (a scan per chunk of 4096 rows,
+ * then one CTA over the chunk totals and the draws); for *size_ptr <= 4096 the bits are trl_per_sample's.
+ * scratch: trl_per_scratch_doubles(capacity) doubles (-1: capacity not in 1..2^24). */
+int trl_per_scratch_doubles(int capacity);
+int trl_per_sample_rows(const float* prio, int capacity, const int* size_ptr, const double* u, const int* pos_ptr,
+                        int b, float beta, int64_t* idx, float* weights, double* scratch, void* stream);
+/* prio[idx_k] = (mean_n |td[k][n]| + eps)^alpha; a row drawn twice keeps its last draw's value (batch order) */
 int trl_per_update(float* prio, const int64_t* idx, const float* td, int b, int n, float alpha, float eps,
                    float* max_prio, void* stream);
 int trl_per_insert(float* prio, const int* row_ptr, const float* max_prio, void* stream);

@@ -73,6 +73,8 @@ SIGNATURES = {
     "trl_split_tf32": [vp, i64, vp, vp, vp],
     "trl_bias_act_bwd": [vp, vp, vp, vp, i64, i32, i32, vp, vp, vp],
     "trl_per_sample": [vp, i32, vp, i32, f32, vp, vp, vp],
+    "trl_per_scratch_doubles": [i32],
+    "trl_per_sample_rows": [vp, i32, vp, vp, vp, i32, f32, vp, vp, vp, vp],
     "trl_per_update": [vp, vp, vp, i32, i32, f32, f32, vp, vp],
     "trl_per_insert": [vp, vp, vp, vp],
     "trl_gemm_tf32x3_nt": [vp, vp, vp, i64, i64, i32, vp, vp, i32, vp],
@@ -126,6 +128,7 @@ SIGNATURES = {
     "trl_sac_policy_loss": [vp, vp, vp, vp, f32, i64, vp, vp, vp, vp, vp, vp, vp],
     "trl_sac_v_loss": [vp, vp, vp, vp, vp, f32, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp],
     "trl_twin_mse_loss": [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp],
+    "trl_twin_mse_loss_weighted": [vp, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp],
     "trl_qr_dqn_loss": [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
     "trl_bootstrapped_dqn_loss": [vp, vp, vp, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp],
     "trl_bootstrapped_act": [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, vp, i64, i32, i32, f32, vp],
@@ -141,7 +144,7 @@ _VALUE_FUNCS = ("trl_abi_version", "trl_synth_env_smem_bytes", "trl_synth_env_nu
                 "trl_pendulum_num_ctas", "trl_comm_flag_bytes",
                 "trl_comm_ipc_handle_bytes", "trl_comm_scratch_doubles", "trl_comm_ll_recv_bytes",
                 "trl_ppo_actor_scratch_doubles", "trl_ppo_categorical_actor_scratch_doubles", "trl_vmpo_categorical_scratch_doubles",
-                "trl_grad_sumsq_blocks")
+                "trl_grad_sumsq_blocks", "trl_per_scratch_doubles")
 
 _lib = None
 

@@ -48,7 +48,7 @@ class DDPG(OffRLAlgo):
         seed = torch.full_like(q_new, -1.0 / q_new.numel())
         torch.autograd.backward([q_new], [seed], inputs=self.opt.segments[0])
         q_pred = self.qf([obs, acts])
-        g, _, _ = ops.twin_mse_loss(q_pred.reshape(-1), None, y, sc, info=info[4:6])
+        g, _, _ = self._critic_loss(batch, q_pred.reshape(-1), None, y, info[4:6])
         torch.autograd.backward([q_pred], [g.reshape(q_pred.shape)], inputs=self.opt.segments[1])
         self._optimizer_step(0b11)
         self._update_target_networks()

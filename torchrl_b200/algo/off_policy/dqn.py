@@ -47,7 +47,6 @@ class DQN(OffRLAlgo):
         batch = self._batch()
         info = ub["info"][0]
         obs, next_obs = self._prep_obs(batch["obs"]), self._prep_obs(batch["next_obs"])
-        B = obs.shape[0]
         acts = batch["acts"].reshape(-1).float()
         rewards, terminals = batch["rewards"].reshape(-1), batch["terminals"].reshape(-1)
         q_pred = self.qf(obs)
@@ -56,11 +55,11 @@ class DQN(OffRLAlgo):
         A = q_pred.shape[-1] // self.quantile_num
         pred = q_pred if q_pred.is_contiguous() else q_pred.contiguous()
         weights = batch.get("weights")                 # prioritised replay: importance weights, TD magnitudes out
-        self._td = torch.empty(B, dtype=torch.float32, device=obs.device) if weights is not None else None
+        td = self._td if weights is not None and self._explicit_batch is None else None
         grad, _ = ops.qr_dqn_loss(pred, next_q, acts.contiguous(), rewards, terminals, self.discount, ub["scratch"],
                                   A, self.quantile_num, mse=self._mse, info=info[0:3],
                                   weights=None if weights is None else weights.reshape(-1).contiguous(),
-                                  td_out=self._td)
+                                  td_out=td)
         torch.autograd.backward([pred], [grad])
         self._optimizer_step()
         self._update_target_networks()

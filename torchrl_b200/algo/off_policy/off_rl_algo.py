@@ -6,6 +6,11 @@ with the reference's own np.random.randint calls (same global RNG stream, bit-ex
 uploaded once, and one captured CUDA graph of {gather, update} is replayed opt_times times reading
 its position from a device counter.  Logged scalars accumulate in a device log and are fetched
 once per epoch (the reference syncs ~20 times per update).
+
+Prioritised replay (no reference counterpart) has the same structure: the uniforms of ALL opt_times draws come from
+one np.random.rand(opt_times * b) (the stream of opt_times calls of rand(b)) and are uploaded once; each update
+{draw rows by priority at the device position, gather, weighted update, write the rows' new priorities, log row} is
+one captured graph per variant.  Only the critics' TD losses are importance weighted (DESIGN.md deviation 24).
 """
 import time
 
@@ -19,6 +24,7 @@ from ..rl_algo import RLAlgo
 
 class OffRLAlgo(RLAlgo):
     INFO_SLOTS = 64
+    TD_COLUMNS = 1               # critics whose |TD| per sample the loss writes for the new priorities
 
     def __init__(self, pretrain_epochs=0, min_pool=0, target_hard_update_period=1000, use_soft_update=True,
                  tau=0.001, opt_times=1, **kwargs):
@@ -34,6 +40,7 @@ class OffRLAlgo(RLAlgo):
         self._graphs = {}
         self._eager_runs = {}
         self._last_infos = []
+        self._td = None              # prioritised replay: (B, TD_COLUMNS) |TD| of the last update, inside self._ub
 
     # ------------------------------------------------------------------ device update loop
     def _ub_setup(self):
@@ -54,17 +61,51 @@ class OffRLAlgo(RLAlgo):
             "scratch": ops.OffPolicyScratch(b * N, dev),
         }
         self._ub["log_plan"] = ops.RowCopyPlan([self._ub["info"]], [self._ub["log32"]], [self.INFO_SLOTS * 4])
-        return self._ub
+        ub = self._ub
+        ub["per"] = hasattr(rb, "update_priorities")
+        if ub["per"]:
+            ub.update({
+                "u": torch.zeros(U * b, dtype=torch.float64, device=dev),
+                "u_host": torch.zeros(U * b, dtype=torch.float64).pin_memory(),
+                "size": torch.zeros(1, dtype=torch.int32, device=dev),
+                "rows": torch.zeros(b, dtype=torch.int64, device=dev),
+                "w": torch.zeros(b, dtype=torch.float32, device=dev),
+                "w_samples": torch.zeros(b * N, 1, dtype=torch.float32, device=dev),
+                "td": torch.zeros((b * N,) if self.TD_COLUMNS == 1 else (b * N, self.TD_COLUMNS), dtype=torch.float32,
+                                  device=dev),
+            })
+            self._td = ub["td"]
+        return ub
 
     def _gather(self):
         ub = self._ub
-        return self.replay_buffer.gather_rows(ub["idx"], self.sample_key, pos_ptr=ub["upd"], rows=ub["b"])
+        rb = self.replay_buffer
+        if not ub["per"]:
+            return rb.gather_rows(ub["idx"], self.sample_key, pos_ptr=ub["upd"], rows=ub["b"])
+        rb.sample_rows(ub["u"], ub["upd"], ub["size"], ub["rows"], ub["w"])
+        batch = dict(rb.gather_rows(ub["rows"], self.sample_key))
+        ub["w_samples"].view(ub["b"], -1).copy_(ub["w"].view(-1, 1).expand(ub["b"], rb.env_nums))
+        batch["weights"] = ub["w_samples"]
+        return batch
+
+    def _critic_loss(self, batch, q1, q2, y, info):
+        """MSE of one or two critics against y: importance weighted when the batch carries prioritised-replay
+        weights, with the unweighted |q - y| of drawn rows into self._td for their new priorities."""
+        sc = self._ub["scratch"]
+        weights = batch.get("weights")
+        if weights is None:
+            return ops.twin_mse_loss(q1, q2, y, sc, info=info)
+        td = self._td if self._explicit_batch is None else None
+        return ops.twin_mse_loss_weighted(q1, q2, y, weights.reshape(-1), sc, info=info, td_out=td)
 
     def _finish_update(self):
-        """Log row of a gathered update, then upd += 1 (an explicit batch's info row is read directly)."""
+        """New priorities of the drawn rows (prioritised replay), log row of a gathered update, then upd += 1 (an
+        explicit batch's info row is read directly)."""
         if self._explicit_batch is not None:
             return
         ub = self._ub
+        if ub["per"]:
+            self.replay_buffer.update_priorities(ub["rows"], self._td)
         ops.ring_write_advance(ub["log_plan"], ub["upd"], ub["U"], ub["log_ticket"])     # log row, then upd += 1
 
     def _variant(self):
@@ -108,34 +149,26 @@ class OffRLAlgo(RLAlgo):
         self._maybe_hard_update()
         return v
 
-    def _update_per_epoch_prioritized(self, flush_infos):
-        """Prioritised replay (no reference counterpart): per update draw rows proportionally to their
-        priority, weight the loss by the importance weights and write the new |TD| priorities back.
-        Round 1: eager launches (the sampler consumes host uniforms per update)."""
-        rb = self.replay_buffer
-        infos = []
-        for _ in range(self.opt_times):
-            batch = rb.random_batch(self.batch_size, self.sample_key)
-            variant = self._explicit_update(batch)
-            td = getattr(self, "_td", None)
-            if td is not None:
-                rb.update_priorities(batch["indices"], td)
-            if flush_infos:
-                infos.append(self._decode_info(self._ub["info"][0].cpu().numpy(), variant))
-        if flush_infos:
-            self._record_infos(infos)
-
     @fused.presplit_scope
     def update_per_epoch(self, flush_infos=True):
         """opt_times x {random_batch; update} (off_rl_algo.py:46-51)."""
         ub = self._ub or self._ub_setup()
-        if hasattr(self.replay_buffer, "update_priorities"):
-            return self._update_per_epoch_prioritized(flush_infos)
         size = self.replay_buffer.num_steps_can_sample()
-        for u in range(ub["U"]):
-            idx = np.random.randint(0, size, ub["b"])           # one draw per update, like random_batch
-            ub["idx_host"][u * ub["b"]:(u + 1) * ub["b"]].copy_(torch.from_numpy(idx.astype(np.int64)))
-        ub["idx"].copy_(ub["idx_host"], non_blocking=True)
+        staged = ub.get("staged")
+        if staged is not None:
+            staged.synchronize()          # the last epoch's upload has left the pinned buffer we are about to refill
+        if ub["per"]:
+            # the uniforms of every draw at once: rand(U * b) is the stream of U calls of rand(b)
+            ub["u_host"].copy_(torch.from_numpy(np.random.rand(ub["U"] * ub["b"])))
+            ub["u"].copy_(ub["u_host"], non_blocking=True)
+            ub["size"].fill_(size)
+        else:
+            for u in range(ub["U"]):
+                idx = np.random.randint(0, size, ub["b"])           # one draw per update, like random_batch
+                ub["idx_host"][u * ub["b"]:(u + 1) * ub["b"]].copy_(torch.from_numpy(idx.astype(np.int64)))
+            ub["idx"].copy_(ub["idx_host"], non_blocking=True)
+        ub["staged"] = torch.cuda.Event()
+        ub["staged"].record()
         ub["upd"].zero_()
         variants = [self._run_update() for _ in range(ub["U"])]
         if flush_infos:
@@ -148,7 +181,7 @@ class OffRLAlgo(RLAlgo):
         dev = self.device
         ub = self._ub or self._ub_setup()
         conv = {}
-        for k in self.sample_key:
+        for k in self.sample_key + (["weights"] if "weights" in batch else []):   # weights: prioritised replay
             v = batch[k]
             v = torch.as_tensor(np.asarray(v)) if not torch.is_tensor(v) else v
             dt = torch.uint8 if k in ("terminals", "masks") else torch.float32   # masks: Bootstrapped DQN

@@ -68,7 +68,7 @@ class SAC(SoftActorCritic):
         with torch.no_grad():
             y, _ = ops.td_target(rewards, terminals, target_v, None, None, None, self.discount, sc, info=info[0:1])
         q2_pred = q_preds[1].reshape(-1) if len(q_preds) > 1 else None
-        g1, g2, _ = ops.twin_mse_loss(q_preds[0].reshape(-1), q2_pred, y, sc, info=info[4:6])
+        g1, g2, _ = self._critic_loss(batch, q_preds[0].reshape(-1), q2_pred, y, info[4:6])
         qns = [qf([obs, new_actions]) for qf in self._critics]
         qn2 = qns[1].reshape(-1) if len(qns) > 1 else None
         g_lp, g_qn1, g_qn2, g_v, _ = ops.sac_v_loss(log_probs.reshape(-1), qns[0].reshape(-1), qn2,

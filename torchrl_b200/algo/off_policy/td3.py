@@ -18,6 +18,8 @@ from .off_rl_algo import OffRLAlgo
 
 
 class TD3(OffRLAlgo):
+    TD_COLUMNS = 2
+
     def __init__(self, pf, qf1, qf2, plr, qlr, optimizer_class=optim.Adam, policy_update_delay=2,
                  norm_std_policy=0.2, noise_clip=0.5, **kwargs):
         super().__init__(**kwargs)
@@ -64,7 +66,7 @@ class TD3(OffRLAlgo):
             y, _ = ops.td_target(rewards, terminals, tq1, tq2, None, None, self.discount, sc, info=info[0:1])
         q1_pred = self.qf1([obs, acts])
         q2_pred = self.qf2([obs, acts])
-        g1, g2, _ = ops.twin_mse_loss(q1_pred.reshape(-1), q2_pred.reshape(-1), y, sc, info=info[4:6])
+        g1, g2, _ = self._critic_loss(batch, q1_pred.reshape(-1), q2_pred.reshape(-1), y, info[4:6])
         torch.autograd.backward([q1_pred, q2_pred], [g1.reshape(q1_pred.shape), g2.reshape(q2_pred.shape)],
                                 inputs=self.opt.segments[1] + self.opt.segments[2])
         self._optimizer_step(0b110)

@@ -9,6 +9,7 @@ from .twin_sac_q import SoftActorCritic
 
 class TwinSAC(SAC):
     _critic_names = ("qf1", "qf2")
+    TD_COLUMNS = 2
 
     def __init__(self, pf, vf, qf1, qf2, plr, vlr, qlr, optimizer_class=optim.Adam, policy_std_reg_weight=1e-3,
                  policy_mean_reg_weight=1e-3, reparameterization=True, automatic_entropy_tuning=True,

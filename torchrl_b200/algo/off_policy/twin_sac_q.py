@@ -106,6 +106,7 @@ class SoftActorCritic(OffRLAlgo):
 
 class TwinSACQ(SoftActorCritic):
     _LOG_PROBS = 21              # sac_policy_loss writes [policy_loss, log_probs stats] at 20..24
+    TD_COLUMNS = 2
 
     def __init__(self, pf, qf1, qf2, plr, qlr, optimizer_class=optim.Adam, policy_std_reg_weight=1e-3,
                  policy_mean_reg_weight=1e-3, reparameterization=True, automatic_entropy_tuning=True,
@@ -142,7 +143,7 @@ class TwinSACQ(SoftActorCritic):
             tq2 = self.target_qf2([next_obs, t_actions]).reshape(-1)
             y, _ = ops.td_target(rewards, terminals, tq1, tq2, t_logp.reshape(-1), log_alpha, self.discount, sc,
                                  info=info[0:1], fixed_alpha=1.0)
-        g1, g2, _ = ops.twin_mse_loss(q1_pred.reshape(-1), q2_pred.reshape(-1), y, sc, info=info[4:6])
+        g1, g2, _ = self._critic_loss(batch, q1_pred.reshape(-1), q2_pred.reshape(-1), y, info[4:6])
         qn1 = self.qf1([obs, new_actions])
         qn2 = self.qf2([obs, new_actions])
         g_lp, g_qn1, g_qn2, _ = ops.sac_policy_loss(log_probs.reshape(-1), qn1.reshape(-1), qn2.reshape(-1),

@@ -282,6 +282,8 @@ __global__ void __launch_bounds__(kOffThreads) sac_v_loss_kernel(const SacVParam
 
 // ---------------------------------------------------------------------------------------------
 // MSE(pred, target) for two critics at once: loss_k = mean((q_k - y)^2), g_k = 2(q_k - y)/B.
+// kWeighted (prioritised replay): loss_k = mean(w_b (q_k - y)^2), g_k = ((2(q_k - y)) w_b) / B, td_out (B, critics) =
+// the unweighted |q_k - y|; weights and td_out may each be null.  w_b = 1 gives the unweighted bits.
 struct TwinMseParams {
   const float* __restrict__ q1;
   const float* __restrict__ q2;   // or nullptr
@@ -292,8 +294,11 @@ struct TwinMseParams {
   double* __restrict__ partial;   // (grid, 2)
   unsigned* __restrict__ ticket;
   long long B;
+  const float* __restrict__ weights;  // (B) importance weights or nullptr (kWeighted only)
+  float* __restrict__ td_out;         // (B, 1 or 2) or nullptr (kWeighted only)
 };
 
+template <bool kWeighted>
 __global__ void __launch_bounds__(kOffThreads) twin_mse_kernel(const TwinMseParams p) {
   __shared__ double shd[32];
   const long long b = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -301,13 +306,17 @@ __global__ void __launch_bounds__(kOffThreads) twin_mse_kernel(const TwinMsePara
   float l1 = 0.f, l2 = 0.f;
   if (b < p.B) {
     const float y = p.y[b];
+    const float w = kWeighted && p.weights ? p.weights[b] : 1.f;
+    const int nc = p.q2 ? 2 : 1;
     const float d1 = p.q1[b] - y;
-    l1 = d1 * d1;
-    p.g1[b] = 2.f * d1 * invB;
+    l1 = kWeighted ? d1 * d1 * w : d1 * d1;
+    p.g1[b] = kWeighted ? 2.f * d1 * w * invB : 2.f * d1 * invB;
+    if (kWeighted && p.td_out) p.td_out[b * nc] = fabsf(d1);
     if (p.q2) {
       const float d2 = p.q2[b] - y;
-      l2 = d2 * d2;
-      p.g2[b] = 2.f * d2 * invB;
+      l2 = kWeighted ? d2 * d2 * w : d2 * d2;
+      p.g2[b] = kWeighted ? 2.f * d2 * w * invB : 2.f * d2 * invB;
+      if (kWeighted && p.td_out) p.td_out[b * nc + 1] = fabsf(d2);
     }
   }
   double r = block_reduce_sum(static_cast<double>(l1), shd);
@@ -509,8 +518,20 @@ TRL_API int trl_twin_mse_loss(const float* q1, const float* q2, const float* y, 
   TRL_REQUIRE(B >= 1, "trl_twin_mse_loss: empty batch");
   TRL_REQUIRE(q1 && y && g1 && info2 && scratch && ticket, "trl_twin_mse_loss: null pointer");
   TRL_REQUIRE(!q2 || g2, "trl_twin_mse_loss: q2 given without g2");
-  TwinMseParams p{q1, q2, y, g1, g2, info2, scratch, ticket, B};
-  twin_mse_kernel<<<off_blocks(B), kOffThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  TwinMseParams p{q1, q2, y, g1, g2, info2, scratch, ticket, B, nullptr, nullptr};
+  twin_mse_kernel<false><<<off_blocks(B), kOffThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch("twin_mse_kernel");
+}
+
+TRL_API int trl_twin_mse_loss_weighted(const float* q1, const float* q2, const float* y, const float* weights, int64_t B,
+                                       float* g1, float* g2, float* td_out, float* info2, double* scratch,
+                                       unsigned* ticket, void* stream) {
+  using namespace trl;
+  TRL_REQUIRE(B >= 1, "trl_twin_mse_loss_weighted: empty batch");
+  TRL_REQUIRE(q1 && y && g1 && info2 && scratch && ticket, "trl_twin_mse_loss_weighted: null pointer");
+  TRL_REQUIRE(!q2 || g2, "trl_twin_mse_loss_weighted: q2 given without g2");
+  TwinMseParams p{q1, q2, y, g1, g2, info2, scratch, ticket, B, weights, td_out};
+  twin_mse_kernel<true><<<off_blocks(B), kOffThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   return check_launch("twin_mse_kernel");
 }
 

@@ -634,6 +634,24 @@ def twin_mse_loss(q1, q2, y, scratch, info=None):
     return g1, g2, info
 
 
+def twin_mse_loss_weighted(q1, q2, y, weights, scratch, info=None, td_out=None):
+    """Importance-weighted MSE of one or two critics against y (prioritised replay): mean(w (q - y)^2) in info[0:2],
+    gradients returned, the unweighted |q - y| in td_out (B, critics) when given.  weights None: twin_mse_loss's bits."""
+    B = q1.numel()
+    g1 = torch.empty_like(q1)
+    g2 = torch.empty_like(q2) if q2 is not None else None
+    if info is None:
+        info = torch.zeros(2, dtype=F32, device=q1.device)
+    if weights is not None and weights.numel() != B:
+        raise ValueError("weights has %d elements for a batch of %d" % (weights.numel(), B))
+    if td_out is not None and td_out.numel() != B * (1 if q2 is None else 2):
+        raise ValueError("td_out has %d elements, want %d" % (td_out.numel(), B * (1 if q2 is None else 2)))
+    _lib.call("trl_twin_mse_loss_weighted", _chk(q1, F32, "q1"), _opt(q2, F32, "q2"), _chk(y, F32, "y"),
+              _opt(weights, F32, "weights"), B, _chk(g1, F32, "g1"), _opt(g2, F32, "g2"), _opt(td_out, F32, "td_out"),
+              _chk(info, F32, "info"), scratch.b(3), scratch.t(3), _stream())
+    return g1, g2, info
+
+
 def qr_dqn_loss(pred, nxt, actions, rewards, terminals, gamma, scratch, n_actions, n_quantiles, mse=False, kappa=1.0,
                 info=None, weights=None, td_out=None):
     """Fused (QR-)DQN loss: quantile-Huber (qrdqn.py:36-60, utils.py:5-13) or squared TD error (dqn.py:53-60);
@@ -698,8 +716,35 @@ def per_sample(prio, size, u, beta, idx=None, weights=None):
     return idx, weights
 
 
+PER_MAX_ROWS = 1 << 24
+
+
+def per_scratch_doubles(capacity):
+    """Scratch doubles per_sample_rows needs for a ring of `capacity` rows."""
+    n = int(_lib.load().trl_per_scratch_doubles(int(capacity)))
+    if n < 0:
+        raise ValueError("a prioritised ring holds 1..%d rows, not %d" % (PER_MAX_ROWS, capacity))
+    return n
+
+
+def per_sample_rows(prio, size_ptr, u, pos_ptr, b, beta, scratch, idx, weights):
+    """per_sample's draw over a ring of prio.numel() <= 2^24 rows with the live size (*size_ptr) and the draw position
+    (uniforms u[*pos_ptr * b:][:b]) on the device, so one captured graph serves every update (two kernels)."""
+    capacity = prio.numel()
+    if scratch.numel() < per_scratch_doubles(capacity):
+        raise ValueError("per_sample_rows: scratch holds %d doubles, want %d" % (scratch.numel(),
+                                                                                 per_scratch_doubles(capacity)))
+    if idx.numel() != b or weights.numel() != b:
+        raise ValueError("per_sample_rows: idx / weights must hold b = %d elements" % b)
+    _lib.call("trl_per_sample_rows", _chk(prio, F32, "prio"), capacity, _chk(size_ptr, I32, "size_ptr"),
+              _chk(u, F64, "u"), _chk(pos_ptr, I32, "pos_ptr"), int(b), float(beta), _chk(idx, I64, "idx"),
+              _chk(weights, F32, "weights"), _chk(scratch, F64, "scratch"), _stream(), kernels=2)
+    return idx, weights
+
+
 def per_update(prio, idx, td, alpha, eps, max_prio):
-    """prio[idx_k] = (mean_n |td[k,n]| + eps)^alpha and running max priority."""
+    """prio[idx_k] = (mean_n |td[k,n]| + eps)^alpha (a row drawn twice: its last draw's value) and running max
+    priority."""
     b = idx.numel()
     n = td.numel() // b
     _lib.call("trl_per_update", _chk(prio, F32, "prio"), _chk(idx, I64, "idx"), _chk(td, F32, "td"), b, n,
