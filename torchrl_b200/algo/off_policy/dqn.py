@@ -6,8 +6,6 @@ TD target, squared-error / quantile-Huber reduction and its gradient -- is ONE k
 (collector/base.py:190-191); the reference's DQN.update itself crashes on that shape
 (dqn.py:54, SURVEY.md A.4) -- the oracle for DQN is the reference expression with acts (B,1).
 """
-import copy
-
 import torch
 import torch.optim as optim
 
@@ -23,12 +21,10 @@ class DQN(OffRLAlgo):
         super().__init__(**kwargs)
         self.pf = pf
         self.qf = qf
-        self.target_qf = copy.deepcopy(qf)
         self.qlr = qlr
-        self.to(self.device)
         # no clipping, whatever grad_clip says: the reference's DQN never clips
-        self._init_optimizer(optimizer_class, [("qf", qf, qlr)], eps=optimizer_info.get("eps", 1e-8), max_norms=[0.0])
-        self._init_targets()
+        self._init_networks(optimizer_class, [("qf", qf, qlr)], eps=optimizer_info.get("eps", 1e-8), max_norms=[0.0],
+                            targets=("qf",))
         self.obs_scale = getattr(self.env, "obs_scale", None)
 
     def _prep_obs(self, x):
@@ -70,16 +66,8 @@ class DQN(OffRLAlgo):
                 'epsilon': float(getattr(self.pf, "epsilon", float("nan"))), 'q_s_a': float(row[1])}
 
     @property
-    def networks(self):
-        return [self.qf, self.target_qf]
-
-    @property
-    def target_networks(self):
-        return [(self.qf, self.target_qf)]
-
-    @property
     def snapshot_networks(self):
-        return [("pf", self.qf)]
+        return [("pf", self.qf)]         # the reference names the Q-network's snapshot files model_pf_*
 
 
 class QRDQN(DQN):

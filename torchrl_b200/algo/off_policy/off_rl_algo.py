@@ -207,6 +207,30 @@ class OffRLAlgo(RLAlgo):
     def _batch(self):
         return self._explicit_batch if self._explicit_batch is not None else self._gather()
 
+    # ------------------------------------------------------------------ pieces of the continuous-control updates
+    def _transitions(self):
+        """The update's batch and its transition fields: obs, acts as (B, -1), next_obs, flat rewards and terminals."""
+        batch = self._batch()
+        obs, acts, next_obs = batch["obs"], batch["acts"], batch["next_obs"]
+        rewards, terminals = batch["rewards"].reshape(-1), batch["terminals"].reshape(-1)
+        return batch, obs, acts.reshape(obs.shape[0], -1), next_obs, rewards, terminals
+
+    def _deterministic_policy_step(self, qf, obs, info):
+        """DDPG's and TD3's policy loss -mean qf(s, pf(s)): its value into info[6], its gradient into the policy
+        segment.  Returns the new actions."""
+        new_actions = self.pf(obs)
+        q_new = qf([obs, new_actions])
+        info[6:7].copy_((-q_new.detach().mean()).reshape(1))
+        seed = torch.full_like(q_new, -1.0 / q_new.numel())
+        torch.autograd.backward([q_new], [seed], inputs=self.opt.segments[0])
+        return new_actions
+
+    def _critic_backward(self, preds, grads, first, last):
+        """Backward from the critics' predictions, seeded with the loss kernel's gradients, into the critic segments
+        first .. last - 1."""
+        torch.autograd.backward(preds, [g.reshape(q.shape) for g, q in zip(grads, preds)],
+                                inputs=[p for seg in self.opt.segments[first:last] for p in seg])
+
     def update_per_timestep(self):
         if self.replay_buffer.num_steps_can_sample() > max(self.min_pool, self.batch_size):
             self.update_per_epoch()

@@ -11,8 +11,6 @@ fused clip+Adam over pf | critics | vf -> Polyak over the flat target V -> log r
 The reference's `assert v_target == v_pred` (sac.py:130, twin_sac.py:142) raises for every batch of more than
 one row; it is not reproduced (DESIGN.md deviation 17): the update is the one the reference runs under `python -O`.
 """
-import copy
-
 import torch
 import torch.optim as optim
 
@@ -31,34 +29,23 @@ class SAC(SoftActorCritic):
     def __init__(self, pf, vf, qf, plr, vlr, qlr, optimizer_class=optim.Adam, policy_std_reg_weight=1e-3,
                  policy_mean_reg_weight=1e-3, reparameterization=True, automatic_entropy_tuning=True,
                  target_entropy=None, **kwargs):
-        SoftActorCritic.__init__(self, pf, policy_std_reg_weight, policy_mean_reg_weight, reparameterization,
-                                 automatic_entropy_tuning, target_entropy, **kwargs)
-        self._init_networks(vf, [qf], plr, vlr, qlr, optimizer_class)
-
-    def _init_networks(self, vf, critics, plr, vlr, qlr, optimizer_class):
-        """The critics (named by `_critic_names`), V and its target, and the optimizer over pf | critics | vf."""
+        """`qf`: the critic, or the list of critics that `_critic_names` names (TwinSAC)."""
+        super().__init__(pf, policy_std_reg_weight, policy_mean_reg_weight, reparameterization,
+                         automatic_entropy_tuning, target_entropy, **kwargs)
         self.vf = vf
-        for name, qf in zip(self._critic_names, critics):
-            setattr(self, name, qf)
-        self._critics = list(critics)
-        self.target_vf = copy.deepcopy(vf)
-        self.to(self.device)
+        self._critics = qf if isinstance(qf, list) else [qf]
+        for name, q in zip(self._critic_names, self._critics):
+            setattr(self, name, q)
         self.plr, self.vlr, self.qlr = plr, vlr, qlr
-        # vf last: the Polyak source is one contiguous slice of the flat buffer
-        segments = [("pf", self.pf, plr)] + [(n, q, qlr) for n, q in zip(self._critic_names, critics)] + [("vf", vf, vlr)]
-        self._vf_seg = self._init_optimizer(optimizer_class, segments, eps=1e-8,
-                                            max_norms=[self.grad_clip or 0.0] * len(segments))["vf"]
-        self._init_targets()
+        # vf last: the checkpoint's network order, and the critics' backward reads segments 1 .. vf - 1
+        segments = [("pf", pf, plr)] + [(n, q, qlr) for n, q in zip(self._critic_names, self._critics)] + \
+            [("vf", vf, vlr)]
+        self._vf_seg = self._init_networks(optimizer_class, segments, eps=1e-8,
+                                           max_norms=[self.grad_clip or 0.0] * len(segments), targets=("vf",))["vf"]
 
     def _update_body(self, variant):
-        ub = self._ub
-        batch = self._batch()
-        info = ub["info"][0]
-        sc = ub["scratch"]
-        obs, acts, next_obs = batch["obs"], batch["acts"], batch["next_obs"]
-        rewards, terminals = batch["rewards"].reshape(-1), batch["terminals"].reshape(-1)
-        B = obs.shape[0]
-        acts = acts.reshape(B, -1)
+        batch, obs, acts, next_obs, rewards, terminals = self._transitions()
+        info, sc = self._ub["info"][0], self._ub["scratch"]
         new_actions, log_probs, mean, log_std = self._sample(obs, True)        # the update's only sample
         q_preds = [qf([obs, acts]) for qf in self._critics]
         v_pred = self.vf(obs)
@@ -79,10 +66,8 @@ class SAC(SoftActorCritic):
             roots += qns
             seeds += [g.reshape(q.shape) for g, q in zip((g_qn1, g_qn2), qns)]
         self._policy_backward(roots, seeds, mean, log_std, info)
-        segs = self.opt.segments
-        torch.autograd.backward(q_preds, [g.reshape(q.shape) for g, q in zip((g1, g2), q_preds)],
-                                inputs=[p for s in segs[1:self._vf_seg] for p in s])
-        torch.autograd.backward([v_pred], [g_v.reshape(v_pred.shape)], inputs=segs[self._vf_seg])
+        self._critic_backward(q_preds, [g1, g2], 1, self._vf_seg)
+        torch.autograd.backward([v_pred], [g_v.reshape(v_pred.shape)], inputs=self.opt.segments[self._vf_seg])
         self._optimizer_step()
         if self.grad_clip:
             info[_NORMS:_NORMS + self.opt.nseg].copy_(self.opt.grad_norms())
@@ -97,15 +82,3 @@ class SAC(SoftActorCritic):
             for i, name in enumerate(("pf",) + self._critic_names + ("vf",)):
                 info['Training/%s_grad_norm' % name] = float(row[_NORMS + i])
         return info
-
-    @property
-    def networks(self):
-        return [self.pf] + self._critics + [self.vf, self.target_vf]
-
-    @property
-    def snapshot_networks(self):
-        return [["pf", self.pf]] + [[n, q] for n, q in zip(self._critic_names, self._critics)] + [["vf", self.vf]]
-
-    @property
-    def target_networks(self):
-        return [(self.vf, self.target_vf)]

@@ -5,8 +5,6 @@ Keeps the reference's conventions, including the actor/target update firing when
 action coming from `target_pf.explore` (exploration noise included) before the clipped smoothing
 noise is added (td3.py:72-84).  Two captured graph variants: critics only / critics + actor.
 """
-import copy
-
 import torch
 import torch.optim as optim
 
@@ -23,16 +21,10 @@ class TD3(OffRLAlgo):
     def __init__(self, pf, qf1, qf2, plr, qlr, optimizer_class=optim.Adam, policy_update_delay=2,
                  norm_std_policy=0.2, noise_clip=0.5, **kwargs):
         super().__init__(**kwargs)
-        self.pf = pf
-        self.target_pf = copy.deepcopy(pf)
-        self.qf1, self.qf2 = qf1, qf2
-        self.target_qf1 = copy.deepcopy(qf1)
-        self.target_qf2 = copy.deepcopy(qf2)
-        self.to(self.device)
+        self.pf, self.qf1, self.qf2 = pf, qf1, qf2
         self.plr, self.qlr = plr, qlr
-        self._init_optimizer(optimizer_class, [("pf", pf, plr), ("qf1", qf1, qlr), ("qf2", qf2, qlr)], eps=1e-8,
-                             max_norms=[self.grad_clip or 0.0] * 3)
-        self._init_targets()
+        self._init_networks(optimizer_class, [("pf", pf, plr), ("qf1", qf1, qlr), ("qf2", qf2, qlr)], eps=1e-8,
+                            max_norms=[self.grad_clip or 0.0] * 3, targets=("pf", "qf1", "qf2"))
         self.policy_update_delay = policy_update_delay
         self.norm_std_policy = norm_std_policy
         self.noise_clip = noise_clip
@@ -43,14 +35,8 @@ class TD3(OffRLAlgo):
 
     # info: 0 Reward_Mean | 4 qf1_loss 5 qf2_loss | 6 policy_loss | 10..13 new_actions stats
     def _update_body(self, variant):
-        ub = self._ub
-        batch = self._batch()
-        info = ub["info"][0]
-        sc = ub["scratch"]
-        obs, acts, next_obs = batch["obs"], batch["acts"], batch["next_obs"]
-        rewards, terminals = batch["rewards"].reshape(-1), batch["terminals"].reshape(-1)
-        B = obs.shape[0]
-        acts = acts.reshape(B, -1)
+        batch, obs, acts, next_obs, rewards, terminals = self._transitions()
+        info, sc = self._ub["info"][0], self._ub["scratch"]
         with torch.no_grad():
             t_act = self.target_pf.explore(next_obs)["action"].contiguous()
             if D.get_noise_mode() == "reference_cpu":
@@ -67,15 +53,10 @@ class TD3(OffRLAlgo):
         q1_pred = self.qf1([obs, acts])
         q2_pred = self.qf2([obs, acts])
         g1, g2, _ = self._critic_loss(batch, q1_pred.reshape(-1), q2_pred.reshape(-1), y, info[4:6])
-        torch.autograd.backward([q1_pred, q2_pred], [g1.reshape(q1_pred.shape), g2.reshape(q2_pred.shape)],
-                                inputs=self.opt.segments[1] + self.opt.segments[2])
+        self._critic_backward([q1_pred, q2_pred], [g1, g2], 1, 3)
         self._optimizer_step(0b110)
         if variant == 1:
-            new_actions = self.pf(obs)
-            q_new = self.qf1([obs, new_actions])            # uses qf1 AFTER its step, like the reference
-            info[6:7].copy_((-q_new.detach().mean()).reshape(1))
-            seed = torch.full_like(q_new, -1.0 / q_new.numel())
-            torch.autograd.backward([q_new], [seed], inputs=self.opt.segments[0])
+            new_actions = self._deterministic_policy_step(self.qf1, obs, info)    # qf1 AFTER its step (reference)
             self._optimizer_step(0b001)
             self._update_target_networks()
             ops.vec_stats(new_actions.detach().reshape(-1), out=info[10:14])
@@ -87,15 +68,3 @@ class TD3(OffRLAlgo):
             info['Training/policy_loss'] = float(row[6])
             info.update(four_stats('new_actions', row[10:14]))
         return info
-
-    @property
-    def networks(self):
-        return [self.pf, self.qf1, self.qf2, self.target_pf, self.target_qf1, self.target_qf2]
-
-    @property
-    def snapshot_networks(self):
-        return [["pf", self.pf], ["qf1", self.qf1], ["qf2", self.qf2]]
-
-    @property
-    def target_networks(self):
-        return [(self.pf, self.target_pf), (self.qf1, self.target_qf1), (self.qf2, self.target_qf2)]

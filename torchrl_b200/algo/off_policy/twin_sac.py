@@ -4,7 +4,6 @@ min(Q1, Q2) in the value target and the policy loss, and one MSE per critic."""
 import torch.optim as optim
 
 from .sac import SAC
-from .twin_sac_q import SoftActorCritic
 
 
 class TwinSAC(SAC):
@@ -14,6 +13,5 @@ class TwinSAC(SAC):
     def __init__(self, pf, vf, qf1, qf2, plr, vlr, qlr, optimizer_class=optim.Adam, policy_std_reg_weight=1e-3,
                  policy_mean_reg_weight=1e-3, reparameterization=True, automatic_entropy_tuning=True,
                  target_entropy=None, **kwargs):
-        SoftActorCritic.__init__(self, pf, policy_std_reg_weight, policy_mean_reg_weight, reparameterization,
-                                 automatic_entropy_tuning, target_entropy, **kwargs)
-        self._init_networks(vf, [qf1, qf2], plr, vlr, qlr, optimizer_class)
+        super().__init__(pf, vf, [qf1, qf2], plr, vlr, qlr, optimizer_class, policy_std_reg_weight,
+                         policy_mean_reg_weight, reparameterization, automatic_entropy_tuning, target_entropy, **kwargs)

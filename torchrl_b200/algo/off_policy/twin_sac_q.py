@@ -8,8 +8,6 @@ Polyak over the flat target buffer -> log row.
 The temperature, the sample and the policy's regularisers and statistics live in SoftActorCritic, which SAC and
 TwinSAC (sac.py) share.
 """
-import copy
-
 import numpy as np
 import torch
 import torch.optim as optim
@@ -116,23 +114,13 @@ class TwinSACQ(SoftActorCritic):
         super().__init__(pf, policy_std_reg_weight, policy_mean_reg_weight, reparameterization,
                          automatic_entropy_tuning, target_entropy, **kwargs)
         self.qf1, self.qf2 = qf1, qf2
-        self.target_qf1 = copy.deepcopy(qf1)
-        self.target_qf2 = copy.deepcopy(qf2)
-        self.to(self.device)
         self.plr, self.qlr = plr, qlr
-        self._init_optimizer(optimizer_class, [("pf", pf, plr), ("qf1", qf1, qlr), ("qf2", qf2, qlr)], eps=1e-8,
-                             max_norms=[self.grad_clip or 0.0] * 3)
-        self._init_targets()
+        self._init_networks(optimizer_class, [("pf", pf, plr), ("qf1", qf1, qlr), ("qf2", qf2, qlr)], eps=1e-8,
+                            max_norms=[self.grad_clip or 0.0] * 3, targets=("qf1", "qf2"))
 
     def _update_body(self, variant):
-        ub = self._ub
-        batch = self._batch()
-        info = ub["info"][0]
-        sc = ub["scratch"]
-        obs, acts, next_obs = batch["obs"], batch["acts"], batch["next_obs"]
-        rewards, terminals = batch["rewards"].reshape(-1), batch["terminals"].reshape(-1)
-        B = obs.shape[0]
-        acts = acts.reshape(B, -1)
+        batch, obs, acts, next_obs, rewards, terminals = self._transitions()
+        info, sc = self._ub["info"][0], self._ub["scratch"]
         new_actions, log_probs, mean, log_std = self._sample(obs, True)
         q1_pred = self.qf1([obs, acts])
         q2_pred = self.qf2([obs, acts])
@@ -151,23 +139,10 @@ class TwinSACQ(SoftActorCritic):
         self._policy_backward([log_probs, qn1, qn2],
                               [g_lp.reshape(log_probs.shape), g_qn1.reshape(qn1.shape), g_qn2.reshape(qn2.shape)],
                               mean, log_std, info)
-        torch.autograd.backward([q1_pred, q2_pred], [g1.reshape(q1_pred.shape), g2.reshape(q2_pred.shape)],
-                                inputs=self.opt.segments[1] + self.opt.segments[2])
+        self._critic_backward([q1_pred, q2_pred], [g1, g2], 1, 3)
         self._optimizer_step()
         self._update_target_networks()
         self._finish_update()
 
     def _critic_info(self, row):
         return {'Training/qf1_loss': float(row[4]), 'Training/qf2_loss': float(row[5])}
-
-    @property
-    def networks(self):
-        return [self.pf, self.qf1, self.qf2, self.target_qf1, self.target_qf2]
-
-    @property
-    def snapshot_networks(self):
-        return [["pf", self.pf], ["qf1", self.qf1], ["qf2", self.qf2]]
-
-    @property
-    def target_networks(self):
-        return [(self.qf1, self.target_qf1), (self.qf2, self.target_qf2)]

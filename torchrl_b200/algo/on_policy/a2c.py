@@ -27,7 +27,6 @@ class A2C(OnRLAlgo):
         super().__init__(**kwargs)
         self.pf = pf
         self.vf = vf
-        self.to(self.device)
         self.plr = plr
         self.vlr = vlr
         self.optimizer_class = optimizer_class
@@ -35,8 +34,8 @@ class A2C(OnRLAlgo):
         # (unclipped)
         nets = self._net_segments(plr, vlr)
         extra = self._extra_opt_segments()
-        self._init_optimizer(optimizer_class, nets + extra, eps=self.adam_eps,
-                             max_norms=[0.5] * len(nets) + [0.0] * len(extra))
+        self._init_networks(optimizer_class, nets + extra, eps=self.adam_eps,
+                            max_norms=[0.5] * len(nets) + [0.0] * len(extra), targets=self._target_segments)
         self.entropy_coeff = entropy_coeff
         self.vf_criterion = torch.nn.MSELoss()
         self.sample_key = ["obs", "acts", "advs", "estimate_returns"]
@@ -50,6 +49,7 @@ class A2C(OnRLAlgo):
 
     # ------------------------------------------------------------------ what subclasses specialise
     adam_eps = 1e-5
+    _target_segments = ()           # the segments whose network has a target network (PPO and V-MPO: "pf")
 
     def _net_segments(self, plr, vlr):
         """[(name, network, lr)] of the networks the agent trains, each clipped to a gradient norm of 0.5."""
@@ -289,7 +289,3 @@ class A2C(OnRLAlgo):
         row = st["info"][0].cpu().numpy()
         row[20:24] = st["adv_table"][0].cpu().numpy()                   # where _flush_infos puts the epoch's table
         return self._decode_info(row, self.opt.grad_norms().cpu().numpy() * scale, st)
-
-    @property
-    def snapshot_networks(self):
-        return [("pf", self.pf), ("vf", self.vf)]

@@ -46,7 +46,3 @@ class OnRLAlgo(RLAlgo):
         record = self.logger.add_update_info
         for batch in self.replay_buffer.one_iteration(self.batch_size, self.sample_key, self.shuffle):
             record(self.update(batch))
-
-    @property
-    def networks(self):
-        return [self.pf, self.vf]

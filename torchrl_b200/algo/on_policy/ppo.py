@@ -13,8 +13,6 @@ Exactness notes (SURVEY.md section 7):
     so the result equals the reference's critic-then-actor order;
   * minibatch row order comes from np.random.permutation on the host (bit-exact indexing).
 """
-import copy
-
 import numpy as np
 import torch
 
@@ -29,14 +27,14 @@ _INFO_KEYS_ACTOR = ['Training/policy_loss', 'logprob/mean', 'logprob/std', 'logp
 
 
 class PPO(A2C):
+    _target_segments = ("pf",)
+
     def __init__(self, pf, clip_para=0.2, opt_epochs=10, clipped_value_loss=False, **kwargs):
-        self.target_pf = copy.deepcopy(pf)
         super().__init__(pf=pf, **kwargs)
         self.clip_para = clip_para
         self.opt_epochs = opt_epochs
         self.clipped_value_loss = clipped_value_loss
         self.sample_key = ["obs", "acts", "advs", "estimate_returns", "values"]
-        self._init_targets()
 
     # ------------------------------------------------------------------ specialisation of the minibatch loop
     def _passes(self):
@@ -103,11 +101,3 @@ class PPO(A2C):
             info[k] = float(row[7 + i])
         info['grad_norm/pf'] = float(norms[0])
         return info
-
-    @property
-    def networks(self):
-        return [self.pf, self.vf, self.target_pf]
-
-    @property
-    def target_networks(self):
-        return [(self.pf, self.target_pf)]

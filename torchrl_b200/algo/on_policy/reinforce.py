@@ -62,5 +62,5 @@ class Reinforce(A2C):
         return info
 
     @property
-    def snapshot_networks(self):
-        return [("pf", self.pf)]
+    def networks(self):
+        return [self.pf, self.vf]        # the ZeroNet value function has no optimizer segment but is in checkpoints

@@ -15,8 +15,6 @@ its gradient wrt the selected rows' logits and the duals' gradient.  reference_q
 summed KL: for a Categorical, kl_divergence(...).sum(-1, keepdim=True) sums over the rows (one scalar K that enters
 every row's loss and the alpha loss); False uses the per-row KL of the Gaussian path and the V-MPO paper.
 """
-import copy
-
 import torch
 
 from ... import ops
@@ -26,9 +24,10 @@ from .policy_heads import CategoricalHead
 
 
 class VMPO(A2C):
+    _target_segments = ("pf",)
+
     def __init__(self, pf, opt_epochs=10, eta_eps=0.02, alpha_eps=0.1, clipped_value_loss=False,
                  reference_quirks=True, **kwargs):
-        self.target_pf = copy.deepcopy(pf)
         self.reference_quirks = reference_quirks
         self.eta_eps, self.alpha_eps = eta_eps, alpha_eps
         self.opt_epochs = opt_epochs
@@ -36,7 +35,6 @@ class VMPO(A2C):
         self.dual = torch.nn.Parameter(torch.tensor([1.0, 0.1], dtype=torch.float32, device=dev))   # [eta, alpha]
         super().__init__(pf=pf, **kwargs)
         self.sample_key = ["obs", "acts", "advs", "estimate_returns", "values"]
-        self._init_targets()
         self._categorical = isinstance(self._head, CategoricalHead)
 
     @property
@@ -166,11 +164,3 @@ class VMPO(A2C):
         info = super().update(batch)
         info['Training/eta'], info['Training/alpha'] = (float(v) for v in self.dual.detach().cpu().numpy())
         return info
-
-    @property
-    def networks(self):
-        return [self.pf, self.vf, self.target_pf]
-
-    @property
-    def target_networks(self):
-        return [(self.pf, self.target_pf)]

@@ -1,4 +1,5 @@
 """Epoch loop shared by every agent (API of /root/reference/torchrl/algo/rl_algo.py:14-190)."""
+import copy
 import os.path as osp
 import pathlib
 import pickle
@@ -57,8 +58,9 @@ class _Stopwatch:
 
 class RLAlgo:
     """Owns the epoch loop: collect -> update -> (every eval_interval) evaluate + report -> (every save_interval)
-    snapshot.  Subclasses provide `update_per_epoch`, the network lists and optionally pretrain / start_epoch /
-    finish_epoch hooks."""
+    snapshot.  Subclasses provide `update_per_epoch`, declare their networks through `_init_networks` and optionally
+    provide pretrain / start_epoch / finish_epoch hooks."""
+    _nets = _targets = ()           # names of the networks and of those with a target: see _init_networks
 
     def __init__(self, env=None, replay_buffer=None, collector=None, logger=None, grad_clip=None, discount=0.99,
                  num_epochs=3000, batch_size=128, device='cpu', save_interval=100, eval_interval=1, save_dir=None,
@@ -222,20 +224,50 @@ class RLAlgo:
             for info in infos:
                 self.logger.add_update_info(info)
 
-    # ------------------------------------------------------------------ the fused optimizer
-    def _init_optimizer(self, optimizer_class, segments, eps, max_norms):
-        """self.opt = one FlatAdam over `segments`, [(name or None, module or parameter list, lr)] in flat-buffer order,
-        with one max grad norm per segment (0: no clipping).  A named segment gets the reference's handle
-        `self.<name>_optimizer`.  Returns {name: segment index}."""
+    # ------------------------------------------------------------------ networks, the fused optimizer, target networks
+    def _init_networks(self, optimizer_class, segments, eps, max_norms, targets=()):
+        """The agent's networks, declared once.  `segments`: [(name or None, module or parameter list, lr)] in
+        flat-buffer order, with one max grad norm per segment (0: no clipping); `targets`: the names of the segments
+        whose network has a target network.  In this order: self.target_<name> = a copy of each such network (before
+        anything moves the online weights), the networks move to the device, self.opt = one FlatAdam over the segments
+        (a named segment gets the reference's handle `self.<name>_optimizer`), and self._target_flat = one flat buffer
+        over the targets.  Returns {name: segment index}.
+
+        Polyak averaging and hard copies read the online networks as one slice of the optimizer's buffer, so the
+        segments with a target must be contiguous."""
         if optimizer_class is not optim.Adam:
             raise NotImplementedError("torchrl_b200 fuses clip + Adam in CUDA; only optim.Adam is supported "
                                       "(DESIGN.md section 6, deviation 10)")
+        index = {name: i for i, (name, _, _) in enumerate(segments) if name is not None}
+        self._nets = [name for name, net, _ in segments if name is not None and isinstance(net, torch.nn.Module)]
+        self._targets = [name for name in self._nets if name in targets]
+        assert len(self._targets) == len(targets), "a network with a target must be a named optimizer segment"
+        for name in self._targets:
+            setattr(self, "target_" + name, copy.deepcopy(getattr(self, name)))
+        self.to(self.device)
         self.opt = FlatAdam([params for _, params, _ in segments], lrs=[lr for _, _, lr in segments], eps=eps,
                             max_norms=max_norms, device=self.device, dist=self.dist)
-        index = {name: i for i, (name, _, _) in enumerate(segments) if name is not None}
         for name, i in index.items():
             setattr(self, name + "_optimizer", SegmentOptimizer(self.opt, i))
+        if self._targets:
+            segs = [index[name] for name in self._targets]
+            assert segs[-1] - segs[0] == len(segs) - 1, "the networks with a target must be contiguous segments"
+            self._target_segs = (segs[0], segs[-1] + 1)
+            self._target_flat = FlatParams([target for _, target in self.target_networks], device=self.device)
         return index
+
+    @property
+    def networks(self):
+        """What a checkpoint saves, in its order: the named networks in segment order, then their targets."""
+        return [getattr(self, name) for name in self._nets] + [target for _, target in self.target_networks]
+
+    @property
+    def target_networks(self):
+        return [(getattr(self, name), getattr(self, "target_" + name)) for name in self._targets]
+
+    @property
+    def snapshot_networks(self):
+        return [(name, getattr(self, name)) for name in self._nets]
 
     def _optimizer_step(self, active_mask=None):
         """Clip + Adam over the segments in `active_mask` (None: all).  Data parallel (every rank draws the same rows
@@ -244,27 +276,6 @@ class RLAlgo:
         scale, reduced = self.dist.reduce_grads(self.opt, active_mask) if self.dist is not None else (1.0, False)
         self.opt.step(active_mask=active_mask, grad_scale=scale, reduced=reduced)
         return scale
-
-    # ------------------------------------------------------------------ target networks
-    def _init_targets(self):
-        """self._target_flat: one flat buffer over the target networks in `target_networks` order.  Polyak averaging
-        and hard copies read the online networks as one slice of the optimizer's buffer, so each online network must
-        be exactly one optimizer segment, and those segments must be contiguous and in the same order."""
-        pairs = self.target_networks
-        segs = []
-        for online, _ in pairs:
-            params = list(online.parameters())
-            matches = [i for i, seg in enumerate(self.opt.segments)
-                       if len(seg) == len(params) and all(p is q for p, q in zip(seg, params))]
-            assert len(matches) == 1, "an online network of target_networks is not one optimizer segment"
-            segs.append(matches[0])
-        assert segs == list(range(segs[0], segs[0] + len(segs))), \
-            "target_networks must follow contiguous optimizer segments in order"
-        self._target_segs = (segs[0], segs[-1] + 1)
-        self._target_flat = FlatParams([target for _, target in pairs], device=self.device)
-        begin = self.opt.seg_begin[segs[0]]
-        assert self._target_flat.seg_begin == [b - begin for b in self.opt.seg_begin[segs[0]:segs[-1] + 2]], \
-            "target and online networks differ in layout"
 
     def _update_target_networks(self):
         """Polyak update of the target nets (rl_algo.py:169-172) on the flat buffers: one launch,
@@ -281,18 +292,6 @@ class RLAlgo:
     def _hard_update_targets(self):
         """Targets <- online networks (copy_model_params_from_to on the flat buffers)."""
         self._target_flat.copy_from(self.opt.seg_slice(*self._target_segs))
-
-    @property
-    def networks(self):
-        return []
-
-    @property
-    def snapshot_networks(self):
-        return []
-
-    @property
-    def target_networks(self):
-        return []
 
     def to(self, device):
         for net in self.networks:
