@@ -13,6 +13,11 @@
  *   - `stream` is a cudaStream_t passed as void*; launches are asynchronous, no host sync;
  *   - return value: 0 = ok, <0 = argument error (TRL_E*), >0 = cudaError_t of the launch;
  *     trl_last_error() returns the message of the calling thread's last failure.
+ *
+ * This header is the one statement of the ABI: every kernel source is compiled against it, and the Python
+ * binding (torchrl_b200/_lib.py) reads each entry point's types from it.  The binding accepts declarations of the
+ * form `ret trl_name(type name, ...);` (block comments anywhere) with ret int, int64_t or const char*, scalar
+ * parameters int, int64_t, unsigned, uint64_t, float or double, and pointers to those, to uint8_t, int32_t or void.
  */
 #ifndef TORCHRL_B200_H
 #define TORCHRL_B200_H

@@ -1,5 +1,6 @@
 """The drop-in boundary: the C-ABI library loads (no GPU needed), exports every symbol that
-include/torchrl_b200.h declares, and the product package never imports the oracle."""
+include/torchrl_b200.h declares, the binding takes its types from that header and checks operands against it, and
+the product package never imports the oracle."""
 import os
 import re
 
@@ -22,6 +23,58 @@ def test_header_symbols_exported(native_lib):
         assert hasattr(native_lib, name), "header declares %s but the library does not export it" % name
     # and the python binding types exactly the declared set
     assert sorted(_lib.SIGNATURES) == declared
+
+
+def test_definitions_match_declarations():
+    """Every TRL_API definition in csrc/ is declared in the header and the other way round (the compiler checks
+    their types: every kernel source includes the header)."""
+    csrc = os.path.join(ROOT, "torchrl_b200", "csrc")
+    defined = set()
+    for fn in os.listdir(csrc):
+        if fn.endswith((".cu", ".cuh")):
+            src = re.sub(r"/\*.*?\*/|//[^\n]*", "", open(os.path.join(csrc, fn)).read(), flags=re.S)
+            defined |= set(re.findall(r"\bTRL_API\s[\w\s*]*?\b(trl_[a-z0-9_]+)\s*\(", src))
+    assert sorted(defined) == _declared_symbols()
+
+
+def test_header_parse_errors(tmp_path):
+    """A missing header or a type the binding does not map fails loudly, naming the declaration."""
+    from torchrl_b200 import _lib
+    with pytest.raises(_lib.NativeLibraryError):
+        _lib.parse_header(str(tmp_path / "missing.h"))
+    h = tmp_path / "bad.h"
+    h.write_text("int trl_ok(const float* x, int64_t n, void* stream);\nint trl_bad(const short* x, int n);\n")
+    with pytest.raises(_lib.NativeLibraryError, match="trl_bad"):
+        _lib.parse_header(str(h))
+
+
+def test_call_checks_argument_count(native_lib):
+    """Too many or too few arguments raise before the library is called (ctypes alone passes extra ones through)."""
+    from torchrl_b200 import _lib
+    args = [None] * 7 + [4, 4, 0.99, 0.95, 1, 1, None]
+    before = _lib.launch_count()
+    with pytest.raises(TypeError, match="takes 14 arguments, got 15"):
+        _lib.call("trl_gae_scan", *args, 7)
+    with pytest.raises(TypeError, match="takes 14 arguments, got 13"):
+        _lib.call("trl_gae_scan", *args[:-1])
+    assert _lib.launch_count() == before
+
+
+def test_call_rejects_cpu_tensors(native_lib):
+    """A CPU tensor for a typed pointer parameter raises ValueError naming the header's parameter; nothing reaches
+    the library (which would reject the NULL operands with RuntimeError)."""
+    import torch
+
+    from torchrl_b200 import _lib
+    x = torch.zeros(16)
+    before = _lib.launch_count()
+    with pytest.raises(ValueError, match="trl_gae_scan: values must be a CUDA tensor"):
+        _lib.call("trl_gae_scan", None, x, None, None, None, None, None, 4, 4, 0.99, 0.95, 1, 1, None)
+    with pytest.raises(ValueError, match="trl_skinny_reduce_jobs: scratch must be a CUDA tensor"):
+        _lib.call("trl_skinny_reduce_jobs", 1, None, [x], [None], [None], None, None, None, None, None)
+    with pytest.raises(RuntimeError, match="trl_gae_scan failed"):
+        _lib.call("trl_gae_scan", None, None, None, None, None, None, None, 4, 4, 0.99, 0.95, 1, 1, None)
+    assert _lib.launch_count() == before
 
 
 def test_abi_version_and_error_string(native_lib):

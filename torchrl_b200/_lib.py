@@ -1,151 +1,39 @@
-"""ctypes binding of libtorchrl_b200.so (the C ABI declared in include/torchrl_b200.h).
+"""ctypes binding of libtorchrl_b200.so.
 
-There is NO fallback: if the shared object is missing or a symbol is absent the import
-of any op raises.  ``load()`` only dlopens the library -- it needs libcudart's static
+The C ABI is declared once, in include/torchrl_b200.h: ``load()`` reads every entry point's argument and return types
+from that header, and ``call()`` checks each operand against its declaration before the launch.
+
+There is NO fallback: if the shared object or the header is missing, a symbol is absent or a declaration uses a type
+the binding does not know, ``load()`` raises.  ``load()`` only dlopens the library -- it needs libcudart's static
 copy inside the .so but no GPU, so the symbol/ABI checks run on CPU boxes too.
 """
 import ctypes
 import os
+import re
+
+import torch
+
+from . import build
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libtorchrl_b200.so")
+HEADER_PATH = build.HEADER
 
-c_f32p = ctypes.c_void_p
-c_u8p = ctypes.c_void_p
-c_i32p = ctypes.c_void_p
-c_i64p = ctypes.c_void_p
-c_f64p = ctypes.c_void_p
-vp = ctypes.c_void_p
-i64 = ctypes.c_int64
-i32 = ctypes.c_int
-f32 = ctypes.c_float
-f64 = ctypes.c_double
-u64 = ctypes.c_uint64
-u32 = ctypes.c_uint32
+_SCALARS = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "unsigned": ctypes.c_uint32, "uint64_t": ctypes.c_uint64,
+            "float": ctypes.c_float, "double": ctypes.c_double}
+_RESTYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "char*": ctypes.c_char_p}
+# the tensor dtype of each pointee type; void: no dtype check
+_DTYPES = {"float": torch.float32, "double": torch.float64, "uint8_t": torch.uint8, "int": torch.int32,
+           "int32_t": torch.int32, "unsigned": torch.int32, "int64_t": torch.int64, "uint64_t": torch.int64,
+           "void": None}
+_DECL = re.compile(r"^\s*([\w *]+?)\s*\b(trl_\w+)\s*\(([^)]*)\)\s*;", re.M)
+_PARAM = re.compile(r"(.*?)(\w+)", re.S)
 
-# name -> argtypes   (restype is int unless listed in _RESTYPES)
-SIGNATURES = {
-    "trl_last_error": [],
-    "trl_abi_version": [],
-    "trl_device_info": [vp, vp, vp],
-    "trl_gae_scan": [vp, vp, vp, vp, vp, vp, vp, i64, i64, f32, f32, i32, i32, vp],
-    "trl_discount_return": [vp, vp, vp, vp, vp, vp, vp, i64, i64, f32, i32, i32, vp],
-    "trl_synth_env_smem_bytes": [i32, i32],
-    "trl_synth_env_num_ctas": [i64],
-    "trl_synth_env_step": [vp] * 20 + [i64, i32, i32, f32, f32, f32, f32, f32, i32, i32, i32, vp],
-    "trl_synth_env_reset": [vp, vp, vp, vp, vp, i64, i32, f64, vp],
-    "trl_synth_env_seed": [vp, vp, i64, u32, u32, u32, vp],
-    "trl_obs_norm_moments": [vp, i64, i32, vp, vp],
-    "trl_obs_norm_merge": [vp, f64, i32, vp, vp, vp, vp],
-    "trl_obs_norm_filt": [vp, vp, vp, i64, i32, f64, vp, vp],
-    "trl_tanh_gaussian_sample": [vp, vp, i32, vp, f32, u64, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp],
-    "trl_tanh_gaussian_sample_bwd": [vp, vp, vp, i32, vp, vp, i64, i32, i32, vp, vp, vp],
-    "trl_collect_finalize": [vp] * 29 + [i64, i32, i32, i32, f32, f64, f64, i32, i32, vp],
-    "trl_step_advance": [vp, i32, vp, vp, vp],
-    "trl_row_gather": [i32, vp, vp, vp, vp, vp, i32, vp],
-    "trl_ring_write": [i32, vp, vp, vp, vp, vp],
-    "trl_ring_write_advance": [i32, vp, vp, vp, vp, i32, vp, vp, vp],
-    "trl_vec_stats": [vp, i64, vp, vp],
-    "trl_vec_moments": [vp, i64, vp, vp],
-    "trl_vec_stats_from_moments": [vp, i32, f64, vp, vp],
-    "trl_row_group_moments": [vp, vp, i32, i32, i64, vp, vp],
-    "trl_group_stats_from_moments": [vp, i32, i32, f64, vp, vp],
-    "trl_ppo_actor_scratch_doubles": [i64, i32],
-    "trl_ppo_actor_loss": [vp, vp, i32, vp, vp, vp, vp, vp, i64, i32, i32, f32, f32, f32, f32, vp, vp, vp, vp, vp, vp, vp],
-    "trl_ppo_critic_loss": [vp, vp, vp, i64, i32, f32, vp, vp, vp, vp, vp],
-    "trl_gaussian_log_prob": [vp, vp, i32, vp, i64, i32, i32, vp, vp],
-    "trl_categorical_sample": [vp, vp, u64, vp, i64, i32, vp, vp, vp, vp],
-    "trl_categorical_log_prob": [vp, vp, i64, i32, vp, vp],
-    "trl_ppo_categorical_actor_scratch_doubles": [i64],
-    "trl_ppo_categorical_actor_loss": [vp, vp, vp, vp, vp, vp, i64, i32, f32, f32, vp, vp, vp, vp, vp, vp],
-    "trl_vmpo_select": [vp, vp, i32, i32, i64, vp, vp, vp],
-    "trl_vmpo_categorical_scratch_doubles": [i64],
-    "trl_vmpo_categorical_loss": [vp, vp, vp, vp, vp, vp, vp, i64, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
-    "trl_categorical_fisher_vp": [vp, vp, i64, i32, f32, vp, vp],
-    "trl_tangent_bias_act": [vp, vp, vp, i64, i32, i64, i32, vp],
-    "trl_categorical_surrogate": [vp, vp, vp, vp, i64, i32, vp, vp, vp, vp],
-    "trl_grad_sumsq_blocks": [i32],
-    "trl_grad_sumsq": [vp, vp, i32, u32, vp, vp, f64, f64, vp, vp, vp],
-    "trl_adam_step": [vp, vp, vp, vp, vp, i32, u32, vp, vp, vp, vp, f32, f32, f32, i32, vp, vp, vp],
-    "trl_polyak_update": [vp, vp, i64, f32, vp, vp, vp],
-    "trl_bias_act_bwd_scratch_floats": [i64, i32],
-    "trl_bias_act_fwd": [vp, vp, i64, i32, i32, vp],
-    "trl_split_tf32": [vp, i64, vp, vp, vp],
-    "trl_bias_act_bwd": [vp, vp, vp, vp, i64, i32, i32, vp, vp, vp],
-    "trl_per_sample": [vp, i32, vp, i32, f32, vp, vp, vp],
-    "trl_per_scratch_doubles": [i32],
-    "trl_per_sample_rows": [vp, i32, vp, vp, vp, i32, f32, vp, vp, vp, vp],
-    "trl_per_update": [vp, vp, vp, i32, i32, f32, f32, vp, vp],
-    "trl_per_insert": [vp, vp, vp, vp],
-    "trl_gemm_tf32x3_nt": [vp, vp, vp, i64, i64, i32, vp, vp, i32, vp],
-    "trl_gemm_tf32x3_tn": [vp, vp, vp, i64, i64, i32, vp, vp],
-    "trl_transpose_f32": [vp, vp, i64, i32, vp],
-    "trl_frame_ring_write": [vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i64, i32, i32, vp],
-    "trl_frame_hist_advance": [vp, vp, i32, vp],
-    "trl_frame_stack_gather": [vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, i64, i32, i64, i32, f32, vp, vp, vp],
-    "trl_comm_flag_bytes": [],
-    "trl_comm_ipc_handle_bytes": [],
-    "trl_comm_alloc": [i64, vp],
-    "trl_comm_free": [vp],
-    "trl_comm_ipc_get": [vp, vp],
-    "trl_comm_ipc_open": [vp, vp],
-    "trl_comm_ipc_close": [vp],
-    "trl_comm_scratch_doubles": [i32],
-    "trl_allreduce_grad": [vp, vp, i32, i32, vp, i64, vp, i32, u32, vp, vp, f64, f64, vp, vp, vp, i32, vp],
-    "trl_allreduce_f64": [vp, vp, i32, i32, vp, i32, i32, vp, vp],
-    "trl_comm_ll_recv_bytes": [i32, i32],
-    "trl_allreduce_f64_ll": [vp, vp, i32, i32, vp, i32, i32, i32, vp, vp],
-    "trl_gemm3_pair": [vp, vp, vp, vp, i64, i64, i32, vp, i32, vp],
-    "trl_gemm3_pair_tn": [vp, vp, vp, i64, i64, i32, vp, vp],
-    "trl_gemm3_pair_tn_cluster": [vp, vp, vp, i64, i64, i32, vp, vp, vp],
-    "trl_gemm3_pair_dgrad_act_wgrad": [vp, vp, vp, vp, vp, i64, i32, i32, vp, vp],
-    "trl_skinny_k_fwd": [vp, vp, vp, vp, i64, i32, i32, i32, vp],
-    "trl_skinny_tn_scratch_floats": [i64, i32, i32],
-    "trl_skinny_tn": [vp, vp, vp, vp, i64, i32, i32, i32, vp, vp],
-    "trl_skinny_n_fwd": [vp, vp, vp, vp, i64, i32, i32, vp],
-    "trl_skinny_n_dgrad": [vp, vp, vp, i64, i32, i32, vp],
-    "trl_skinny_act_wgrad": [vp, vp, vp, vp, vp, i64, i32, i32, i32, vp, vp],
-    "trl_skinny_dgrad_act_scratch_floats": [i64, i32],
-    "trl_skinny_n_dgrad_act": [vp, vp, vp, vp, vp, i64, i32, i32, i32, vp, vp],
-    "trl_skinny_tn_partial": [vp, vp, i64, i32, i32, i32, vp, vp],
-    "trl_skinny_act_wgrad_partial": [vp, vp, vp, i64, i32, i32, i32, vp, vp],
-    "trl_skinny_n_dgrad_act_partial": [vp, vp, vp, vp, i64, i32, i32, i32, vp, vp],
-    "trl_skinny_reduce_jobs": [i32, vp, vp, vp, vp, vp, vp, vp, vp, vp],
-    "trl_skinny_n_dgrad_act_wgrad_partial": [vp, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp],
-    "trl_skinny_n_dgrad_act_wgrad": [vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp],
-    "trl_synth_atari_step": [vp, vp, vp, vp, vp, vp, vp, i64, i32, vp],
-    "trl_synth_atari_reset": [vp, vp, vp, vp, vp, vp, vp, i32, i32, i64, vp],
-    "trl_u8_to_f32": [vp, vp, i64, f32, vp],
-    "trl_cartpole_num_ctas": [i64],
-    "trl_cartpole_step": [vp] * 16 + [i64, f32, i32, i32, i32, vp],
-    "trl_pendulum_num_ctas": [i64],
-    "trl_pendulum_step": [vp] * 17 + [i64, f32, i32, i32, i32, vp],
-    "trl_pendulum_reset": [vp] * 13 + [i64, f64, i32, vp],
-    "trl_offpolicy_scratch_doubles": [i64],
-    "trl_td_target": [vp, vp, vp, vp, vp, vp, f32, f32, i64, vp, vp, vp, vp, vp],
-    "trl_td3_smooth_action": [vp, vp, f32, f32, u64, vp, i64, vp, vp],
-    "trl_sac_alpha_step": [vp, f32, vp, vp, f32, f32, f32, f32, i64, vp, vp, vp, vp],
-    "trl_sac_policy_loss": [vp, vp, vp, vp, f32, i64, vp, vp, vp, vp, vp, vp, vp],
-    "trl_sac_v_loss": [vp, vp, vp, vp, vp, f32, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp],
-    "trl_twin_mse_loss": [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp],
-    "trl_twin_mse_loss_weighted": [vp, vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp],
-    "trl_qr_dqn_loss": [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, i32, vp, vp, vp, vp, vp, vp],
-    "trl_bootstrapped_dqn_loss": [vp, vp, vp, vp, vp, vp, i64, i32, i32, f32, vp, vp, vp, vp, vp],
-    "trl_bootstrapped_act": [vp, vp, vp, vp, vp, vp, vp, vp, u64, vp, vp, i64, i32, i32, f32, vp],
-}
-_RESTYPES = {"trl_last_error": ctypes.c_char_p, "trl_ppo_actor_scratch_doubles": ctypes.c_int64,
-             "trl_ppo_categorical_actor_scratch_doubles": ctypes.c_int64,
-             "trl_vmpo_categorical_scratch_doubles": ctypes.c_int64,
-             "trl_offpolicy_scratch_doubles": ctypes.c_int64, "trl_bias_act_bwd_scratch_floats": ctypes.c_int64,
-             "trl_skinny_tn_scratch_floats": ctypes.c_int64,
-             "trl_skinny_dgrad_act_scratch_floats": ctypes.c_int64, "trl_comm_ll_recv_bytes": ctypes.c_int64}
-# entry points that return a value rather than an error code
-_VALUE_FUNCS = ("trl_abi_version", "trl_synth_env_smem_bytes", "trl_synth_env_num_ctas", "trl_cartpole_num_ctas",
-                "trl_pendulum_num_ctas", "trl_comm_flag_bytes",
-                "trl_comm_ipc_handle_bytes", "trl_comm_scratch_doubles", "trl_comm_ll_recv_bytes",
-                "trl_ppo_actor_scratch_doubles", "trl_ppo_categorical_actor_scratch_doubles", "trl_vmpo_categorical_scratch_doubles",
-                "trl_grad_sumsq_blocks", "trl_per_scratch_doubles")
-
+# name -> (restype, params), params: (name, ctypes type, pointee dtype or None, pointer depth) per parameter
+SIGNATURES = {}
+# name -> (function, parameter count, (index, dtype) of each pointer parameter (dtype None: not checked),
+#         (index, element dtype) of each `T* const*` parameter)
+_CALLS = {}
 _lib = None
 
 
@@ -153,29 +41,60 @@ class NativeLibraryError(RuntimeError):
     pass
 
 
+def _bare(ctype):
+    return re.sub(r"\bconst\b|\s", "", ctype)
+
+
+def parse_header(path):
+    """SIGNATURES of every declaration `ret trl_name(type name, ...);` of the header, comments stripped."""
+    if not os.path.exists(path):
+        raise NativeLibraryError("%s not found: the binding reads the C ABI from it" % path)
+    src = re.sub(r"/\*.*?\*/", "", open(path).read(), flags=re.S)
+    sigs = {}
+    for ret, name, params in _DECL.findall(src):
+        decl = "%s(%s)" % (name, " ".join(params.split()))
+        if _bare(ret) not in _RESTYPES:
+            raise NativeLibraryError("%s: unsupported return type %r of %s" % (path, ret.strip(), decl))
+        out = []
+        for p in ([] if params.strip() == "void" else params.split(",")):
+            ctype, pname = _PARAM.fullmatch(p.strip()).groups()
+            t = _bare(ctype)
+            base = t.rstrip("*")
+            depth = len(t) - len(base)
+            if base not in (_DTYPES if depth else _SCALARS):
+                raise NativeLibraryError("%s: unsupported type %r in %s" % (path, ctype.strip(), decl))
+            out.append((pname, ctypes.c_void_p if depth else _SCALARS[base], _DTYPES[base] if depth else None, depth))
+        sigs[name] = (_RESTYPES[_bare(ret)], out)
+    return sigs
+
+
 def load():
-    """dlopen the library once and type every entry point.  Raises if anything is missing."""
+    """dlopen the library once and type every entry point the header declares.  Raises if anything is missing."""
     global _lib
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH) and os.environ.get("TORCHRL_B200_NO_AUTOBUILD") != "1":
         try:                                    # nvcc is part of the image: compile in-tree on first use
-            from . import build as _build
-            _build.build()
+            build.build()
         except Exception as e:                  # noqa: BLE001
             raise NativeLibraryError("%s not found and the in-tree nvcc build failed (%s); there is no CPU "
                                      "fallback" % (LIB_PATH, e)) from e
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
             "%s not found: build it with `python -m torchrl_b200.build` (there is no CPU fallback)" % LIB_PATH)
+    sigs = parse_header(HEADER_PATH)
     lib = ctypes.CDLL(LIB_PATH)
-    for name, argtypes in SIGNATURES.items():
+    for name, (restype, params) in sigs.items():
         try:
             fn = getattr(lib, name)
         except AttributeError as e:
             raise NativeLibraryError("symbol %s missing from %s" % (name, LIB_PATH)) from e
-        fn.argtypes = argtypes
-        fn.restype = _RESTYPES.get(name, ctypes.c_int)
+        fn.argtypes = [p[1] for p in params]
+        fn.restype = restype
+        ptrs = [(i, dtype, depth) for i, (_, _, dtype, depth) in enumerate(params) if depth]
+        _CALLS[name] = (fn, len(params), tuple((i, dtype if depth == 1 else None) for i, dtype, depth in ptrs),
+                        tuple((i, dtype) for i, dtype, depth in ptrs if depth == 2 and dtype is not None))
+    SIGNATURES.update(sigs)
     _lib = lib
     return lib
 
@@ -199,12 +118,48 @@ def add_launches(n):
     _LAUNCHES += int(n)
 
 
+def _reject(name, i, t, dtype):
+    what = "%s: %s" % (name, SIGNATURES[name][1][i][0])
+    if not t.is_cuda:
+        raise ValueError("%s must be a CUDA tensor (torchrl_b200 has no CPU path)" % what)
+    if t.dtype != dtype:
+        raise TypeError("%s must be %s, got %s" % (what, dtype, t.dtype))
+    raise ValueError("%s must be contiguous" % what)
+
+
+def _ptr(t, dtype, name, i):
+    if not (t.is_cuda and t.dtype is dtype and t.is_contiguous()):
+        _reject(name, i, t, dtype)
+    return t.data_ptr()
+
+
 def call(name, *args, kernels=1):
     """Invoke a kernel-launching entry point, raise on error and count the `kernels` kernels it launched (the
-    wrappers in ops.py know that number for each entry point and its arguments)."""
+    wrappers in ops.py know that number for each entry point and its arguments).
+
+    The arguments are those of the header's declaration, exactly as many.  A tensor passed for a `T*` parameter must
+    be a contiguous CUDA tensor of T's dtype (float32, float64, uint8, int32 for int / unsigned, int64 for int64_t /
+    uint64_t); for `void*` and pointer-to-pointer parameters it passes its address unchecked.  A list passed for a
+    `T* const*` parameter becomes a host array of its tensors' addresses (None: NULL), each checked against T.  None
+    is NULL; ints, ctypes objects and ctypes arrays pass through unchanged."""
     global _LAUNCHES
-    lib = load()
-    rc = getattr(lib, name)(*args)
+    if _lib is None:
+        load()
+    fn, nparams, pointers, arrays = _CALLS[name]
+    if len(args) != nparams:
+        raise TypeError("%s takes %d arguments, got %d" % (name, nparams, len(args)))
+    args = list(args)
+    for i, dtype in pointers:          # the hot loop: _ptr's test inlined
+        a = args[i]
+        if isinstance(a, torch.Tensor):
+            if dtype is not None and not (a.is_cuda and a.dtype is dtype and a.is_contiguous()):
+                _reject(name, i, a, dtype)
+            args[i] = a.data_ptr()
+    for i, dtype in arrays:
+        if isinstance(args[i], list):
+            args[i] = (ctypes.c_void_p * len(args[i]))(*[None if t is None else _ptr(t, dtype, name, i)
+                                                         for t in args[i]])
+    rc = fn(*args)
     if rc != 0:
         check(rc, name)
     _LAUNCHES += kernels

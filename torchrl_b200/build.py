@@ -14,6 +14,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
+HEADER = os.path.join(os.path.dirname(HERE), "include", "torchrl_b200.h")     # included by csrc/common.cuh
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 LIBNAME = "libtorchrl_b200.so"
@@ -50,7 +51,7 @@ def _digest(path, extra):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJDIR, exist_ok=True)
-    headers = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h")))
+    headers = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [HEADER]
     nvcc = _nvcc()
     jobs = []
     objs = []

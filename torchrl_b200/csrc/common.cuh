@@ -10,12 +10,10 @@
 #include <stdint.h>
 #include <stdio.h>
 
-#define TRL_API extern "C" __attribute__((visibility("default")))
+// The public declarations (and the TRL_E* codes): a definition that disagrees with its declaration does not compile.
+#include "../../include/torchrl_b200.h"
 
-#define TRL_OK 0
-#define TRL_EINVAL (-1)
-#define TRL_EALIGN (-2)
-#define TRL_EUNSUPPORTED (-3)
+#define TRL_API extern "C" __attribute__((visibility("default")))
 
 namespace trl {
 

@@ -1,9 +1,10 @@
 """Tensor-level wrappers over the C ABI (include/torchrl_b200.h).
 
-Each function takes torch CUDA tensors, checks dtype / contiguity / device, and launches
-the sm_90a kernel on torch's *current* stream (so every call is CUDA-graph capturable).
-Memory is owned by PyTorch's caching allocator; the library never allocates.  There is no
-CPU implementation: CPU tensors raise.
+Each function takes torch CUDA tensors and launches the sm_90a kernel on torch's *current*
+stream (so every call is CUDA-graph capturable); _lib.call checks every tensor's dtype,
+contiguity and device against the header's declaration before the launch.  Memory is owned
+by PyTorch's caching allocator; the library never allocates.  There is no CPU
+implementation: CPU tensors raise.
 """
 import ctypes
 
@@ -11,11 +12,13 @@ import torch
 
 from . import _lib
 
-F32, F64, U8, I32, I64 = torch.float32, torch.float64, torch.uint8, torch.int32, torch.int64
+F32, F64, I32, I64 = torch.float32, torch.float64, torch.int32, torch.int64
 
 
 def _stream():
-    return torch.cuda.current_stream().cuda_stream
+    """torch's current stream.  Until torch has initialised CUDA that is the null stream (0) and no tensor is on the
+    device, so a wrapper handed CPU tensors reaches _lib.call's operand check instead of failing here first."""
+    return torch.cuda.current_stream().cuda_stream if torch.cuda.is_initialized() else 0
 
 
 class CapturedGraph:
@@ -33,20 +36,6 @@ class CapturedGraph:
     def replay(self):
         self.graph.replay()
         _lib.add_launches(self.launches)
-
-
-def _chk(t, dtype, name):
-    if not t.is_cuda:
-        raise ValueError("%s must be a CUDA tensor (torchrl_b200 has no CPU path)" % name)
-    if t.dtype != dtype:
-        raise TypeError("%s must be %s, got %s" % (name, dtype, t.dtype))
-    if not t.is_contiguous():
-        raise ValueError("%s must be contiguous" % name)
-    return t.data_ptr()
-
-
-def _opt(t, dtype, name):
-    return None if t is None else _chk(t, dtype, name)
 
 
 def _tn(t):
@@ -70,11 +59,8 @@ def gae_scan(rewards, values, terminals, time_limits, last_value, gamma, tau, ti
         returns = torch.empty_like(rewards)
     assert values.shape == rewards.shape and terminals.shape == rewards.shape and \
         time_limits.shape == rewards.shape and last_value.numel() == N
-    _lib.call("trl_gae_scan",
-              _chk(rewards, F32, "rewards"), _chk(values, F32, "values"),
-              _chk(terminals, U8, "terminals"), _chk(time_limits, U8, "time_limits"),
-              _chk(last_value, F32, "last_value"), _chk(advs, F32, "advs"), _chk(returns, F32, "returns"),
-              T, N, float(gamma), float(tau), int(bool(time_limit_filter)), int(variant), _stream())
+    _lib.call("trl_gae_scan", rewards, values, terminals, time_limits, last_value, advs, returns, T, N, float(gamma),
+              float(tau), int(bool(time_limit_filter)), int(variant), _stream())
     return advs, returns
 
 
@@ -88,11 +74,8 @@ def discount_return(rewards, values, terminals, time_limits, last_value, gamma, 
     if returns is None:
         returns = torch.empty_like(rewards)
     assert values.shape == rewards.shape and last_value.numel() == N
-    _lib.call("trl_discount_return",
-              _chk(rewards, F32, "rewards"), _chk(values, F32, "values"),
-              _chk(terminals, U8, "terminals"), _chk(time_limits, U8, "time_limits"),
-              _chk(last_value, F32, "last_value"), _chk(advs, F32, "advs"), _chk(returns, F32, "returns"),
-              T, N, float(gamma), int(bool(time_limit_filter)), int(variant), _stream())
+    _lib.call("trl_discount_return", rewards, values, terminals, time_limits, last_value, advs, returns, T, N,
+              float(gamma), int(bool(time_limit_filter)), int(variant), _stream())
     return advs, returns
 
 
@@ -101,22 +84,20 @@ def obs_norm_moments(x, sums=None):
     N, o = x.shape
     if sums is None:
         sums = torch.empty(2 * o, dtype=F64, device=x.device)
-    _lib.call("trl_obs_norm_moments", _chk(x, F32, "x"), N, o, _chk(sums, F64, "sums"), _stream())
+    _lib.call("trl_obs_norm_moments", x, N, o, sums, _stream())
     return sums
 
 
 def obs_norm_merge(sums, batch_n, mean, var, count):
     o = mean.numel()
-    _lib.call("trl_obs_norm_merge", _chk(sums, F64, "sums"), float(batch_n), o, _chk(mean, F64, "mean"),
-              _chk(var, F64, "var"), _chk(count, F64, "count"), _stream())
+    _lib.call("trl_obs_norm_merge", sums, float(batch_n), o, mean, var, count, _stream())
 
 
 def obs_norm_filt(raw, mean, var, clip=10.0, out=None):
     N, o = raw.shape
     if out is None:
         out = torch.empty_like(raw)
-    _lib.call("trl_obs_norm_filt", _chk(raw, F32, "raw"), _chk(mean, F64, "mean"), _chk(var, F64, "var"), N, o,
-              float(clip), _chk(out, F32, "out"), _stream())
+    _lib.call("trl_obs_norm_filt", raw, mean, var, N, o, float(clip), out, _stream())
     return out
 
 
@@ -140,10 +121,8 @@ def tanh_gaussian_sample(mean, log_std, eps=None, tanh_action=True, want_log_pro
         if rng is None or rng.counter is None:
             raise ValueError("tanh_gaussian_sample needs either eps or an rng state")
         seed, ctr = rng.seed, rng.counter
-    _lib.call("trl_tanh_gaussian_sample", _chk(mean, F32, "mean"), _chk(log_std, F32, "log_std"), ls_stride,
-              _opt(eps, F32, "eps"), float(noise_scale), ctypes.c_uint64(seed), _opt(ctr, I64, "rng_counter"), M, a,
-              int(bool(tanh_action)), _chk(action, F32, "action"), _opt(pre, F32, "pre_tanh"),
-              _opt(logp, F32, "log_prob"), _opt(eps_out, F32, "eps_out"), _opt(nan_flag, I32, "nan_flag"), _stream())
+    _lib.call("trl_tanh_gaussian_sample", mean, log_std, ls_stride, eps, float(noise_scale), ctypes.c_uint64(seed), ctr,
+              M, a, int(bool(tanh_action)), action, pre, logp, eps_out, nan_flag, _stream())
     out = {"action": action}
     if pre is not None:
         out["pre_tanh"] = pre
@@ -162,16 +141,14 @@ def tanh_gaussian_sample_bwd(action, eps, log_std, g_action, g_logp, tanh_action
     ls_stride = 0 if log_std.dim() == 1 else a
     ga = g_action.contiguous() if g_action is not None else None
     gl = g_logp.contiguous() if g_logp is not None else None
-    _lib.call("trl_tanh_gaussian_sample_bwd", _chk(action, F32, "action"), _chk(eps, F32, "eps"),
-              _chk(log_std, F32, "log_std"), ls_stride, _opt(ga, F32, "g_action"), _opt(gl, F32, "g_logp"), M, a,
-              int(bool(tanh_action)), _chk(g_mean, F32, "g_mean"), _chk(g_ls, F32, "g_log_std"), _stream())
+    _lib.call("trl_tanh_gaussian_sample_bwd", action, eps, log_std, ls_stride, ga, gl, M, a, int(bool(tanh_action)),
+              g_mean, g_ls, _stream())
     return g_mean, g_ls
 
 
 def counter_advance(counter, t_ptr=None, T=1, size_ptr=None):
     """Device-side `counter += 1` (and optionally t = (t+1) % T, size = min(size+1, T))."""
-    _lib.call("trl_step_advance", _opt(t_ptr, I32, "t_ptr"), int(T), _opt(size_ptr, I32, "size_ptr"),
-              _opt(counter, I64, "counter"), _stream())
+    _lib.call("trl_step_advance", t_ptr, int(T), size_ptr, counter, _stream())
 
 
 def collect_finalize(cur_ob_in, next_norm, state, act, value, v_next, reward, done, tl, elapsed, episode, seeds,
@@ -182,19 +159,11 @@ def collect_finalize(cur_ob_in, next_norm, state, act, value, v_next, reward, do
     bootstrap and the partial reset of the finished envs.  cur_ob_in (N, o), act (N, a).  state / elapsed / episode /
     seeds / any_reset None: host envs (the host resets them afterwards)."""
     N, o = cur_ob_in.shape
-    _lib.call("trl_collect_finalize", _chk(cur_ob_in, F32, "cur_ob_in"), _chk(next_norm, F32, "next_norm"),
-              _opt(state, F32, "state"), _chk(act, F32, "act"), _opt(value, F32, "value"), _opt(v_next, F32, "v_next"),
-              _chk(reward, F32, "reward"), _chk(done, U8, "done"), _chk(tl, U8, "time_limit"),
-              _opt(elapsed, I32, "elapsed"), _opt(episode, I32, "episode"), _opt(seeds, I32, "seeds"),
-              _chk(step_count, I32, "step_count"), _chk(ep_return, F64, "ep_return"),
-              _chk(epoch_reward, F64, "epoch_reward"), _chk(ret_log, F32, "ret_log"), _chk(n_done, I32, "n_done"),
-              _opt(any_reset, I32, "any_reset"), _opt(norm_mean, F64, "norm_mean"), _opt(norm_var, F64, "norm_var"),
-              _chk(cur_ob_out, F32, "cur_ob_out"), _chk(b_obs, F32, "b_obs"), _chk(b_next_obs, F32, "b_next_obs"),
-              _chk(b_acts, F32, "b_acts"), _opt(b_values, F32, "b_values"), _chk(b_rewards, F32, "b_rewards"),
-              _chk(b_terminals, U8, "b_terminals"), _chk(b_time_limits, U8, "b_time_limits"),
-              _chk(t_ptr, I32, "t_ptr"), N, o, act.numel() // N, int(max_episode_frames), float(discount),
-              float(init_scale), float(clip), int(bool(terminal_includes_surpass)), int(bool(raw_obs_after_reset)),
-              _stream())
+    _lib.call("trl_collect_finalize", cur_ob_in, next_norm, state, act, value, v_next, reward, done, tl, elapsed,
+              episode, seeds, step_count, ep_return, epoch_reward, ret_log, n_done, any_reset, norm_mean, norm_var,
+              cur_ob_out, b_obs, b_next_obs, b_acts, b_values, b_rewards, b_terminals, b_time_limits, t_ptr, N, o,
+              act.numel() // N, int(max_episode_frames), float(discount), float(init_scale), float(clip),
+              int(bool(terminal_includes_surpass)), int(bool(raw_obs_after_reset)), _stream())
 
 
 # ------------------------------------------------------------------------------------------ K7/K9/K4
@@ -218,40 +187,38 @@ def row_bytes_of(t):
 
 def row_gather(plan, idx, rows, pos_ptr=None):
     """dst[k] = src[idx[pos*rows + k]] for every key of the plan; idx is an int64 device tensor."""
-    _lib.call("trl_row_gather", plan.n, plan.src, plan.dst, plan.rb, _chk(idx, I64, "idx"),
-              _opt(pos_ptr, I32, "pos_ptr"), int(rows), _stream())
+    _lib.call("trl_row_gather", plan.n, plan.src, plan.dst, plan.rb, idx, pos_ptr, int(rows), _stream())
 
 
 def ring_write(plan, row_ptr):
     """dst[*row_ptr] = src[0] for every key of the plan (one time-row)."""
-    _lib.call("trl_ring_write", plan.n, plan.src, plan.dst, plan.rb, _chk(row_ptr, I32, "row_ptr"), _stream())
+    _lib.call("trl_ring_write", plan.n, plan.src, plan.dst, plan.rb, row_ptr, _stream())
 
 
 def ring_write_advance(plan, row_ptr, T, ticket, size_ptr=None):
     """ring_write(plan, row_ptr) then row_ptr = (row_ptr + 1) % T [, size = min(size + 1, T)] in one launch.
     ticket: a zero-initialised int32[1] owned by the caller."""
-    _lib.call("trl_ring_write_advance", plan.n, plan.src, plan.dst, plan.rb, _chk(row_ptr, I32, "row_ptr"), int(T),
-              _opt(size_ptr, I32, "size_ptr"), _chk(ticket, I32, "ticket"), _stream())
+    _lib.call("trl_ring_write_advance", plan.n, plan.src, plan.dst, plan.rb, row_ptr, int(T), size_ptr, ticket,
+              _stream())
 
 
 def vec_stats(x, out=None):
     """[mean, unbiased std, max, min] of a float vector, on the device."""
     if out is None:
         out = torch.empty(4, dtype=F32, device=x.device)
-    _lib.call("trl_vec_stats", _chk(x, F32, "x"), x.numel(), _chk(out, F32, "stats"), _stream())
+    _lib.call("trl_vec_stats", x, x.numel(), out, _stream())
     return out
 
 
 def vec_moments(x, out):
     """out (4) f64 = sum, sum of squares, max, -min of a float vector: one rank's share of vec_stats."""
-    _lib.call("trl_vec_moments", _chk(x, F32, "x"), x.numel(), _chk(out, F64, "moments"), _stream())
+    _lib.call("trl_vec_moments", x, x.numel(), out, _stream())
     return out
 
 
 def vec_stats_from_moments(gathered, world, n_total, out):
     """out (4) f32 = mean, unbiased std, max, min from `world` ranks' vec_moments, (world, 4) f64."""
-    _lib.call("trl_vec_stats_from_moments", _chk(gathered, F64, "moments"), int(world), float(n_total),
-              _chk(out, F32, "stats"), _stream())
+    _lib.call("trl_vec_stats_from_moments", gathered, int(world), float(n_total), out, _stream())
     return out
 
 
@@ -284,13 +251,9 @@ def ppo_actor_loss(mean, log_std, actions, old_logp, advs, adv_stats, clip_para,
         g_log_std = torch.empty_like(log_std)
     if info is None:
         info = torch.zeros(16, dtype=F32, device=mean.device)
-    _lib.call("trl_ppo_actor_loss", _chk(mean, F32, "mean"), _chk(log_std, F32, "log_std"), ls_stride,
-              _chk(actions, F32, "actions"), _opt(old_logp, F32, "old_logp"), _chk(advs, F32, "advs"),
-              _opt(adv_stats, F32, "adv_stats"), _opt(stats_pos, I32, "stats_pos"), B, a, int(bool(tanh_action)),
-              float(clip_para),
-              float(entropy_coeff), ls_lo, ls_hi, _chk(g_mean, F32, "g_mean"), _chk(g_log_std, F32, "g_log_std"),
-              _opt(logp_out, F32, "logp_out"), _chk(info, F32, "info"), _chk(scratch.actor, F64, "scratch"),
-              _chk(scratch.tickets[0:1], I32, "ticket"), _stream())
+    _lib.call("trl_ppo_actor_loss", mean, log_std, ls_stride, actions, old_logp, advs, adv_stats, stats_pos, B, a,
+              int(bool(tanh_action)), float(clip_para), float(entropy_coeff), ls_lo, ls_hi, g_mean, g_log_std, logp_out,
+              info, scratch.actor, scratch.tickets[0:1], _stream())
     return g_mean, g_log_std, info
 
 
@@ -301,10 +264,8 @@ def ppo_critic_loss(values, returns, old_values, clipped, clip_para, scratch, g_
         g_values = torch.empty_like(values)
     if info is None:
         info = torch.zeros(1, dtype=F32, device=values.device)
-    _lib.call("trl_ppo_critic_loss", _chk(values, F32, "values"), _chk(returns, F32, "returns"),
-              _opt(old_values, F32, "old_values"), B, int(bool(clipped)), float(clip_para),
-              _chk(g_values, F32, "g_values"), _chk(info, F32, "info"), _chk(scratch.critic, F64, "scratch"),
-              _chk(scratch.tickets[1:2], I32, "ticket"), _stream())
+    _lib.call("trl_ppo_critic_loss", values, returns, old_values, B, int(bool(clipped)), float(clip_para), g_values,
+              info, scratch.critic, scratch.tickets[1:2], _stream())
     return g_values, info
 
 
@@ -313,8 +274,7 @@ def gaussian_log_prob(mean, log_std, actions, tanh_action, out=None):
     if out is None:
         out = torch.empty(B, dtype=F32, device=mean.device)
     ls_stride = 0 if log_std.dim() == 1 else a
-    _lib.call("trl_gaussian_log_prob", _chk(mean, F32, "mean"), _chk(log_std, F32, "log_std"), ls_stride,
-              _chk(actions, F32, "actions"), B, a, int(bool(tanh_action)), _chk(out, F32, "logp"), _stream())
+    _lib.call("trl_gaussian_log_prob", mean, log_std, ls_stride, actions, B, a, int(bool(tanh_action)), out, _stream())
     return out
 
 
@@ -333,9 +293,7 @@ def categorical_sample(logits, u=None, rng=None, action_out=None, want_log_prob=
         if rng is None or rng.counter is None:
             raise ValueError("categorical_sample needs either u or an rng state")
         seed, ctr = rng.seed, rng.counter
-    _lib.call("trl_categorical_sample", _chk(logits, F32, "logits"), _opt(u, F32, "u"), ctypes.c_uint64(seed),
-              _opt(ctr, I64, "rng_counter"), M, A, _chk(action, F32, "action"), _opt(logp, F32, "log_prob"),
-              _opt(nan_flag, I32, "nan_flag"), _stream())
+    _lib.call("trl_categorical_sample", logits, u, ctypes.c_uint64(seed), ctr, M, A, action, logp, nan_flag, _stream())
     return (action, logp) if want_log_prob else action
 
 
@@ -346,8 +304,7 @@ def categorical_log_prob(logits, actions, out=None):
     if out is None:
         out = torch.empty(M, dtype=F32, device=logits.device)
     assert actions.numel() == M and out.numel() == M
-    _lib.call("trl_categorical_log_prob", _chk(logits, F32, "logits"), _chk(actions, F32, "actions"), M, A,
-              _chk(out, F32, "logp"), _stream())
+    _lib.call("trl_categorical_log_prob", logits, actions, M, A, out, _stream())
     return out
 
 
@@ -362,11 +319,9 @@ def ppo_categorical_actor_loss(logits, actions, old_logp, advs, adv_stats, clip_
         g_logits = torch.empty_like(logits)
     if info is None:
         info = torch.zeros(16, dtype=F32, device=logits.device)
-    _lib.call("trl_ppo_categorical_actor_loss", _chk(logits, F32, "logits"), _chk(actions, F32, "actions"),
-              _opt(old_logp, F32, "old_logp"), _chk(advs, F32, "advs"), _opt(adv_stats, F32, "adv_stats"),
-              _opt(stats_pos, I32, "stats_pos"), B, A, float(clip_para), float(entropy_coeff),
-              _chk(g_logits, F32, "g_logits"), _opt(logp_out, F32, "logp_out"), _chk(info, F32, "info"),
-              _chk(scratch.actor, F64, "scratch"), _chk(scratch.tickets[0:1], I32, "ticket"), _stream())
+    _lib.call("trl_ppo_categorical_actor_loss", logits, actions, old_logp, advs, adv_stats, stats_pos, B, A,
+              float(clip_para), float(entropy_coeff), g_logits, logp_out, info, scratch.actor, scratch.tickets[0:1],
+              _stream())
     return g_logits, info
 
 
@@ -385,8 +340,7 @@ def vmpo_select(advs, stats, groups, b, perm=None, out=None):
         out = torch.empty(groups, B - B // 2, dtype=I64, device=advs.device)
     if out.numel() != groups * (B - B // 2):
         raise ValueError("vmpo_select: out must hold (groups, B - B // 2) positions")
-    _lib.call("trl_vmpo_select", _chk(advs, F32, "advs"), _opt(perm, I64, "perm"), int(groups), int(b), int(n),
-              _chk(stats, F32, "stats"), _chk(out, I64, "sel"), _stream())
+    _lib.call("trl_vmpo_select", advs, perm, int(groups), int(b), int(n), stats, out, _stream())
     return out
 
 
@@ -415,12 +369,9 @@ def vmpo_categorical_loss(logits, target_logits, actions, advs, adv_stats, dual,
         raise ValueError("vmpo_categorical_loss: scratch sized for %d rows, got %d" % (scratch.k, k))
     if g_logits is None:
         g_logits = torch.empty_like(logits)
-    _lib.call("trl_vmpo_categorical_loss", _chk(logits, F32, "logits"), _chk(target_logits, F32, "target_logits"),
-              _chk(actions, F32, "actions"), _chk(advs, F32, "advs"), _chk(adv_stats, F32, "adv_stats"),
-              _opt(stats_pos, I32, "stats_pos"), _chk(dual, F32, "dual"), int(k), int(A), float(eta_eps),
-              float(alpha_eps), int(bool(per_row_kl)), _chk(g_logits, F32, "g_logits"), _chk(g_dual, F32, "g_dual"),
-              _chk(info, F32, "info"), _chk(scratch.partial, F64, "scratch"), _chk(scratch.ticket, I32, "ticket"),
-              _stream())
+    _lib.call("trl_vmpo_categorical_loss", logits, target_logits, actions, advs, adv_stats, stats_pos, dual, int(k),
+              int(A), float(eta_eps), float(alpha_eps), int(bool(per_row_kl)), g_logits, g_dual, info, scratch.partial,
+              scratch.ticket, _stream())
     return g_logits
 
 
@@ -436,8 +387,7 @@ def categorical_fisher_vp(logits, tangent, scale, out=None):
         out = torch.empty_like(logits)
     if out.shape != logits.shape:
         raise ValueError("categorical_fisher_vp: out must have the shape of logits")
-    _lib.call("trl_categorical_fisher_vp", _chk(logits, F32, "logits"), _chk(tangent, F32, "tangent"), M, A,
-              float(scale), _chk(out, F32, "g_logits"), _stream())
+    _lib.call("trl_categorical_fisher_vp", logits, tangent, M, A, float(scale), out, _stream())
     return out
 
 
@@ -453,8 +403,7 @@ def tangent_bias_act(t, bias_tangent, y, act):
         raise ValueError("tangent_bias_act: bias_tangent must hold one value per channel (%d)" % C)
     if act != 0 and (y is None or y.shape != t.shape):
         raise ValueError("tangent_bias_act: y must have the shape of t")
-    _lib.call("trl_tangent_bias_act", _chk(t, F32, "t"), _chk(bias_tangent, F32, "bias_tangent"),
-              _opt(y if act != 0 else None, F32, "y"), M, C, S, int(act), _stream())
+    _lib.call("trl_tangent_bias_act", t, bias_tangent, y if act != 0 else None, M, C, S, int(act), _stream())
     return t
 
 
@@ -478,9 +427,8 @@ def categorical_surrogate(logits, actions, logp_old, advn, scratch, out=None):
         raise ValueError("categorical_surrogate: scratch sized for %d rows, got %d" % (scratch.M, M))
     if out is None:
         out = torch.empty(1, dtype=F32, device=logits.device)
-    _lib.call("trl_categorical_surrogate", _chk(logits, F32, "logits"), _chk(actions, F32, "actions"),
-              _chk(logp_old, F32, "logp_old"), _chk(advn, F32, "advn"), M, A, _chk(out, F32, "out"),
-              _chk(scratch.partial, F64, "scratch"), _chk(scratch.ticket, I32, "ticket"), _stream())
+    _lib.call("trl_categorical_surrogate", logits, actions, logp_old, advn, M, A, out, scratch.partial, scratch.ticket,
+              _stream())
     return out
 
 
@@ -489,8 +437,7 @@ def row_group_moments(x, idx, groups, b, out=None):
     n = x.numel() // x.shape[0]
     if out is None:
         out = torch.empty(groups, 4, dtype=F64, device=x.device)
-    _lib.call("trl_row_group_moments", _chk(x, F32, "x"), _chk(idx, I64, "idx"), int(groups), int(b), n,
-              _chk(out, F64, "moments"), _stream())
+    _lib.call("trl_row_group_moments", x, idx, int(groups), int(b), n, out, _stream())
     return out
 
 
@@ -498,8 +445,7 @@ def group_stats_from_moments(gathered, world, groups, n_total, out=None):
     """out (groups,4) f32 = mean, unbiased std, max, min per group from (world, groups, 4) raw moments."""
     if out is None:
         out = torch.empty(groups, 4, dtype=F32, device=gathered.device)
-    _lib.call("trl_group_stats_from_moments", _chk(gathered, F64, "moments"), int(world), int(groups), float(n_total),
-              _chk(out, F32, "stats"), _stream())
+    _lib.call("trl_group_stats_from_moments", gathered, int(world), int(groups), float(n_total), out, _stream())
     return out
 
 
@@ -508,8 +454,7 @@ def polyak_update(target_flat, source_flat, tau, planes=None):
     """target <- (1 - tau) target + tau source on flat buffers; planes = (hi, lo) flat TF32 planes of the target
     kept current in the same pass (flat.FlatParams.hi / .lo)."""
     hi, lo = planes if planes is not None else (None, None)
-    _lib.call("trl_polyak_update", _chk(target_flat, F32, "target"), _chk(source_flat, F32, "source"),
-              target_flat.numel(), float(tau), _opt(hi, F32, "hi"), _opt(lo, F32, "lo"), _stream())
+    _lib.call("trl_polyak_update", target_flat, source_flat, target_flat.numel(), float(tau), hi, lo, _stream())
 
 
 def grad_sumsq_blocks(nseg):
@@ -520,19 +465,16 @@ def grad_sumsq_blocks(nseg):
 def grad_sumsq(grad, seg_begin, nseg, mask, sumsq3, step_counts, betas, scratch, ticket):
     """Per-segment sum of squares of the flat gradient, Adam step counts and bias corrections into sumsq3 (3 nseg f64)
     for the active segments of `mask`.  seg_begin: host int64 array of the nseg + 1 segment offsets."""
-    _lib.call("trl_grad_sumsq", _chk(grad, F32, "grad"), seg_begin, int(nseg), int(mask), _chk(sumsq3, F64, "sumsq3"),
-              _chk(step_counts, I32, "step_counts"), float(betas[0]), float(betas[1]), _chk(scratch, F64, "scratch"),
-              _chk(ticket, I32, "ticket"), _stream())
+    _lib.call("trl_grad_sumsq", grad, seg_begin, int(nseg), int(mask), sumsq3, step_counts, float(betas[0]),
+              float(betas[1]), scratch, ticket, _stream())
 
 
 def adam_step(param, grad, exp_avg, exp_avg_sq, seg_begin, nseg, mask, sumsq3, lr, max_norm, eps, betas, grad_scale,
               zero_grad, hi, lo):
     """Clip (per segment, by the norms in sumsq3) + Adam on the flat buffers, optionally zeroing `grad`; hi / lo: the
     TF32 planes of `param` kept current.  seg_begin / max_norm / eps: host arrays (int64, float, float)."""
-    _lib.call("trl_adam_step", _chk(param, F32, "param"), _chk(grad, F32, "grad"), _chk(exp_avg, F32, "exp_avg"),
-              _chk(exp_avg_sq, F32, "exp_avg_sq"), seg_begin, int(nseg), int(mask), _chk(sumsq3, F64, "sumsq3"),
-              _chk(lr, F32, "lr"), max_norm, eps, float(betas[0]), float(betas[1]), float(grad_scale),
-              int(bool(zero_grad)), _chk(hi, F32, "hi"), _chk(lo, F32, "lo"), _stream())
+    _lib.call("trl_adam_step", param, grad, exp_avg, exp_avg_sq, seg_begin, int(nseg), int(mask), sumsq3, lr, max_norm,
+              eps, float(betas[0]), float(betas[1]), float(grad_scale), int(bool(zero_grad)), hi, lo, _stream())
 
 
 # ------------------------------------------------------------------------------------------ K10
@@ -546,10 +488,10 @@ class OffPolicyScratch:
         self.B = int(B)
 
     def t(self, i):
-        return _chk(self.tickets[i:i + 1], I32, "ticket")
+        return self.tickets[i:i + 1]
 
     def b(self, i):
-        return _chk(self.buf[i], F64, "scratch")
+        return self.buf[i]
 
 
 def td_target(rewards, terminals, q1_next, q2_next, logp_next, log_alpha, gamma, scratch, y=None, info=None,
@@ -561,10 +503,8 @@ def td_target(rewards, terminals, q1_next, q2_next, logp_next, log_alpha, gamma,
         y = torch.empty(B, dtype=F32, device=rewards.device)
     if info is None:
         info = torch.zeros(1, dtype=F32, device=rewards.device)
-    _lib.call("trl_td_target", _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"),
-              _chk(q1_next, F32, "q1_next"), _opt(q2_next, F32, "q2_next"), _opt(logp_next, F32, "logp_next"),
-              _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha), float(gamma), B, _chk(y, F32, "y"),
-              _chk(info, F32, "info"), scratch.b(0), scratch.t(0), _stream())
+    _lib.call("trl_td_target", rewards, terminals, q1_next, q2_next, logp_next, log_alpha, float(fixed_alpha),
+              float(gamma), B, y, info, scratch.b(0), scratch.t(0), _stream())
     return y, info
 
 
@@ -575,9 +515,8 @@ def td3_smooth_action(action, sigma, noise_clip, eps=None, rng=None, out=None):
     seed, ctr = (0, None)
     if eps is None:
         seed, ctr = rng.seed, rng.counter
-    _lib.call("trl_td3_smooth_action", _chk(action, F32, "action"), _opt(eps, F32, "eps"), float(sigma),
-              float(noise_clip), ctypes.c_uint64(seed), _opt(ctr, I64, "rng_counter"), action.numel(),
-              _chk(out, F32, "out"), _stream())
+    _lib.call("trl_td3_smooth_action", action, eps, float(sigma), float(noise_clip), ctypes.c_uint64(seed), ctr,
+              action.numel(), out, _stream())
     return out
 
 
@@ -585,9 +524,8 @@ def sac_alpha_step(logp, target_entropy, log_alpha, adam_state, lr, scratch, inf
     """Temperature loss and its Adam step in one launch (twin_sac_q.py:111-123); info = [alpha, alpha_loss]."""
     if info is None:
         info = torch.zeros(2, dtype=F32, device=logp.device)
-    _lib.call("trl_sac_alpha_step", _chk(logp, F32, "logp"), float(target_entropy), _chk(log_alpha, F32, "log_alpha"),
-              _chk(adam_state, F32, "adam_state"), float(lr), float(betas[0]), float(betas[1]), float(eps),
-              logp.numel(), _chk(info, F32, "info"), scratch.b(1), scratch.t(1), _stream())
+    _lib.call("trl_sac_alpha_step", logp, float(target_entropy), log_alpha, adam_state, float(lr), float(betas[0]),
+              float(betas[1]), float(eps), logp.numel(), info, scratch.b(1), scratch.t(1), _stream())
     return info
 
 
@@ -597,9 +535,7 @@ def sac_policy_loss(logp, q1, q2, log_alpha, scratch, info=None, fixed_alpha=1.0
     g_lp, g1, g2 = torch.empty_like(logp), torch.empty_like(q1), torch.empty_like(q2)
     if info is None:
         info = torch.zeros(5, dtype=F32, device=logp.device)
-    _lib.call("trl_sac_policy_loss", _chk(logp, F32, "logp"), _chk(q1, F32, "q1"), _chk(q2, F32, "q2"),
-              _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha), B, _chk(g_lp, F32, "g_logp"),
-              _chk(g1, F32, "g_q1"), _chk(g2, F32, "g_q2"), _chk(info, F32, "info"), scratch.b(2),
+    _lib.call("trl_sac_policy_loss", logp, q1, q2, log_alpha, float(fixed_alpha), B, g_lp, g1, g2, info, scratch.b(2),
               scratch.t(2), _stream())
     return g_lp, g1, g2, info
 
@@ -613,11 +549,8 @@ def sac_v_loss(logp, qn1, qn2, v_pred, log_alpha, scratch, reparameterization=Tr
     g2 = torch.empty_like(qn2) if qn2 is not None else None
     if info is None:
         info = torch.zeros(6, dtype=F32, device=logp.device)
-    _lib.call("trl_sac_v_loss", _chk(logp, F32, "logp"), _chk(qn1, F32, "qn1"), _opt(qn2, F32, "qn2"),
-              _chk(v_pred, F32, "v_pred"), _opt(log_alpha, F32, "log_alpha"), float(fixed_alpha),
-              int(bool(reparameterization)), B, _chk(g_lp, F32, "g_logp"), _chk(g1, F32, "g_qn1"),
-              _opt(g2, F32, "g_qn2"), _chk(g_v, F32, "g_v"), _chk(info, F32, "info"), scratch.b(2),
-              scratch.t(5), _stream())
+    _lib.call("trl_sac_v_loss", logp, qn1, qn2, v_pred, log_alpha, float(fixed_alpha), int(bool(reparameterization)), B,
+              g_lp, g1, g2, g_v, info, scratch.b(2), scratch.t(5), _stream())
     return g_lp, g1, g2, g_v, info
 
 
@@ -628,9 +561,7 @@ def twin_mse_loss(q1, q2, y, scratch, info=None):
     g2 = torch.empty_like(q2) if q2 is not None else None
     if info is None:
         info = torch.zeros(2, dtype=F32, device=q1.device)
-    _lib.call("trl_twin_mse_loss", _chk(q1, F32, "q1"), _opt(q2, F32, "q2"), _chk(y, F32, "y"), B,
-              _chk(g1, F32, "g1"), _opt(g2, F32, "g2"), _chk(info, F32, "info"), scratch.b(3),
-              scratch.t(3), _stream())
+    _lib.call("trl_twin_mse_loss", q1, q2, y, B, g1, g2, info, scratch.b(3), scratch.t(3), _stream())
     return g1, g2, info
 
 
@@ -646,9 +577,8 @@ def twin_mse_loss_weighted(q1, q2, y, weights, scratch, info=None, td_out=None):
         raise ValueError("weights has %d elements for a batch of %d" % (weights.numel(), B))
     if td_out is not None and td_out.numel() != B * (1 if q2 is None else 2):
         raise ValueError("td_out has %d elements, want %d" % (td_out.numel(), B * (1 if q2 is None else 2)))
-    _lib.call("trl_twin_mse_loss_weighted", _chk(q1, F32, "q1"), _opt(q2, F32, "q2"), _chk(y, F32, "y"),
-              _opt(weights, F32, "weights"), B, _chk(g1, F32, "g1"), _opt(g2, F32, "g2"), _opt(td_out, F32, "td_out"),
-              _chk(info, F32, "info"), scratch.b(3), scratch.t(3), _stream())
+    _lib.call("trl_twin_mse_loss_weighted", q1, q2, y, weights, B, g1, g2, td_out, info, scratch.b(3), scratch.t(3),
+              _stream())
     return g1, g2, info
 
 
@@ -660,11 +590,8 @@ def qr_dqn_loss(pred, nxt, actions, rewards, terminals, gamma, scratch, n_action
     grad = torch.empty_like(pred)
     if info is None:
         info = torch.zeros(3, dtype=F32, device=pred.device)
-    _lib.call("trl_qr_dqn_loss", _chk(pred, F32, "pred"), _chk(nxt, F32, "next"), _chk(actions, F32, "actions"),
-              _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"), _opt(weights, F32, "weights"), B,
-              int(n_actions), int(n_quantiles), float(gamma), float(kappa), int(bool(mse)), _chk(grad, F32, "grad"),
-              _opt(td_out, F32, "td_out"), _chk(info, F32, "info"),
-              scratch.b(4), scratch.t(4), _stream())
+    _lib.call("trl_qr_dqn_loss", pred, nxt, actions, rewards, terminals, weights, B, int(n_actions), int(n_quantiles),
+              float(gamma), float(kappa), int(bool(mse)), grad, td_out, info, scratch.b(4), scratch.t(4), _stream())
     return grad, info
 
 
@@ -677,10 +604,8 @@ def bootstrapped_dqn_loss(pred, nxt, actions, rewards, terminals, masks, gamma, 
         grad = torch.empty_like(pred)
     if info is None:
         info = torch.zeros(3, dtype=F32, device=pred.device)
-    _lib.call("trl_bootstrapped_dqn_loss", _chk(pred, F32, "pred"), _chk(nxt, F32, "next"),
-              _chk(actions, F32, "actions"), _chk(rewards, F32, "rewards"), _chk(terminals, U8, "terminals"),
-              _chk(masks, U8, "masks"), B, H, A, float(gamma), _chk(grad, F32, "grad"), _chk(info, F32, "info"),
-              scratch.b(4), scratch.t(4), _stream())
+    _lib.call("trl_bootstrapped_dqn_loss", pred, nxt, actions, rewards, terminals, masks, B, H, A, float(gamma), grad,
+              info, scratch.b(4), scratch.t(4), _stream())
     return grad, info
 
 
@@ -696,10 +621,8 @@ def bootstrapped_act(q_all, current_step, head, action, masks_ring, top, bernoul
         if rng is None or rng.counter is None or ticket is None:
             raise ValueError("bootstrapped_act needs u_head / u_mask or an rng state and a ticket")
         seed, ctr = rng.seed, rng.counter
-    _lib.call("trl_bootstrapped_act", _chk(q_all, F32, "q_all"), _chk(current_step, I32, "current_step"),
-              _chk(head, I32, "head"), _chk(action, F32, "action"), _chk(masks_ring, U8, "masks_ring"),
-              _chk(top, I32, "top"), _opt(u_head, F32, "u_head"), _opt(u_mask, F32, "u_mask"), ctypes.c_uint64(seed),
-              _opt(ctr, I64, "rng_counter"), _opt(ticket, I32, "ticket"), N, H, A, float(bernoulli_p), _stream())
+    _lib.call("trl_bootstrapped_act", q_all, current_step, head, action, masks_ring, top, u_head, u_mask,
+              ctypes.c_uint64(seed), ctr, ticket, N, H, A, float(bernoulli_p), _stream())
     return action
 
 
@@ -711,8 +634,7 @@ def per_sample(prio, size, u, beta, idx=None, weights=None):
         idx = torch.empty(b, dtype=I64, device=prio.device)
     if weights is None:
         weights = torch.empty(b, dtype=F32, device=prio.device)
-    _lib.call("trl_per_sample", _chk(prio, F32, "prio"), int(size), _chk(u, F64, "u"), b, float(beta),
-              _chk(idx, I64, "idx"), _chk(weights, F32, "weights"), _stream())
+    _lib.call("trl_per_sample", prio, int(size), u, b, float(beta), idx, weights, _stream())
     return idx, weights
 
 
@@ -736,9 +658,8 @@ def per_sample_rows(prio, size_ptr, u, pos_ptr, b, beta, scratch, idx, weights):
                                                                                  per_scratch_doubles(capacity)))
     if idx.numel() != b or weights.numel() != b:
         raise ValueError("per_sample_rows: idx / weights must hold b = %d elements" % b)
-    _lib.call("trl_per_sample_rows", _chk(prio, F32, "prio"), capacity, _chk(size_ptr, I32, "size_ptr"),
-              _chk(u, F64, "u"), _chk(pos_ptr, I32, "pos_ptr"), int(b), float(beta), _chk(idx, I64, "idx"),
-              _chk(weights, F32, "weights"), _chk(scratch, F64, "scratch"), _stream(), kernels=2)
+    _lib.call("trl_per_sample_rows", prio, capacity, size_ptr, u, pos_ptr, int(b), float(beta), idx, weights, scratch,
+              _stream(), kernels=2)
     return idx, weights
 
 
@@ -747,13 +668,11 @@ def per_update(prio, idx, td, alpha, eps, max_prio):
     priority."""
     b = idx.numel()
     n = td.numel() // b
-    _lib.call("trl_per_update", _chk(prio, F32, "prio"), _chk(idx, I64, "idx"), _chk(td, F32, "td"), b, n,
-              float(alpha), float(eps), _chk(max_prio, F32, "max_prio"), _stream())
+    _lib.call("trl_per_update", prio, idx, td, b, n, float(alpha), float(eps), max_prio, _stream())
 
 
 def per_insert(prio, row_ptr, max_prio):
-    _lib.call("trl_per_insert", _chk(prio, F32, "prio"), _chk(row_ptr, I32, "row_ptr"), _chk(max_prio, F32, "max_prio"),
-              _stream())
+    _lib.call("trl_per_insert", prio, row_ptr, max_prio, _stream())
 
 
 # ------------------------------------------------------------------------------------------ tensor-core GEMM
@@ -766,8 +685,7 @@ def gemm_tf32x3_nt(a, b, out=None, splits=1, workspace=None, bias=None, act=0):
         out = torch.empty(M, 256, dtype=F32, device=a.device)
     if splits > 1 and workspace is None:
         workspace = torch.empty(splits * M * 256, dtype=F32, device=a.device)
-    _lib.call("trl_gemm_tf32x3_nt", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K, int(splits),
-              _opt(workspace, F32, "workspace"), _opt(bias, F32, "bias"), int(act), _stream(),
+    _lib.call("trl_gemm_tf32x3_nt", a, b, out, M, K, int(splits), workspace, bias, int(act), _stream(),
               kernels=2 if splits > 1 else 1)       # + the split-K reduction
     return out
 
@@ -781,8 +699,7 @@ def gemm_tf32x3_tn(a, b, out=None, splits=1, workspace=None):
         out = torch.empty(M, 256, dtype=F32, device=a.device)
     if splits > 1 and workspace is None:
         workspace = torch.empty(splits * M * 256, dtype=F32, device=a.device)
-    _lib.call("trl_gemm_tf32x3_tn", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K, int(splits),
-              _opt(workspace, F32, "workspace"), _stream(), kernels=2 if splits > 1 else 1)
+    _lib.call("trl_gemm_tf32x3_tn", a, b, out, M, K, int(splits), workspace, _stream(), kernels=2 if splits > 1 else 1)
     return out
 
 
@@ -794,14 +711,9 @@ def gemm3_pair(a, b, out=None, planes=None, b_nmajor=False, bias=None, act=0):
     assert tuple(b.shape) == ((K, 256) if b_nmajor else (256, K)), "B must be (K,256) if b_nmajor else (256,K)"
     if out is None:
         out = torch.empty(M, 256, dtype=F32, device=a.device)
-    if planes is not None:
-        hi, lo = planes
-        assert hi.shape == b.shape and lo.shape == b.shape
-        bh, bl = _chk(hi, F32, "b_hi"), _chk(lo, F32, "b_lo")
-    else:
-        bh, bl = _chk(b, F32, "b"), None
-    _lib.call("trl_gemm3_pair", _chk(a, F32, "a"), bh, bl, _chk(out, F32, "out"), M, K, int(bool(b_nmajor)),
-              _opt(bias, F32, "bias"), int(act), _stream())
+    bh, bl = planes if planes is not None else (b, None)
+    assert bh.shape == b.shape and (bl is None or bl.shape == b.shape)
+    _lib.call("trl_gemm3_pair", a, bh, bl, out, M, K, int(bool(b_nmajor)), bias, int(act), _stream())
     return out
 
 
@@ -813,8 +725,7 @@ def gemm3_pair_tn(a, b, out=None, splits=1, workspace=None):
         out = torch.empty(M, 256, dtype=F32, device=a.device)
     if splits > 1 and workspace is None:
         workspace = torch.empty(splits * M * 256, dtype=F32, device=a.device)
-    _lib.call("trl_gemm3_pair_tn", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K, int(splits),
-              _opt(workspace, F32, "workspace"), _stream(), kernels=2 if splits > 1 else 1)
+    _lib.call("trl_gemm3_pair_tn", a, b, out, M, K, int(splits), workspace, _stream(), kernels=2 if splits > 1 else 1)
     return out
 
 
@@ -826,8 +737,7 @@ def gemm3_pair_tn_cluster(a, b, workspace, tickets, out=None, splits=64):
     assert workspace.numel() >= 8 * M * 256 and tickets.numel() >= M // 8, "workspace / tickets too small"
     if out is None:
         out = torch.empty(M, 256, dtype=F32, device=a.device)
-    _lib.call("trl_gemm3_pair_tn_cluster", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), M, K,
-              int(splits), _chk(workspace, F32, "workspace"), _chk(tickets, torch.int32, "tickets"), _stream())
+    _lib.call("trl_gemm3_pair_tn_cluster", a, b, out, M, K, int(splits), workspace, tickets, _stream())
     return out
 
 
@@ -839,8 +749,7 @@ def gemm3_pair_dgrad_act_wgrad(g, planes_t, h1, x, act, scratch):
     M, K = x.shape
     hi, lo = planes_t
     assert g.shape == (M, 256) and h1.shape == (M, 256) and hi.shape == (256, 256) and lo.shape == (256, 256)
-    _lib.call("trl_gemm3_pair_dgrad_act_wgrad", _chk(g, F32, "g"), _chk(hi, F32, "w_hi_t"), _chk(lo, F32, "w_lo_t"),
-              _chk(h1, F32, "h1"), _chk(x, F32, "x"), M, K, int(act), _chk(scratch, F32, "scratch"), _stream())
+    _lib.call("trl_gemm3_pair_dgrad_act_wgrad", g, hi, lo, h1, x, M, K, int(act), scratch, _stream())
     return scratch
 
 
@@ -852,9 +761,7 @@ def skinny_n_dgrad_act_wgrad_partial(g, w, y, act, gz, db_scratch, w_scratch):
     M, H = y.shape
     N = w.shape[0]
     assert g.shape == (M, N) and w.shape == (N, H) and gz.shape == (M, H)
-    _lib.call("trl_skinny_n_dgrad_act_wgrad_partial", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
-              _chk(gz, F32, "gz"), M, H, N, int(act), _chk(db_scratch, F32, "db_scratch"),
-              _chk(w_scratch, F32, "w_scratch"), _stream())
+    _lib.call("trl_skinny_n_dgrad_act_wgrad_partial", g, w, y, gz, M, H, N, int(act), db_scratch, w_scratch, _stream())
 
 
 def skinny_n_dgrad_act_wgrad(g, w, y, act, gz, db, dw, dbias, db_scratch, w_scratch):
@@ -863,9 +770,8 @@ def skinny_n_dgrad_act_wgrad(g, w, y, act, gz, db, dw, dbias, db_scratch, w_scra
     N = w.shape[0]
     assert g.shape == (M, N) and w.shape == (N, H) and gz.shape == (M, H)
     assert db.shape == (H,) and dw.shape == (N, H) and dbias.shape == (N,)
-    _lib.call("trl_skinny_n_dgrad_act_wgrad", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
-              _chk(gz, F32, "gz"), _chk(db, F32, "db"), _chk(dw, F32, "dw"), _chk(dbias, F32, "dbias"), M, H, N,
-              int(act), _chk(db_scratch, F32, "db_scratch"), _chk(w_scratch, F32, "w_scratch"), _stream(), kernels=2)
+    _lib.call("trl_skinny_n_dgrad_act_wgrad", g, w, y, gz, db, dw, dbias, M, H, N, int(act), db_scratch, w_scratch,
+              _stream(), kernels=2)
 
 
 def transpose_f32(x, out=None):
@@ -873,7 +779,7 @@ def transpose_f32(x, out=None):
     R, C = x.shape
     if out is None:
         out = torch.empty(C, R, dtype=F32, device=x.device)
-    _lib.call("trl_transpose_f32", _chk(x, F32, "x"), _chk(out, F32, "out"), R, C, _stream())
+    _lib.call("trl_transpose_f32", x, out, R, C, _stream())
     return out
 
 
@@ -882,8 +788,7 @@ def split_tf32(x, hi=None, lo=None):
     hi = torch.empty_like(x) if hi is None else hi
     lo = torch.empty_like(x) if lo is None else lo
     assert hi.numel() == x.numel() and lo.numel() == x.numel()
-    _lib.call("trl_split_tf32", _chk(x, F32, "x"), x.numel(), _chk(hi, F32, "hi"), _chk(lo, F32, "lo"), _stream(),
-              kernels=int(x.numel() > 0))
+    _lib.call("trl_split_tf32", x, x.numel(), hi, lo, _stream(), kernels=int(x.numel() > 0))
     return hi, lo
 
 
@@ -895,8 +800,7 @@ def bias_act_bwd_scratch_floats(M, H):
 def bias_act_fwd(z, bias, act):
     """z (M,H) <- act(z + bias) in place."""
     M, H = z.shape
-    _lib.call("trl_bias_act_fwd", _chk(z, F32, "z"), _chk(bias, F32, "bias"), M, H, int(act), _stream(),
-              kernels=int(M > 0))
+    _lib.call("trl_bias_act_fwd", z, bias, M, H, int(act), _stream(), kernels=int(M > 0))
     return z
 
 
@@ -904,8 +808,7 @@ def bias_act_bwd(g, y, gz, db, act, scratch, tickets):
     """gz = g * act'(y) and db = colsum(gz) for y (M,H); scratch: bias_act_bwd_scratch_floats(M, H) floats, tickets:
     (H + 127) // 128 zeroed int32 (left zero)."""
     M, H = y.shape
-    _lib.call("trl_bias_act_bwd", _chk(g, F32, "g"), _chk(y, F32, "y"), _chk(gz, F32, "gz"), _chk(db, F32, "db"), M, H,
-              int(act), _chk(scratch, F32, "scratch"), _chk(tickets, I32, "tickets"), _stream())
+    _lib.call("trl_bias_act_bwd", g, y, gz, db, M, H, int(act), scratch, tickets, _stream())
 
 
 # ------------------------------------------------------------------------------------------ skinny layers
@@ -926,8 +829,7 @@ def skinny_k_fwd(x, w, bias, act, out=None):
     H = w.shape[0]
     if out is None:
         out = torch.empty(M, H, dtype=F32, device=x.device)
-    _lib.call("trl_skinny_k_fwd", _chk(x, F32, "x"), _chk(w, F32, "w"), _chk(bias, F32, "bias"), _chk(out, F32, "out"),
-              M, K, H, int(act), _stream())
+    _lib.call("trl_skinny_k_fwd", x, w, bias, out, M, K, H, int(act), _stream())
     return out
 
 
@@ -937,8 +839,7 @@ def skinny_n_fwd(x, w, bias, out=None):
     N = w.shape[0]
     if out is None:
         out = torch.empty(M, N, dtype=F32, device=x.device)
-    _lib.call("trl_skinny_n_fwd", _chk(x, F32, "x"), _chk(w, F32, "w"), _chk(bias, F32, "bias"), _chk(out, F32, "out"),
-              M, H, N, _stream())
+    _lib.call("trl_skinny_n_fwd", x, w, bias, out, M, H, N, _stream())
     return out
 
 
@@ -948,7 +849,7 @@ def skinny_n_dgrad(g, w, out=None):
     N, H = w.shape
     if out is None:
         out = torch.empty(M, H, dtype=F32, device=g.device)
-    _lib.call("trl_skinny_n_dgrad", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(out, F32, "dx"), M, H, N, _stream())
+    _lib.call("trl_skinny_n_dgrad", g, w, out, M, H, N, _stream())
     return out
 
 
@@ -957,8 +858,7 @@ def skinny_tn(a, b, out, colsum, out_transposed, scratch):
     scratch: skinny_tn_scratch_floats(M, H, K) floats."""
     M, H = a.shape
     K = b.shape[1]
-    _lib.call("trl_skinny_tn", _chk(a, F32, "a"), _chk(b, F32, "b"), _chk(out, F32, "out"), _opt(colsum, F32, "colsum"),
-              M, H, K, int(bool(out_transposed)), _chk(scratch, F32, "scratch"), _stream(), kernels=2)
+    _lib.call("trl_skinny_tn", a, b, out, colsum, M, H, K, int(bool(out_transposed)), scratch, _stream(), kernels=2)
     return out
 
 
@@ -966,8 +866,7 @@ def skinny_tn_partial(a, b, want_colsum, scratch):
     """The slabs of skinny_tn (reduce job kind 0)."""
     M, H = a.shape
     K = b.shape[1]
-    _lib.call("trl_skinny_tn_partial", _chk(a, F32, "a"), _chk(b, F32, "b"), M, H, K, int(bool(want_colsum)),
-              _chk(scratch, F32, "scratch"), _stream())
+    _lib.call("trl_skinny_tn_partial", a, b, M, H, K, int(bool(want_colsum)), scratch, _stream())
 
 
 def skinny_act_wgrad(g, y, x, dw, db, act, scratch):
@@ -975,32 +874,28 @@ def skinny_act_wgrad(g, y, x, dw, db, act, scratch):
     scratch: skinny_tn_scratch_floats(M, H, K) floats."""
     M, H = y.shape
     K = x.shape[1]
-    _lib.call("trl_skinny_act_wgrad", _chk(g, F32, "g"), _chk(y, F32, "y"), _chk(x, F32, "x"), _chk(dw, F32, "dw"),
-              _chk(db, F32, "db"), M, H, K, int(act), _chk(scratch, F32, "scratch"), _stream(), kernels=2)
+    _lib.call("trl_skinny_act_wgrad", g, y, x, dw, db, M, H, K, int(act), scratch, _stream(), kernels=2)
 
 
 def skinny_act_wgrad_partial(g, y, x, act, scratch):
     """The slabs of skinny_act_wgrad (reduce job kind 1)."""
     M, H = y.shape
     K = x.shape[1]
-    _lib.call("trl_skinny_act_wgrad_partial", _chk(g, F32, "g"), _chk(y, F32, "y"), _chk(x, F32, "x"), M, H, K,
-              int(act), _chk(scratch, F32, "scratch"), _stream())
+    _lib.call("trl_skinny_act_wgrad_partial", g, y, x, M, H, K, int(act), scratch, _stream())
 
 
 def skinny_n_dgrad_act(g, w, y, gz, db, act, scratch):
     """gz (M,H) = (g (M,N) @ w (N,H)) * act'(y) and db = colsum(gz); scratch: skinny_dgrad_act_scratch_floats(M, H)."""
     M, H = y.shape
     N = w.shape[0]
-    _lib.call("trl_skinny_n_dgrad_act", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"), _chk(gz, F32, "gz"),
-              _chk(db, F32, "db"), M, H, N, int(act), _chk(scratch, F32, "scratch"), _stream(), kernels=2)
+    _lib.call("trl_skinny_n_dgrad_act", g, w, y, gz, db, M, H, N, int(act), scratch, _stream(), kernels=2)
 
 
 def skinny_n_dgrad_act_partial(g, w, y, gz, act, scratch):
     """gz of skinny_n_dgrad_act and the slabs of its db (reduce job kind 2)."""
     M, H = y.shape
     N = w.shape[0]
-    _lib.call("trl_skinny_n_dgrad_act_partial", _chk(g, F32, "g"), _chk(w, F32, "w"), _chk(y, F32, "y"),
-              _chk(gz, F32, "gz"), M, H, N, int(act), _chk(scratch, F32, "scratch"), _stream())
+    _lib.call("trl_skinny_n_dgrad_act_partial", g, w, y, gz, M, H, N, int(act), scratch, _stream())
 
 
 def skinny_reduce_jobs(jobs):
@@ -1009,12 +904,11 @@ def skinny_reduce_jobs(jobs):
     skinny_n_dgrad_act_partial (colsum = db (H), out None)."""
     n = len(jobs)
     assert n <= 8
-    vp, ci = ctypes.c_void_p, ctypes.c_int
-    _lib.call("trl_skinny_reduce_jobs", n, (ci * n)(*[j[0] for j in jobs]),
-              (vp * n)(*[_chk(j[1], F32, "scratch") for j in jobs]),
-              (vp * n)(*[_opt(j[2], F32, "out") for j in jobs]), (vp * n)(*[_opt(j[3], F32, "colsum") for j in jobs]),
-              (ctypes.c_int64 * n)(*[j[4] for j in jobs]), (ci * n)(*[j[5] for j in jobs]),
-              (ci * n)(*[j[6] for j in jobs]), (ci * n)(*[j[7] for j in jobs]), _stream(), kernels=int(n > 0))
+    ci = ctypes.c_int
+    _lib.call("trl_skinny_reduce_jobs", n, (ci * n)(*[j[0] for j in jobs]), [j[1] for j in jobs],
+              [j[2] for j in jobs], [j[3] for j in jobs], (ctypes.c_int64 * n)(*[j[4] for j in jobs]),
+              (ci * n)(*[j[5] for j in jobs]), (ci * n)(*[j[6] for j in jobs]), (ci * n)(*[j[7] for j in jobs]),
+              _stream(), kernels=int(n > 0))
 
 
 # ------------------------------------------------------------------------------------------ K1 synthetic envs
@@ -1024,16 +918,14 @@ def synth_env_num_ctas(N):
 
 def synth_env_seed(seeds, episode, seed, n_total, first_env):
     """VecEnv.seed: env i of this shard gets seed * n_total + first_env + i; episode counters restart."""
-    _lib.call("trl_synth_env_seed", _chk(seeds, I32, "seeds"), _chk(episode, I32, "episode"), seeds.numel(),
-              int(seed) & 0xFFFFFFFF, int(n_total) & 0xFFFFFFFF, int(first_env) & 0xFFFFFFFF, _stream())
+    _lib.call("trl_synth_env_seed", seeds, episode, seeds.numel(), int(seed) & 0xFFFFFFFF, int(n_total) & 0xFFFFFFFF,
+              int(first_env) & 0xFFFFFFFF, _stream())
 
 
 def synth_env_reset(state, elapsed, episode, seeds, mask, init_scale):
     """New episodes for every env (mask None) or the envs whose uint8 mask is set; state (N, o)."""
     N, o = state.shape
-    _lib.call("trl_synth_env_reset", _chk(state, F32, "state"), _chk(elapsed, I32, "elapsed"),
-              _chk(episode, I32, "episode"), _chk(seeds, I32, "seeds"), _opt(mask, U8, "mask"), N, o,
-              float(init_scale), _stream())
+    _lib.call("trl_synth_env_reset", state, elapsed, episode, seeds, mask, N, o, float(init_scale), _stream())
 
 
 def synth_env_step(state, actions, A, B, c, lb, ub, elapsed, step_count, reward, done, time_limit, partial, batch_sums,
@@ -1043,15 +935,10 @@ def synth_env_step(state, actions, A, B, c, lb, ub, elapsed, step_count, reward,
     norm_*: the observation-normaliser moments (all None: not estimated); step_count / t_ptr: the collector's step
     counters and ring row (None outside a collector)."""
     N, o = state.shape
-    _lib.call("trl_synth_env_step", _chk(state, F32, "state"), _chk(actions, F32, "actions"), _chk(A, F32, "A"),
-              _chk(B, F32, "B"), _chk(c, F32, "c"), _chk(lb, F32, "lb"), _chk(ub, F32, "ub"),
-              _chk(elapsed, I32, "elapsed"), _opt(step_count, I32, "step_count"), _chk(reward, F32, "reward"),
-              _chk(done, U8, "done"), _chk(time_limit, U8, "time_limit"), _opt(partial, F64, "partial"),
-              _opt(batch_sums, F64, "batch_sums"), _opt(norm_mean, F64, "norm_mean"), _opt(norm_var, F64, "norm_var"),
-              _opt(norm_count, F64, "norm_count"), _chk(ticket, I32, "ticket"), _chk(any_reset, I32, "any_reset"),
-              _opt(t_ptr, I32, "t_ptr"), N, o, actions.numel() // N, float(rho), float(eta), float(ctrl_cost),
-              float(term_thr), float(reward_scale), int(max_episode_steps), int(max_episode_frames),
-              int(bool(merge_stats)), _stream())
+    _lib.call("trl_synth_env_step", state, actions, A, B, c, lb, ub, elapsed, step_count, reward, done, time_limit,
+              partial, batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, o,
+              actions.numel() // N, float(rho), float(eta), float(ctrl_cost), float(term_thr), float(reward_scale),
+              int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream())
 
 
 def cartpole_num_ctas(N):
@@ -1069,12 +956,8 @@ def cartpole_step(state, actions, elapsed, step_count, reward, done, time_limit,
         raise ValueError("cartpole_step: state must be (N, 4), got %s" % (tuple(state.shape),))
     if actions.numel() != N:
         raise ValueError("cartpole_step: one action per env expected, got %d for %d envs" % (actions.numel(), N))
-    _lib.call("trl_cartpole_step", _chk(state, F32, "state"), _chk(actions, F32, "actions"),
-              _chk(elapsed, I32, "elapsed"), _opt(step_count, I32, "step_count"), _chk(reward, F32, "reward"),
-              _chk(done, U8, "done"), _chk(time_limit, U8, "time_limit"), _chk(action_error, I32, "action_error"),
-              _opt(partial, F64, "partial"), _opt(batch_sums, F64, "batch_sums"), _opt(norm_mean, F64, "norm_mean"),
-              _opt(norm_var, F64, "norm_var"), _opt(norm_count, F64, "norm_count"), _chk(ticket, I32, "ticket"),
-              _chk(any_reset, I32, "any_reset"), _opt(t_ptr, I32, "t_ptr"), N, float(reward_scale),
+    _lib.call("trl_cartpole_step", state, actions, elapsed, step_count, reward, done, time_limit, action_error, partial,
+              batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, float(reward_scale),
               int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream(), kernels=int(N > 0))
 
 
@@ -1095,12 +978,8 @@ def pendulum_step(phys, obs, actions, elapsed, step_count, reward, done, time_li
                          % (tuple(phys.shape), tuple(obs.shape)))
     if actions.numel() != N:
         raise ValueError("pendulum_step: one action per env expected, got %d for %d envs" % (actions.numel(), N))
-    _lib.call("trl_pendulum_step", _chk(phys, F64, "phys"), _chk(obs, F32, "obs"), _chk(actions, F32, "actions"),
-              _chk(elapsed, I32, "elapsed"), _opt(step_count, I32, "step_count"), _chk(reward, F32, "reward"),
-              _chk(done, U8, "done"), _chk(time_limit, U8, "time_limit"), _chk(action_error, I32, "action_error"),
-              _opt(partial, F64, "partial"), _opt(batch_sums, F64, "batch_sums"), _opt(norm_mean, F64, "norm_mean"),
-              _opt(norm_var, F64, "norm_var"), _opt(norm_count, F64, "norm_count"), _chk(ticket, I32, "ticket"),
-              _chk(any_reset, I32, "any_reset"), _opt(t_ptr, I32, "t_ptr"), N, float(reward_scale),
+    _lib.call("trl_pendulum_step", phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error,
+              partial, batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, float(reward_scale),
               int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream(), kernels=int(N > 0))
 
 
@@ -1117,26 +996,20 @@ def pendulum_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=Non
         raise ValueError("pendulum_reset: select envs by mask or by step_count, not both")
     if cur_ob is not None and (step_count is None or next_norm is None or any_reset is None or t_ptr is None):
         raise ValueError("pendulum_reset: cur_ob needs step_count, next_norm, any_reset and t_ptr")
-    _lib.call("trl_pendulum_reset", _chk(phys, F64, "phys"), _chk(obs, F32, "obs"), _chk(elapsed, I32, "elapsed"),
-              _chk(episode, I32, "episode"), _chk(seeds, I32, "seeds"), _opt(mask, U8, "mask"),
-              _opt(step_count, I32, "step_count"), _opt(next_norm, F32, "next_norm"), _opt(cur_ob, F32, "cur_ob"),
-              _opt(any_reset, I32, "any_reset"), _opt(t_ptr, I32, "t_ptr"), _opt(norm_mean, F64, "norm_mean"),
-              _opt(norm_var, F64, "norm_var"), N, float(clip), int(bool(raw_obs_after_reset)), _stream(),
-              kernels=int(N > 0))
+    _lib.call("trl_pendulum_reset", phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset,
+              t_ptr, norm_mean, norm_var, N, float(clip), int(bool(raw_obs_after_reset)), _stream(), kernels=int(N > 0))
 
 
 def synth_atari_reset(obs, latent, elapsed, episode, seeds, mask=None, zero_is_mask=None, episode_bias=0, bump=1):
     """New episodes for every env, the envs of the uint8 `mask`, or those whose int32 `zero_is_mask` entry is 0."""
-    _lib.call("trl_synth_atari_reset", _chk(obs, U8, "obs"), _chk(latent, I32, "latent"), _chk(elapsed, I32, "elapsed"),
-              _chk(episode, I32, "episode"), _chk(seeds, I32, "seeds"), _opt(mask, U8, "mask"),
-              _opt(zero_is_mask, I32, "zero_is_mask"), int(episode_bias), int(bump), obs.shape[0], _stream())
+    _lib.call("trl_synth_atari_reset", obs, latent, elapsed, episode, seeds, mask, zero_is_mask, int(episode_bias),
+              int(bump), obs.shape[0], _stream())
 
 
 def synth_atari_step(obs, latent, actions, elapsed, reward, done, time_limit, max_steps):
     """One step of all envs: obs (N, 4, 84, 84) uint8 in place, actions (N) float action indices."""
-    _lib.call("trl_synth_atari_step", _chk(obs, U8, "obs"), _chk(latent, I32, "latent"), _chk(actions, F32, "actions"),
-              _chk(elapsed, I32, "elapsed"), _chk(reward, F32, "reward"), _chk(done, U8, "done"),
-              _chk(time_limit, U8, "time_limit"), obs.shape[0], int(max_steps), _stream())
+    _lib.call("trl_synth_atari_step", obs, latent, actions, elapsed, reward, done, time_limit, obs.shape[0],
+              int(max_steps), _stream())
 
 
 def u8_to_f32(x, scale, out=None):
@@ -1144,7 +1017,7 @@ def u8_to_f32(x, scale, out=None):
     if out is None:
         out = torch.empty(x.shape, dtype=F32, device=x.device)
     assert out.numel() == x.numel()
-    _lib.call("trl_u8_to_f32", _chk(x, U8, "x"), _chk(out, F32, "out"), x.numel(), float(scale), _stream())
+    _lib.call("trl_u8_to_f32", x, out, x.numel(), float(scale), _stream())
     return out
 
 
@@ -1155,14 +1028,13 @@ def frame_ring_write(stack, ring, top, age=None, elapsed=None, hist=None, hist_c
     T, N, F = ring.shape
     C = stack.shape[1]
     assert stack.numel() == N * C * F
-    _lib.call("trl_frame_ring_write", _chk(stack, U8, "stack"), _chk(ring, U8, "ring"), _opt(age, U8, "age"),
-              _opt(elapsed, I32, "elapsed"), _opt(hist, U8, "hist"), _opt(hist_count, I32, "hist_count"),
-              _chk(top, I32, "top"), _opt(size, I32, "size"), N, C, F, T, C - 1, _stream())
+    _lib.call("trl_frame_ring_write", stack, ring, age, elapsed, hist, hist_count, top, size, N, C, F, T, C - 1,
+              _stream())
 
 
 def frame_hist_advance(hist_count, size, T):
     """Once per step after the step's frame_ring_write calls."""
-    _lib.call("trl_frame_hist_advance", _chk(hist_count, I32, "hist_count"), _chk(size, I32, "size"), int(T), _stream())
+    _lib.call("trl_frame_hist_advance", hist_count, size, int(T), _stream())
 
 
 def frame_stack_gather(obs_last, next_last, age, hist, hist_count, idx, rows, top, size, scale, out_obs, out_next,
@@ -1171,11 +1043,8 @@ def frame_stack_gather(obs_last, next_last, age, hist, hist_count, idx, rows, to
     idx[k]), rebuilt from the de-duplicated ring: obs_last / next_last (T, N, F), hist (C-1, N, F)."""
     T, N, F = obs_last.shape
     C = hist.shape[0] + 1
-    _lib.call("trl_frame_stack_gather", _chk(obs_last, U8, "obs_last"), _chk(next_last, U8, "next_last"),
-              _chk(age, U8, "age"), _chk(hist, U8, "hist"), _chk(hist_count, I32, "hist_count"), _chk(idx, I64, "idx"),
-              _opt(pos, I32, "pos"), int(rows), _chk(top, I32, "top"), _chk(size, I32, "size"), N, C, F, T,
-              float(scale), _chk(out_obs, F32, "out_obs"), _chk(out_next, F32, "out_next"), _stream(),
-              kernels=int(rows > 0))
+    _lib.call("trl_frame_stack_gather", obs_last, next_last, age, hist, hist_count, idx, pos, int(rows), top, size, N,
+              C, F, T, float(scale), out_obs, out_next, _stream(), kernels=int(rows > 0))
 
 
 # ------------------------------------------------------------------------------------------ K12 peer communication
@@ -1221,21 +1090,20 @@ def allreduce_grad(peer_data, flags, rank, world, out, seg_begin, nseg, mask, su
                    ticket, seq, zero_local=True):
     """out = the sum over ranks of the peers' flat gradients, with what grad_sumsq computes for it; zero_local: this
     rank's gradient is zeroed once every peer has read it."""
-    _lib.call("trl_allreduce_grad", peer_data, flags, int(rank), int(world), _chk(out, F32, "out"), out.numel(),
-              seg_begin, int(nseg), int(mask), _chk(sumsq3, F64, "sumsq3"), _chk(step_counts, I32, "step_counts"),
-              float(betas[0]), float(betas[1]), _chk(scratch, F64, "scratch"), _chk(ticket, I32, "ticket"),
-              _chk(seq, I32, "seq"), int(bool(zero_local)), _stream())
+    _lib.call("trl_allreduce_grad", peer_data, flags, int(rank), int(world), out, out.numel(), seg_begin, int(nseg),
+              int(mask), sumsq3, step_counts, float(betas[0]), float(betas[1]), scratch, ticket, seq,
+              int(bool(zero_local)), _stream())
 
 
 def allreduce_f64(peer_data, flags, rank, world, out, n, gather, seq):
     """out = the sum over ranks (gather: the (world, n) stack) of the first n doubles of the peers' regions."""
-    _lib.call("trl_allreduce_f64", peer_data, flags, int(rank), int(world), _chk(out, F64, "out"), int(n),
-              int(bool(gather)), _chk(seq, I32, "seq"), _stream())
+    _lib.call("trl_allreduce_f64", peer_data, flags, int(rank), int(world), out, int(n), int(bool(gather)), seq,
+              _stream())
     return out
 
 
 def allreduce_f64_ll(local, peer_recv, rank, world, out, n, nmax, gather, ll_seq):
     """allreduce_f64 for n <= nmax doubles of `local` in one NVLink traversal (flag-carrying packets)."""
-    _lib.call("trl_allreduce_f64_ll", _chk(local, F64, "local"), peer_recv, int(rank), int(world),
-              _chk(out, F64, "out"), int(n), int(nmax), int(bool(gather)), _chk(ll_seq, I32, "ll_seq"), _stream())
+    _lib.call("trl_allreduce_f64_ll", local, peer_recv, int(rank), int(world), out, int(n), int(nmax),
+              int(bool(gather)), ll_seq, _stream())
     return out
