@@ -478,6 +478,53 @@ int trl_pendulum_reset(double* phys, float* obs, int* elapsed, unsigned* episode
                        const uint8_t* mask, const int* step_count, const float* next_norm, float* cur_ob,
                        const int* any_reset, const int* t_ptr, const double* norm_mean, const double* norm_var,
                        int64_t N, double clip, int raw_obs_after_reset, void* stream);
+/* ---- K1 for Acrobot-v1: gym.make("Acrobot-v1") (torchrl/env/get_env.py:53) with TimeLimitAugment.step
+ * (env/base_wrapper.py:152-156), RewardShift.reward (env/base_wrapper.py:37-41) and VecEnv.step / partial_reset
+ * (env/vecenv.py:47-61) fused in (defined in oracle/acrobot.py).  phys (N,4) fp64 (theta1, theta2, dtheta1, dtheta2) in
+ * place; obs (N,6) fp32 raw observation (cos theta1, sin theta1, cos theta2, sin theta2, dtheta1, dtheta2).  actions (N)
+ * are 0.0, 1.0 or 2.0 (torque -1, 0, +1); any other value sets *action_error = 1 and leaves that env's state and
+ * observation unchanged (reward 0).  The step is one RK4 step of gym's "book" dynamics over dt = 0.2 in fp64 in gym's
+ * order, the angles wrapped into [-pi, pi] by gym's loop, the velocities bounded by 4 pi and 9 pi.  done = terminal
+ * (-cos theta1 - cos(theta1 + theta2) > 1) or elapsed >= max_episode_steps, time_limit = done && elapsed ==
+ * max_episode_steps; reward = reward_scale * (terminal ? 0 : -1).
+ * partial ((trl_acrobot_num_ctas(N), 12) doubles) / batch_sums (12) / norm_*: the NormObs batch moments of the six
+ * observation columns, as in trl_cartpole_step. */
+int trl_acrobot_num_ctas(int64_t N);
+int trl_acrobot_step(double* phys, float* obs, const float* actions, int* elapsed, const int* step_count, float* reward,
+                     uint8_t* done, uint8_t* time_limit, int* action_error, double* partial, double* batch_sums,
+                     double* norm_mean, double* norm_var, double* norm_count, unsigned* ticket, int* any_reset,
+                     const int* t_ptr, int64_t N, float reward_scale, int max_episode_steps, int max_episode_frames,
+                     int merge_stats, void* stream);
+/* AcrobotEnv.reset + VecEnv.partial_reset, and for a collector the partial reset of collect_finalize, as
+ * trl_pendulum_reset: every state component 0.1 (2U - 1) in fp64 from the counter hash of trl_synth_env_reset. */
+int trl_acrobot_reset(double* phys, float* obs, int* elapsed, unsigned* episode, const unsigned* seeds,
+                      const uint8_t* mask, const int* step_count, const float* next_norm, float* cur_ob,
+                      const int* any_reset, const int* t_ptr, const double* norm_mean, const double* norm_var,
+                      int64_t N, double clip, int raw_obs_after_reset, void* stream);
+/* ---- K1 for MountainCar-v0 (continuous = 0) and MountainCarContinuous-v0 (continuous = 1): gym.make(env_id)
+ * (torchrl/env/get_env.py:53) with, for the continuous variant, NormAct.action (env/continuous_wrapper.py:18-20), and
+ * TimeLimitAugment.step (env/base_wrapper.py:152-156), RewardShift.reward (env/base_wrapper.py:37-41) and VecEnv.step /
+ * partial_reset (env/vecenv.py:47-61) fused in (defined in oracle/mountain_car.py).  phys (N,2) fp64 (position,
+ * velocity) in place; obs (N,2) fp32 raw observation.  v0: actions (N) are 0.0, 1.0 or 2.0 (push left, none, right),
+ * reward -1; continuous: actions (N) in [-1, 1], the force is NormAct's map to [-1, 1] in fp32, widened exactly, reward
+ * 100 on reaching the goal minus 0.1 force^2.  A refused action (v0: any other value; continuous: not finite) sets
+ * *action_error = 1 and leaves that env's state and observation unchanged (reward 0).  done = terminal (position >= 0.5,
+ * continuous 0.45, with velocity >= 0) or elapsed >= max_episode_steps; time_limit as in trl_acrobot_step.
+ * partial ((trl_mountain_car_num_ctas(N), 4) doubles) / batch_sums (4) / norm_*: the NormObs batch moments, as in
+ * trl_cartpole_step. */
+int trl_mountain_car_num_ctas(int64_t N);
+int trl_mountain_car_step(double* phys, float* obs, const float* actions, int* elapsed, const int* step_count,
+                          float* reward, uint8_t* done, uint8_t* time_limit, int* action_error, double* partial,
+                          double* batch_sums, double* norm_mean, double* norm_var, double* norm_count,
+                          unsigned* ticket, int* any_reset, const int* t_ptr, int64_t N, float reward_scale,
+                          int max_episode_steps, int max_episode_frames, int merge_stats, int continuous,
+                          void* stream);
+/* MountainCarEnv.reset + VecEnv.partial_reset, and for a collector the partial reset of collect_finalize, as
+ * trl_pendulum_reset: position -0.6 + 0.2 U in fp64 from the counter hash of trl_synth_env_reset, velocity 0. */
+int trl_mountain_car_reset(double* phys, float* obs, int* elapsed, unsigned* episode, const unsigned* seeds,
+                           const uint8_t* mask, const int* step_count, const float* next_norm, float* cur_ob,
+                           const int* any_reset, const int* t_ptr, const double* norm_mean, const double* norm_var,
+                           int64_t N, double clip, int raw_obs_after_reset, void* stream);
 
 /* ScaledFloatFrame (env/atari_wrapper.py:171-180): out = in * scale */
 int trl_u8_to_f32(const uint8_t* in, float* out, int64_t n, float scale, void* stream);

@@ -110,12 +110,23 @@ __device__ __forceinline__ void env_moments(const EnvStepFields& f, const float 
     f.partial[static_cast<long long>(blockIdx.x) * 2 * D + tid] = t;
   }
   if (last_cta(f.ticket, gridDim.x)) {
-    if (wid < 2 * D) {
-      double acc = 0.0;
-      for (unsigned b = lane; b < gridDim.x; b += 32)
-        acc += __ldcg(f.partial + static_cast<long long>(b) * 2 * D + wid);
-      acc = warp_sum(acc);
-      if (lane == 0) sred[wid] = acc;
+    if constexpr (2 * D <= kWarps) {
+      if (wid < 2 * D) {
+        double acc = 0.0;
+        for (unsigned b = lane; b < gridDim.x; b += 32)
+          acc += __ldcg(f.partial + static_cast<long long>(b) * 2 * D + wid);
+        acc = warp_sum(acc);
+        if (lane == 0) sred[wid] = acc;
+      }
+    } else {
+      // more quantities than warps (Acrobot's 12 over 8 warps): warp k also folds k + kWarps, ..., in the same order
+      for (int k = wid; k < 2 * D; k += kWarps) {
+        double acc = 0.0;
+        for (unsigned b = lane; b < gridDim.x; b += 32)
+          acc += __ldcg(f.partial + static_cast<long long>(b) * 2 * D + k);
+        acc = warp_sum(acc);
+        if (lane == 0) sred[k] = acc;
+      }
     }
     __syncthreads();
     if (tid < D) merge_feature(f, D, tid, sred[tid], sred[D + tid]);
@@ -133,6 +144,73 @@ __device__ __forceinline__ float next_observation(bool all_raw, bool normalise, 
   if (!normalise) return *carried;
   const double y = (static_cast<double>(raw) - norm_mean[j]) / (sqrt(norm_var[j]) + 1e-4);
   return static_cast<float>(fmin(fmax(y, -clip), clip));
+}
+
+// ---- the own reset of an env whose observation is not its state -----------------------------------------------------
+// An fp64 physical state (N, Env::kPhys) and its fp32 raw observation (N, Env::kObs).  Env supplies
+//   static __device__ void reset_state(unsigned seed, unsigned episode, double (&s)[kPhys]);
+//   static __device__ void observe(const double (&s)[kPhys], float (&o)[kObs]);
+struct SelfResetParams {
+  double* __restrict__ phys;              // (N, kPhys)
+  float* __restrict__ obs;                // (N, kObs) raw observation
+  int* __restrict__ elapsed;              // (N)
+  unsigned* __restrict__ episode;         // (N)
+  const unsigned* __restrict__ seeds;     // (N)
+  const uint8_t* __restrict__ mask;       // (N) envs to reset, or nullptr
+  const int* __restrict__ step_count;     // (N) reset where 0 (the collector's path), or nullptr
+  // collector path (cur_ob != nullptr): the next observation of every env, as collect_finalize writes it
+  const float* __restrict__ next_norm;    // (N, kObs) observation the env step returned (normalised if NormObs)
+  float* __restrict__ cur_ob;             // (N, kObs) or nullptr
+  const int* __restrict__ any_reset;      // (2) flag written by the step kernel
+  const int* __restrict__ t_ptr;          // (1) ring row (selects the flag slot)
+  const double* __restrict__ norm_mean;   // (kObs) or nullptr (no NormObs)
+  const double* __restrict__ norm_var;    // (kObs)
+  long long N;
+  double clip;
+  int raw_obs_after_reset;                // reference quirk A.1 (SURVEY.md): raw obs for ALL envs after any reset
+};
+
+// The reset arguments' rules; `fn` names the entry point in the message.
+inline int check_self_reset(const char* fn, const SelfResetParams& p) {
+  TRL_REQUIRE(p.phys && p.obs && p.elapsed && p.episode && p.seeds, "%s: null pointer", fn);
+  TRL_REQUIRE(!(p.mask && p.step_count), "%s: select envs by mask or by step_count, not both", fn);
+  TRL_REQUIRE(!p.cur_ob || (p.step_count && p.next_norm && p.any_reset && p.t_ptr),
+              "%s: cur_ob needs step_count, next_norm, any_reset and t_ptr", fn);
+  TRL_REQUIRE(!p.norm_mean || p.norm_var, "%s: norm_mean given without norm_var", fn);
+  return TRL_OK;
+}
+
+// Env n's reset: selected by step_count == 0, else by mask, else always.  A selected env gets a new state from the
+// counter hash of (seed, episode), its raw observation, elapsed = 0 and episode += 1.  With cur_ob, every env's next
+// observation is written by collect_finalize's rules (next_observation).
+template <class Env>
+__device__ __forceinline__ void env_self_reset(const SelfResetParams& p, long long n) {
+  constexpr int P = Env::kPhys, D = Env::kObs;
+  if (n >= p.N) return;
+  const bool sel = p.step_count ? p.step_count[n] == 0 : (p.mask ? p.mask[n] != 0 : true);
+  float raw[D];
+  if (sel) {
+    const unsigned ep = p.episode[n];
+    double s[P];
+    Env::reset_state(p.seeds[n], ep, s);
+    Env::observe(s, raw);
+#pragma unroll
+    for (int j = 0; j < P; ++j) p.phys[n * P + j] = s[j];
+#pragma unroll
+    for (int j = 0; j < D; ++j) p.obs[n * D + j] = raw[j];
+    p.episode[n] = ep + 1u;
+    p.elapsed[n] = 0;
+  } else {
+#pragma unroll
+    for (int j = 0; j < D; ++j) raw[j] = p.obs[n * D + j];
+  }
+  if (!p.cur_ob) return;
+  const bool all_raw = !p.norm_mean || (p.raw_obs_after_reset && p.any_reset[*p.t_ptr & 1]);
+#pragma unroll
+  for (int j = 0; j < D; ++j) {
+    p.cur_ob[n * D + j] =
+        next_observation(all_raw, sel, raw[j], p.next_norm + n * D + j, p.norm_mean, p.norm_var, j, p.clip);
+  }
 }
 
 }  // namespace trl

@@ -1,14 +1,17 @@
 """Env factories with the reference's names (/root/reference/torchrl/env/get_env.py:32-87).
 
 Synthetic ids ("SynthHalfCheetah-v0", "SynthAnt-v0") build the device-resident
-SynthVecEnv, "SynthAtari-v0" the pixel env, "CartPole-v0" / "CartPole-v1" the device CartPole and "Pendulum-v1" the
-device Pendulum; any other id (Pendulum-v0 included: its dynamics differ from v1's) needs a real gym + the host-env
+SynthVecEnv, "SynthAtari-v0" the pixel env, "CartPole-v0" / "CartPole-v1" the device CartPole, "Pendulum-v1" the
+device Pendulum, "Acrobot-v1" the device Acrobot and "MountainCar-v0" / "MountainCarContinuous-v0" the device Mountain
+Car; any other id (Pendulum-v0 included: its dynamics differ from v1's) needs a real gym + the host-env
 bridge (SURVEY.md section 8(f).1), which is outside this round's hot path and raises.
 """
 import torch
 
 from . import synth_spec
+from .acrobot import AcrobotVecEnv, is_acrobot
 from .cartpole import CartPoleVecEnv, is_cartpole
+from .mountain_car import MountainCarVecEnv, is_mountain_car
 from .pendulum import PendulumVecEnv, is_pendulum
 from .synth import SynthVecEnv
 from .synth_atari import SynthAtariVecEnv, ENV_ID as ATARI_ID
@@ -31,6 +34,10 @@ def get_vec_env(env_id, env_param, vec_env_nums, device=None, **kwargs):
         return CartPoleVecEnv(env_id, vec_env_nums, env_param, device=_device(device), **kwargs)
     if is_pendulum(env_id):
         return PendulumVecEnv(vec_env_nums, env_param, device=_device(device), **kwargs)
+    if is_acrobot(env_id):
+        return AcrobotVecEnv(vec_env_nums, env_param, device=_device(device), **kwargs)
+    if is_mountain_car(env_id):
+        return MountainCarVecEnv(env_id, vec_env_nums, env_param, device=_device(device), **kwargs)
     raise NotImplementedError("only the synthetic device envs are built in this round: %r" % (env_id,))
 
 

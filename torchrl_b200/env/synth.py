@@ -1,5 +1,5 @@
 """Device-resident vectorised envs with the reference's vec-env API: `DeviceVecEnv`, the base of the state-vector
-device envs (synthetic, CartPole, Pendulum), and the synthetic env itself.
+device envs (synthetic, CartPole, Pendulum, Acrobot, Mountain Car), and the synthetic env itself.
 
 Stands where ``NormObs(VecEnv(...))`` / ``NormObs(SubProcVecEnv(...))`` stand in the reference
 (/root/reference/torchrl/env/get_env.py:70-87): same methods and attributes

@@ -1000,6 +1000,84 @@ def pendulum_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=Non
               t_ptr, norm_mean, norm_var, N, float(clip), int(bool(raw_obs_after_reset)), _stream(), kernels=int(N > 0))
 
 
+def _check_phys_obs(fn, phys, obs, P, D):
+    N = phys.shape[0]
+    if phys.dim() != 2 or phys.shape[1] != P or tuple(obs.shape) != (N, D):
+        raise ValueError("%s: phys must be (N, %d) and obs (N, %d), got %s and %s"
+                         % (fn, P, D, tuple(phys.shape), tuple(obs.shape)))
+    return N
+
+
+def _env_step(fn, P, D, phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error, partial,
+              batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale, max_episode_steps,
+              max_episode_frames, merge_stats, *extra):
+    """The step of an env with an fp64 state (N, P), an fp32 observation (N, D) and one action per env."""
+    N = _check_phys_obs(fn, phys, obs, P, D)
+    if actions.numel() != N:
+        raise ValueError("%s: one action per env expected, got %d for %d envs" % (fn, actions.numel(), N))
+    _lib.call("trl_" + fn, phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error, partial,
+              batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, float(reward_scale),
+              int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), *extra, _stream(),
+              kernels=int(N > 0))
+
+
+def _env_reset(fn, P, D, phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset, t_ptr,
+               norm_mean, norm_var, clip, raw_obs_after_reset):
+    """The own reset of an env with an fp64 state (N, P) and an fp32 observation (N, D), as pendulum_reset."""
+    N = _check_phys_obs(fn, phys, obs, P, D)
+    if mask is not None and step_count is not None:
+        raise ValueError("%s: select envs by mask or by step_count, not both" % fn)
+    if cur_ob is not None and (step_count is None or next_norm is None or any_reset is None or t_ptr is None):
+        raise ValueError("%s: cur_ob needs step_count, next_norm, any_reset and t_ptr" % fn)
+    _lib.call("trl_" + fn, phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset, t_ptr,
+              norm_mean, norm_var, N, float(clip), int(bool(raw_obs_after_reset)), _stream(), kernels=int(N > 0))
+
+
+def acrobot_num_ctas(N):
+    return int(_lib.load().trl_acrobot_num_ctas(int(N)))
+
+
+def acrobot_step(phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error, partial, batch_sums,
+                 norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale, max_episode_steps,
+                 max_episode_frames, merge_stats):
+    """One Acrobot-v1 step of all N envs (csrc/acrobot.cu): phys (N, 4) fp64 and obs (N, 6) in place, actions (N) 0.0 /
+    1.0 / 2.0 (anything else sets action_error (1) int32).  partial / batch_sums / norm_*: the observation-normaliser
+    moments (all None: not estimated); step_count / t_ptr: the collector's step counters and ring row (None outside a
+    collector)."""
+    _env_step("acrobot_step", 4, 6, phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error,
+              partial, batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale,
+              max_episode_steps, max_episode_frames, merge_stats)
+
+
+def acrobot_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=None, next_norm=None, cur_ob=None,
+                  any_reset=None, t_ptr=None, norm_mean=None, norm_var=None, clip=10.0, raw_obs_after_reset=True):
+    """New Acrobot episodes, selected and written as pendulum_reset does."""
+    _env_reset("acrobot_reset", 4, 6, phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob,
+               any_reset, t_ptr, norm_mean, norm_var, clip, raw_obs_after_reset)
+
+
+def mountain_car_num_ctas(N):
+    return int(_lib.load().trl_mountain_car_num_ctas(int(N)))
+
+
+def mountain_car_step(phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error, partial,
+                      batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale,
+                      max_episode_steps, max_episode_frames, merge_stats, continuous):
+    """One Mountain Car step of all N envs (csrc/mountain_car.cu): phys (N, 2) fp64 and obs (N, 2) in place.
+    MountainCar-v0 (continuous False): actions (N) 0.0 / 1.0 / 2.0; MountainCarContinuous-v0: actions (N) in [-1, 1]; a
+    refused action sets action_error (1) int32.  Other arguments as acrobot_step."""
+    _env_step("mountain_car_step", 2, 2, phys, obs, actions, elapsed, step_count, reward, done, time_limit,
+              action_error, partial, batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr,
+              reward_scale, max_episode_steps, max_episode_frames, merge_stats, int(bool(continuous)))
+
+
+def mountain_car_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=None, next_norm=None, cur_ob=None,
+                       any_reset=None, t_ptr=None, norm_mean=None, norm_var=None, clip=10.0, raw_obs_after_reset=True):
+    """New Mountain Car episodes (both ids), selected and written as pendulum_reset does."""
+    _env_reset("mountain_car_reset", 2, 2, phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob,
+               any_reset, t_ptr, norm_mean, norm_var, clip, raw_obs_after_reset)
+
+
 def synth_atari_reset(obs, latent, elapsed, episode, seeds, mask=None, zero_is_mask=None, episode_bias=0, bump=1):
     """New episodes for every env, the envs of the uint8 `mask`, or those whose int32 `zero_is_mask` entry is 0."""
     _lib.call("trl_synth_atari_reset", obs, latent, elapsed, episode, seeds, mask, zero_is_mask, int(episode_bias),
