@@ -1,5 +1,5 @@
-"""Throughput of the device Acrobot-v1, MountainCar-v0 and MountainCarContinuous-v0: each bare env-step kernel at
-N = 2^20 (CUDA events over a captured graph of many launches, bytes per env from the operand shapes, bandwidth against
+"""Throughput of the device classic-control envs (CartPole-v1, Pendulum-v1, Acrobot-v1, MountainCar-v0,
+MountainCarContinuous-v0): each bare env-step kernel at N = 2^20 (CUDA events over a captured graph of many launches, bytes per env from the operand shapes, bandwidth against
 the H100 SXM's 3.35 TB/s), and the captured DQN collector step (Q-network forward, epsilon-greedy, env step, finalize,
 the env's own reset, ring advance) at a few thousand Acrobot envs.  Prints the card and its power limit and one JSON
 line.
@@ -26,8 +26,9 @@ from scripts.pendulum_bench import HBM_BYTES_PER_S, card  # noqa: E402
 
 def bytes_per_env(P, D):
     """Per env and step: phys (P fp64) + action (fp32) + elapsed (int32) read; phys + obs (D fp32) + reward (fp32) +
-    done + time_limit (uint8) + elapsed written."""
-    return (P * 8 + 4 + 4) + (P * 8 + D * 4 + 4 + 1 + 1 + 4)
+    done + time_limit (uint8) + elapsed written.  P = 0 (CartPole): the state is the fp32 observation, read too."""
+    state = P * 8 if P else D * 4
+    return (state + 4 + 4) + (P * 8 + D * 4 + 4 + 1 + 1 + 4)
 
 
 def kernel_us(env_id, N, launches, reps, actions):
@@ -86,10 +87,13 @@ def main():
     name, limit = card()
     print("card: %s, power limit: %s W" % (name, "unknown" if limit is None else "%.0f" % limit), flush=True)
     N = a.kernel_envs
+    binary = (torch.arange(N, device="cuda") % 2).float()
     discrete = (torch.arange(N, device="cuda") % 3).float()
     continuous = torch.linspace(-1, 1, N, device="cuda")
     out = {"gpu": name, "power_limit_w": limit, "kernel_envs": N}
-    for key, env_id, P, D, act in (("acrobot", "Acrobot-v1", 4, 6, discrete),
+    for key, env_id, P, D, act in (("cartpole", "CartPole-v1", 0, 4, binary),
+                                   ("pendulum", "Pendulum-v1", 2, 3, continuous),
+                                   ("acrobot", "Acrobot-v1", 4, 6, discrete),
                                    ("mountain_car", "MountainCar-v0", 2, 2, discrete),
                                    ("mountain_car_continuous", "MountainCarContinuous-v0", 2, 2, continuous)):
         us = kernel_us(env_id, N, a.launches, 5, act)

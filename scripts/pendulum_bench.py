@@ -1,8 +1,8 @@
-"""Throughput of the device Pendulum-v1: the bare env-step kernel at N = 2^20 (CUDA events over a captured graph of many
-launches, bytes per env from the operand shapes, bandwidth against the H100 SXM's 3.35 TB/s), and the captured TD3
-collector step plus the TD3 update at a few thousand envs.  Prints the card and its power limit and one JSON line.
+"""Throughput of the device Pendulum-v1 under TD3: the captured TD3 collector step plus the TD3 update at a few thousand
+envs (scripts/classic_control_bench.py times the bare env-step kernel).  Prints the card and its power limit and one
+JSON line.
 
-    python scripts/pendulum_bench.py --kernel-envs 1048576 --envs 4096
+    python scripts/pendulum_bench.py --envs 4096
 """
 import argparse
 import json
@@ -17,7 +17,6 @@ import torch
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import torchrl_b200.networks as networks  # noqa: E402
 import torchrl_b200.policies as policies  # noqa: E402
-from torchrl_b200 import ops  # noqa: E402
 from torchrl_b200.algo import TD3  # noqa: E402
 from torchrl_b200.collector import VecCollector  # noqa: E402
 from torchrl_b200.env import get_vec_env  # noqa: E402
@@ -25,10 +24,6 @@ from torchrl_b200.replay_buffers import BaseReplayBuffer  # noqa: E402
 from torchrl_b200.utils import NullLogger  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
-# per env and step: phys (2 fp64) + action (fp32) + elapsed (int32) read; phys + obs (3 fp32) + reward (fp32) + done +
-# time_limit (uint8) + elapsed written
-BYTES_READ = 2 * 8 + 4 + 4
-BYTES_WRITTEN = 2 * 8 + 3 * 4 + 4 + 1 + 1 + 4
 
 
 def card():
@@ -40,27 +35,6 @@ def card():
         return name, float(out.splitlines()[0])
     except Exception:                                   # noqa: BLE001 -- the number is reported as unknown
         return name, None
-
-
-def kernel_us(N, launches, reps):
-    """Mean time of one trl_pendulum_step launch over N envs, from a captured graph of `launches` launches."""
-    env = get_vec_env("Pendulum-v1", {}, N)
-    env.reset()
-    act = torch.linspace(-1, 1, N, device="cuda")
-    for _ in range(10):
-        env.launch_step(act)
-    g = ops.CapturedGraph(lambda: [env.launch_step(act) for _ in range(launches)])
-    g.replay()
-    torch.cuda.synchronize()
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    times = []
-    for _ in range(reps):
-        ev0.record()
-        g.replay()
-        ev1.record()
-        torch.cuda.synchronize()
-        times.append(1000.0 * ev0.elapsed_time(ev1) / launches)
-    return float(np.median(times))
 
 
 def td3_rate(N, T, epochs, hidden, opt_times, batch):
@@ -98,8 +72,6 @@ def td3_rate(N, T, epochs, hidden, opt_times, batch):
 
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--kernel-envs", type=int, default=1 << 20)
-    p.add_argument("--launches", type=int, default=200)
     p.add_argument("--envs", type=int, default=4096)
     p.add_argument("--steps", type=int, default=50, help="collector steps per epoch")
     p.add_argument("--epochs", type=int, default=5, help="timed epochs (after 3 warm-up epochs)")
@@ -109,15 +81,9 @@ def main():
     a = p.parse_args()
     name, limit = card()
     print("card: %s, power limit: %s W" % (name, "unknown" if limit is None else "%.0f" % limit), flush=True)
-    us = kernel_us(a.kernel_envs, a.launches, 5)
-    per_env = BYTES_READ + BYTES_WRITTEN
-    bw = per_env * a.kernel_envs / (us * 1e-6)
     col_rate, epoch_rate, upd_ms = td3_rate(a.envs, a.steps, a.epochs, a.hidden, a.opt_times, a.batch)
     print(json.dumps({
-        "gpu": name, "power_limit_w": limit, "kernel_envs": a.kernel_envs, "pendulum_step_kernel_us": round(us, 2),
-        "bytes_per_env": per_env, "achieved_tb_per_s": round(bw / 1e12, 3),
-        "fraction_of_3_35_tb_per_s": round(bw / HBM_BYTES_PER_S, 3),
-        "envs": a.envs, "hidden": a.hidden, "steps_per_epoch": a.steps, "opt_times": a.opt_times, "batch": a.batch,
+        "gpu": name, "power_limit_w": limit, "envs": a.envs, "hidden": a.hidden, "steps_per_epoch": a.steps, "opt_times": a.opt_times, "batch": a.batch,
         "td3_collector_env_steps_per_s": round(col_rate), "td3_epoch_env_steps_per_s": round(epoch_rate),
         "td3_update_ms": round(upd_ms, 3),
     }))

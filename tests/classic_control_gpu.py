@@ -1,7 +1,7 @@
-"""What the GPU tests of the self-resetting classic-control envs (Acrobot-v1, MountainCar-v0,
+"""What the GPU tests of the self-resetting classic-control envs (Pendulum-v1, Acrobot-v1, MountainCar-v0,
 MountainCarContinuous-v0) share: the tolerance checks, one kernel step from given fp64 states, a stub policy that runs
 the scripted controller inside the collector's step, and the off- and on-policy agents of the one-epoch tests.  Each
-env's test module holds an `Case` naming its oracle, kernel and controller."""
+env's test module holds a `Case` naming its oracle, kernel and controller."""
 from dataclasses import dataclass
 from typing import Callable
 
@@ -225,3 +225,59 @@ def one_epoch(agent, col, kind, off_policy):
             else:
                 assert np.isfinite(v), k
     return out
+
+
+def continuous_agent(env_id, kind, obs_dim, max_episode_frames, time_limit_filter, use_graph=True, N=16, T=40, seed=0):
+    """One of TD3, DDPG, SAC, TwinSAC-Q, PPO on a continuous env with one action; `time_limit_filter` is the
+    off-policy replay buffer's (PPO's buffer always filters)."""
+    import torch
+    import torch.nn as nn
+    import torchrl_b200.networks as networks
+    import torchrl_b200.policies as policies
+    from torchrl_b200.algo import DDPG, PPO, SAC, TD3, TwinSACQ
+    from torchrl_b200.collector import VecCollector, VecOnPolicyCollector
+    from torchrl_b200.env import get_vec_env
+    from torchrl_b200.replay_buffers import BaseReplayBuffer, OnPolicyReplayBuffer
+    from torchrl_b200.utils import NullLogger
+    dev = torch.device("cuda:0")
+    env = get_vec_env(env_id, {"reward_scale": 1, "obs_norm": kind == "ppo"}, N)
+    eval_env = get_vec_env(env_id, {"reward_scale": 1, "obs_norm": kind == "ppo"}, N)
+    env.seed(seed); eval_env.seed(seed + 1000); torch.manual_seed(seed); np.random.seed(seed)
+    o, a = obs_dim, 1
+    net = dict(hidden_shapes=[64, 64], append_hidden_shapes=[], base_type=networks.MLPBase, activation_func=nn.ReLU)
+    if kind == "ppo":
+        buf = OnPolicyReplayBuffer(env_nums=N, max_replay_buffer_size=T * N, time_limit_filter=True)
+        pf = policies.GuassianContPolicyBasicBias(input_shape=o, output_shape=a, tanh_action=True, **net)
+        vf = networks.Net(input_shape=o, output_shape=1, **net)
+        col = VecOnPolicyCollector(vf, env=env, eval_env=eval_env, pf=pf, replay_buffer=buf, device=dev,
+                                   epoch_frames=T * N, max_episode_frames=max_episode_frames, use_cuda_graph=use_graph)
+        return PPO(pf=pf, vf=vf, plr=3e-4, vlr=3e-4, clip_para=0.2, opt_epochs=2, tau=0.95, shuffle=True, env=env,
+                   replay_buffer=buf, collector=col, logger=NullLogger(), discount=0.99, num_epochs=3,
+                   batch_size=10 * N, gae=True, device=dev, save_dir=None, use_cuda_graph=use_graph), col, buf, env
+    buf = BaseReplayBuffer(env_nums=N, max_replay_buffer_size=4 * T * N, time_limit_filter=time_limit_filter)
+    if kind in ("sac", "twin_sac_q"):
+        pf = policies.GuassianContPolicy(input_shape=o, output_shape=2 * a, tanh_action=True, **net)
+    elif kind == "ddpg":
+        pf = policies.DetContPolicy(input_shape=o, output_shape=a, tanh_action=True, **net)
+    else:
+        pf = policies.FixGuassianContPolicy(input_shape=o, output_shape=a, tanh_action=True, norm_std_explore=0.1,
+                                            **net)
+    qf1 = networks.QNet(input_shape=o + a, output_shape=1, **net)
+    col = VecCollector(env=env, eval_env=eval_env, pf=pf, replay_buffer=buf, device=dev, epoch_frames=T * N,
+                       max_episode_frames=max_episode_frames, use_cuda_graph=use_graph)
+    common = dict(env=env, replay_buffer=buf, collector=col, logger=NullLogger(), discount=0.99, batch_size=8 * N,
+                  device=dev, save_dir=None, tau=0.005, use_soft_update=True, opt_times=8, pretrain_epochs=1,
+                  num_epochs=3, use_cuda_graph=use_graph)
+    if kind == "td3":
+        agent = TD3(pf=pf, qf1=qf1, qf2=networks.QNet(input_shape=o + a, output_shape=1, **net), plr=1e-3, qlr=1e-3,
+                    **common)
+    elif kind == "ddpg":
+        agent = DDPG(pf=pf, qf=qf1, plr=1e-3, qlr=1e-3, **common)
+    elif kind == "twin_sac_q":
+        agent = TwinSACQ(pf=pf, qf1=qf1, qf2=networks.QNet(input_shape=o + a, output_shape=1, **net), plr=3e-4,
+                         qlr=3e-4, policy_std_reg_weight=0, policy_mean_reg_weight=0, **common)
+    else:
+        vf = networks.Net(input_shape=o, output_shape=1, **net)
+        agent = SAC(pf=pf, vf=vf, qf=qf1, plr=3e-4, vlr=3e-4, qlr=3e-4, policy_std_reg_weight=1e-3,
+                    policy_mean_reg_weight=1e-3, **common)
+    return agent, col, buf, env

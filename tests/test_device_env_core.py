@@ -63,8 +63,8 @@ def test_checkpoint_saved_before_a_step_restores_after_it(tmp_path, env_id):
         agent, _, _, env = _dqn("dqn", use_graph=False)
         acts = (torch.arange(env.env_nums, device="cuda") % 2).float()
     else:
-        from tests.test_pendulum_gpu import _agent
-        agent, _, _, env = _agent("td3", use_graph=False)
+        from tests.classic_control_gpu import continuous_agent
+        agent, _, _, env = continuous_agent("Pendulum-v1", "td3", 3, 200, False, use_graph=False)
         acts = torch.linspace(-1.0, 1.0, env.env_nums, device="cuda")
     env.reset()
     path = str(tmp_path / "ck.pt")

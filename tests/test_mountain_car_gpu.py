@@ -286,63 +286,9 @@ def test_one_epoch_of_each_discrete_agent(kind):
     assert len(ev["eval_rewards"]) == 16 and all(-200 <= r <= 0 for r in ev["eval_rewards"])
 
 
-def _continuous_agent(kind, N=16, T=40, seed=0):
-    import torch
-    import torch.nn as nn
-    import torchrl_b200.networks as networks
-    import torchrl_b200.policies as policies
-    from torchrl_b200.algo import DDPG, PPO, SAC, TD3, TwinSACQ
-    from torchrl_b200.collector import VecCollector, VecOnPolicyCollector
-    from torchrl_b200.env import get_vec_env
-    from torchrl_b200.replay_buffers import BaseReplayBuffer, OnPolicyReplayBuffer
-    from torchrl_b200.utils import NullLogger
-    dev = torch.device("cuda:0")
-    env = get_vec_env(CONT, {"reward_scale": 1, "obs_norm": kind == "ppo"}, N)
-    eval_env = get_vec_env(CONT, {"reward_scale": 1, "obs_norm": kind == "ppo"}, N)
-    env.seed(seed); eval_env.seed(seed + 1000); torch.manual_seed(seed); np.random.seed(seed)
-    o, a = 2, 1
-    net = dict(hidden_shapes=[64, 64], append_hidden_shapes=[], base_type=networks.MLPBase, activation_func=nn.ReLU)
-    if kind == "ppo":
-        buf = OnPolicyReplayBuffer(env_nums=N, max_replay_buffer_size=T * N, time_limit_filter=True)
-        pf = policies.GuassianContPolicyBasicBias(input_shape=o, output_shape=a, tanh_action=True, **net)
-        vf = networks.Net(input_shape=o, output_shape=1, **net)
-        col = VecOnPolicyCollector(vf, env=env, eval_env=eval_env, pf=pf, replay_buffer=buf, device=dev,
-                                   epoch_frames=T * N, max_episode_frames=999)
-        return PPO(pf=pf, vf=vf, plr=3e-4, vlr=3e-4, clip_para=0.2, opt_epochs=2, tau=0.95, shuffle=True, env=env,
-                   replay_buffer=buf, collector=col, logger=NullLogger(), discount=0.99, num_epochs=3,
-                   batch_size=10 * N, gae=True, device=dev, save_dir=None), col, buf, env
-    buf = BaseReplayBuffer(env_nums=N, max_replay_buffer_size=4 * T * N, time_limit_filter=True)
-    if kind in ("sac", "twin_sac_q"):
-        pf = policies.GuassianContPolicy(input_shape=o, output_shape=2 * a, tanh_action=True, **net)
-    elif kind == "ddpg":
-        pf = policies.DetContPolicy(input_shape=o, output_shape=a, tanh_action=True, **net)
-    else:
-        pf = policies.FixGuassianContPolicy(input_shape=o, output_shape=a, tanh_action=True, norm_std_explore=0.1,
-                                            **net)
-    qf1 = networks.QNet(input_shape=o + a, output_shape=1, **net)
-    col = VecCollector(env=env, eval_env=eval_env, pf=pf, replay_buffer=buf, device=dev, epoch_frames=T * N,
-                       max_episode_frames=999)
-    common = dict(env=env, replay_buffer=buf, collector=col, logger=NullLogger(), discount=0.99, batch_size=8 * N,
-                  device=dev, save_dir=None, tau=0.005, use_soft_update=True, opt_times=8, pretrain_epochs=1,
-                  num_epochs=3)
-    if kind == "td3":
-        agent = TD3(pf=pf, qf1=qf1, qf2=networks.QNet(input_shape=o + a, output_shape=1, **net), plr=1e-3, qlr=1e-3,
-                    **common)
-    elif kind == "ddpg":
-        agent = DDPG(pf=pf, qf=qf1, plr=1e-3, qlr=1e-3, **common)
-    elif kind == "twin_sac_q":
-        agent = TwinSACQ(pf=pf, qf1=qf1, qf2=networks.QNet(input_shape=o + a, output_shape=1, **net), plr=3e-4,
-                         qlr=3e-4, policy_std_reg_weight=0, policy_mean_reg_weight=0, **common)
-    else:
-        vf = networks.Net(input_shape=o, output_shape=1, **net)
-        agent = SAC(pf=pf, vf=vf, qf=qf1, plr=3e-4, vlr=3e-4, qlr=3e-4, policy_std_reg_weight=1e-3,
-                    policy_mean_reg_weight=1e-3, **common)
-    return agent, col, buf, env
-
-
 @pytest.mark.parametrize("kind", ["td3", "ddpg", "sac", "twin_sac_q", "ppo"])
 def test_one_epoch_of_each_continuous_agent(kind):
-    agent, col, buf, env = _continuous_agent(kind)
+    agent, col, buf, env = cc.continuous_agent(CONT, kind, 2, 999, True)
     out = cc.one_epoch(agent, col, kind, kind != "ppo")
     assert all(-0.1 * 999 - 1e-3 <= r <= 100 for r in out["train_rewards"])
     acts = buf._acts.cpu().numpy()

@@ -15,48 +15,20 @@ import numpy as np
 import pytest
 
 from oracle import pendulum as P
+from tests import classic_control_gpu as cc
 
 pytestmark = pytest.mark.gpu
 
 
-def _check_phys(got, want):
-    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
-    tol = 4 * np.spacing(np.maximum(np.abs(want), 1.0))
-    diff = np.abs(got - want)
-    assert np.all(diff <= tol), np.max(diff / tol)
-    if got.size >= 128:
-        assert np.mean(got == want) >= 0.75, np.mean(got == want)        # most components agree to the last bit
-
-
-def _check_obs(got, want):
-    got, want = np.asarray(got, np.float32), np.asarray(want, np.float32)
-    ulp = np.spacing(np.abs(want)).astype(np.float64)
-    diff = np.abs(got.astype(np.float64) - want.astype(np.float64))
-    assert np.all(diff <= np.maximum(ulp, 1e-45)), np.max(diff)
-
-
-def _tensors(N, dev="cuda"):
-    import torch
-    return dict(reward=torch.zeros(N, device=dev), done=torch.zeros(N, dtype=torch.uint8, device=dev),
-                time_limit=torch.zeros(N, dtype=torch.uint8, device=dev),
-                err=torch.zeros(1, dtype=torch.int32, device=dev), ticket=torch.zeros(1, dtype=torch.int32, device=dev),
-                any_reset=torch.zeros(2, dtype=torch.int32, device=dev))
-
-
-def _step_kernel(phys, actions, elapsed, reward_scale=1.0, max_steps=200):
-    import torch
+def _case():
     from torchrl_b200 import ops
-    N = phys.shape[0]
-    ph = torch.as_tensor(phys, dtype=torch.float64, device="cuda").contiguous()
-    obs = torch.zeros(N, 3, device="cuda")
-    el = torch.as_tensor(elapsed, dtype=torch.int32, device="cuda").contiguous()
-    t = _tensors(N)
-    ops.pendulum_step(ph, obs, torch.as_tensor(actions, dtype=torch.float32, device="cuda"), el, None, t["reward"],
-                      t["done"], t["time_limit"], t["err"], None, None, None, None, None, t["ticket"], t["any_reset"],
-                      None, reward_scale, max_steps, 1 << 30, False)
-    return (ph.cpu().numpy(), obs.cpu().numpy(), t["reward"].cpu().numpy(), t["done"].cpu().numpy().astype(bool),
-            t["time_limit"].cpu().numpy().astype(bool), el.cpu().numpy(), int(t["err"].item()),
-            t["any_reset"].cpu().numpy())
+    return cc.Case("Pendulum-v1", 2, 3, P.step, P.reset_phys, P.observe, None, ops.pendulum_step)
+
+
+def _check_phys(got, want):
+    cc.check_phys(got, want, 4)
+    if np.size(got) >= 128:
+        assert np.mean(got == want) >= 0.75, np.mean(got == want)        # most components agree to the last bit
 
 
 @pytest.mark.parametrize("N", [1, 33, 4099])
@@ -72,12 +44,12 @@ def test_step_matches_oracle(N, reward_scale):
     a[pick == 3] = rs.choice([1.5, -1.5, 3.0, -7.0], int((pick == 3).sum()))
     el = rs.randint(0, 200, N)
     el[rs.rand(N) < 0.3] = 199
-    ph, obs, r, d, tl, el2, err, any_reset = _step_kernel(phys, a, el, reward_scale)
+    ph, obs, r, d, tl, el2, err, any_reset = cc.step_kernel(_case(), phys, a, el, reward_scale, 200)
     wph, wobs, wr, wd, wtl, wel = P.step(phys, a, el, reward_scale=reward_scale)
     assert err == 0
     _check_phys(ph, wph)
-    _check_obs(obs, wobs)
-    _check_obs(obs, P.observe(ph))
+    cc.check_obs(obs, wobs)
+    cc.check_obs(obs, P.observe(ph))
     np.testing.assert_array_equal(r, wr)
     np.testing.assert_array_equal(el2, wel)
     np.testing.assert_array_equal(d, wd)
@@ -88,7 +60,7 @@ def test_step_matches_oracle(N, reward_scale):
 
 
 def test_step_from_the_rest_state():
-    ph, obs, r, *_ = _step_kernel(np.zeros((3, 2)), [1.0, -1.0, 0.0], [0, 0, 0])
+    ph, obs, r, *_ = cc.step_kernel(_case(), np.zeros((3, 2)), [1.0, -1.0, 0.0], [0, 0, 0], max_steps=200)
     assert ph.tolist() == [[0.30000000000000004 * 0.05, 0.30000000000000004], [-0.015000000000000003,
                                                                                -0.30000000000000004], [0.0, 0.0]]
     assert r.tolist() == np.float32([-0.004, -0.004, 0.0]).tolist()
@@ -104,7 +76,7 @@ def test_reset_seeding_and_sharding():
     seeds = 5 * 2 * N + np.arange(2 * N)
     want = P.reset_phys(seeds, np.zeros(2 * N))
     np.testing.assert_array_equal(env.phys.cpu().numpy(), want)
-    _check_obs(full, P.observe(want))
+    cc.check_obs(full, P.observe(want))
     parts, pphys = [], []
     for r in range(2):
         e = get_vec_env("Pendulum-v1", {}, N, first_env=r * N, total_envs=2 * N)
@@ -124,7 +96,7 @@ def test_reset_seeding_and_sharding():
     np.testing.assert_array_equal(after[~m], before[~m])
     np.testing.assert_array_equal(raw[~m], before_obs[~m])
     np.testing.assert_array_equal(after[m], P.reset_phys(seeds[m], np.full(m.sum(), 2)))
-    _check_obs(raw[m], P.observe(after[m]))
+    cc.check_obs(raw[m], P.observe(after[m]))
 
 
 def test_rollout_tracks_the_oracle_step_by_step():
@@ -149,7 +121,7 @@ def test_rollout_tracks_the_oracle_step_by_step():
         wph, wobs, wr, wd, wtl, wel = P.step(phys, a, el, reward_scale=0.1)
         got = env.phys.cpu().numpy().copy()
         _check_phys(got, wph)
-        _check_obs(obs.cpu().numpy(), wobs)
+        cc.check_obs(obs.cpu().numpy(), wobs)
         np.testing.assert_array_equal(r.cpu().numpy().reshape(-1), wr)
         d = done.cpu().numpy().reshape(-1)
         np.testing.assert_array_equal(d, wd)
@@ -288,7 +260,7 @@ def test_collector_resets_cut_episodes(quirks):
     for t in range(T - 1):
         if (t + 1) % 5 == 0:                                      # rows 4, 9: the step that cut every env
             want = P.observe(P.reset_phys(seeds, np.full(N, ep)))
-            _check_obs(obs[t + 1], want)
+            cc.check_obs(obs[t + 1], want)
             ep += 1
         else:
             np.testing.assert_array_equal(obs[t + 1], nxt[t])
@@ -311,77 +283,10 @@ def test_collector_step_graph_launch_count():
 
 
 # ------------------------------------------------------------------------------------------ agents
-def _agent(kind, N=16, seed=0, use_graph=True):
-    import torch
-    import torch.nn as nn
-    import torchrl_b200.networks as networks
-    import torchrl_b200.policies as policies
-    from torchrl_b200.algo import DDPG, PPO, SAC, TD3, TwinSACQ
-    from torchrl_b200.collector import VecCollector, VecOnPolicyCollector
-    from torchrl_b200.env import get_vec_env
-    from torchrl_b200.replay_buffers import BaseReplayBuffer, OnPolicyReplayBuffer
-    from torchrl_b200.utils import NullLogger
-    dev = torch.device("cuda:0")
-    env = get_vec_env("Pendulum-v1", {"reward_scale": 1, "obs_norm": kind == "ppo"}, N)
-    eval_env = get_vec_env("Pendulum-v1", {"reward_scale": 1, "obs_norm": kind == "ppo"}, N)
-    env.seed(seed); eval_env.seed(seed + 1000); torch.manual_seed(seed); np.random.seed(seed)
-    o, a = 3, 1
-    net = dict(hidden_shapes=[64, 64], append_hidden_shapes=[], base_type=networks.MLPBase, activation_func=nn.ReLU)
-    T = 40
-    if kind == "ppo":
-        buf = OnPolicyReplayBuffer(env_nums=N, max_replay_buffer_size=T * N, time_limit_filter=True)
-        pf = policies.GuassianContPolicyBasicBias(input_shape=o, output_shape=a, tanh_action=True, **net)
-        vf = networks.Net(input_shape=o, output_shape=1, **net)
-        col = VecOnPolicyCollector(vf, env=env, eval_env=eval_env, pf=pf, replay_buffer=buf, device=dev,
-                                   epoch_frames=T * N, max_episode_frames=200, use_cuda_graph=use_graph)
-        return PPO(pf=pf, vf=vf, plr=3e-4, vlr=3e-4, clip_para=0.2, opt_epochs=2, tau=0.95, shuffle=True, env=env,
-                   replay_buffer=buf, collector=col, logger=NullLogger(), discount=0.99, num_epochs=3,
-                   batch_size=10 * N, gae=True, device=dev, save_dir=None, use_cuda_graph=use_graph), col, buf, env
-    buf = BaseReplayBuffer(env_nums=N, max_replay_buffer_size=4 * T * N, time_limit_filter=False)
-    if kind in ("sac", "twin_sac_q"):
-        pf = policies.GuassianContPolicy(input_shape=o, output_shape=2 * a, tanh_action=True, **net)
-    elif kind == "ddpg":
-        pf = policies.DetContPolicy(input_shape=o, output_shape=a, tanh_action=True, **net)
-    else:
-        pf = policies.FixGuassianContPolicy(input_shape=o, output_shape=a, tanh_action=True, norm_std_explore=0.1,
-                                            **net)
-    qf1 = networks.QNet(input_shape=o + a, output_shape=1, **net)
-    col = VecCollector(env=env, eval_env=eval_env, pf=pf, replay_buffer=buf, device=dev, epoch_frames=T * N,
-                       max_episode_frames=200, use_cuda_graph=use_graph)
-    common = dict(env=env, replay_buffer=buf, collector=col, logger=NullLogger(), discount=0.99, batch_size=8 * N,
-                  device=dev, save_dir=None, tau=0.005, use_soft_update=True, opt_times=8, pretrain_epochs=1,
-                  num_epochs=3, use_cuda_graph=use_graph)
-    if kind == "td3":
-        qf2 = networks.QNet(input_shape=o + a, output_shape=1, **net)
-        agent = TD3(pf=pf, qf1=qf1, qf2=qf2, plr=1e-3, qlr=1e-3, **common)
-    elif kind == "ddpg":
-        agent = DDPG(pf=pf, qf=qf1, plr=1e-3, qlr=1e-3, **common)
-    elif kind == "twin_sac_q":
-        qf2 = networks.QNet(input_shape=o + a, output_shape=1, **net)
-        agent = TwinSACQ(pf=pf, qf1=qf1, qf2=qf2, plr=3e-4, qlr=3e-4, policy_std_reg_weight=0,
-                         policy_mean_reg_weight=0, **common)
-    else:
-        vf = networks.Net(input_shape=o, output_shape=1, **net)
-        agent = SAC(pf=pf, vf=vf, qf=qf1, plr=3e-4, vlr=3e-4, qlr=3e-4, policy_std_reg_weight=1e-3,
-                    policy_mean_reg_weight=1e-3, **common)
-    return agent, col, buf, env
-
-
 @pytest.mark.parametrize("kind", ["td3", "ddpg", "sac", "twin_sac_q", "ppo"])
 def test_one_epoch_of_each_agent(kind):
-    agent, col, buf, env = _agent(kind)
-    if kind != "ppo":
-        agent.pretrain()
-    agent.current_epoch = 0
-    out = col.train_one_epoch()
-    agent.update_per_epoch()
-    assert agent._last_infos
-    for info in agent._last_infos:
-        for k, v in info.items():
-            if kind == "ppo" and k == "log_std/std":      # the reference's torch std of PPO's one log-std: NaN
-                assert np.isnan(v)
-            else:
-                assert np.isfinite(v), k
+    agent, col, buf, env = cc.continuous_agent("Pendulum-v1", kind, 3, 200, False)
+    out = cc.one_epoch(agent, col, kind, kind != "ppo")
     assert all(-16.3 * 200 <= r <= 0 for r in out["train_rewards"])     # the cost is at most pi^2 + 6.4 + 0.004
     acts = buf._acts.cpu().numpy()
     assert np.all(np.abs(acts[:buf._size]) <= 1.0)
@@ -401,13 +306,13 @@ def test_td3_resume_continues_identically(tmp_path):
             agent.update_per_epoch()
         return out
 
-    agent, col, buf, env = _agent("td3", seed=1, use_graph=False)
+    agent, col, buf, env = cc.continuous_agent("Pendulum-v1", "td3", 3, 200, False, use_graph=False, seed=1)
     agent.pretrain()
     epochs(agent, col, 0, 3)                                      # 3 x 40 steps: mid-episode at the checkpoint
     agent.save_checkpoint(path)
     want_r = epochs(agent, col, 3, 3)
     want, want_t, want_phys = agent.opt.data.clone(), agent._target_flat.data.clone(), env.phys.clone()
-    agent2, col2, buf2, env2 = _agent("td3", seed=77, use_graph=False)
+    agent2, col2, buf2, env2 = cc.continuous_agent("Pendulum-v1", "td3", 3, 200, False, use_graph=False, seed=77)
     assert agent2.load_checkpoint(path) == 3
     got_r = epochs(agent2, col2, 3, 3)
     np.testing.assert_allclose(got_r, want_r, rtol=1e-6)

@@ -13,13 +13,12 @@
 // once in gym's evaluation order (explicit __dadd_rn / __dmul_rn / __ddiv_rn, so -fmad=true cannot contract them); the
 // observation (cos theta1, sin theta1, cos theta2, sin theta2, dtheta1, dtheta2) is rounded to fp32 once.
 //
-// Layout: phys (N,4) fp64, obs (N,6) fp32 raw observation; one thread per env, kAcroThreads envs per CTA.  The reset has
-// its own kernel because the observation is not the state: collect_finalize's in-kernel reset cannot serve it.
+// Layout: phys (N,4) fp64, obs (N,6) fp32 raw observation; one thread per env (env_step_kernel<Acrobot>).  The reset has
+// its own kernel (env_reset_kernel<Acrobot>) because the observation is not the state: collect_finalize's in-kernel
+// reset cannot serve it.
 #include "env_common.cuh"
 
 namespace trl {
-
-constexpr int kAcroThreads = 256;
 
 // gym's AcrobotEnv constants (classic_control/acrobot.py)
 constexpr double kAcroDt = 0.2;
@@ -109,7 +108,18 @@ __device__ __forceinline__ void acrobot_dynamics(double (&s)[4], double a) {
 }
 
 struct Acrobot {
+  using State = double;
   static constexpr int kPhys = 4, kObs = 6;
+  // 0.0, 1.0 or 2.0: torque -1, 0, +1
+  static __device__ __forceinline__ bool accepts(float a) { return a == 0.0f || a == 1.0f || a == 2.0f; }
+  // _terminal: -cos(theta1) - cos(theta2 + theta1) > 1; reward -1, or 0 on the terminal step
+  static __device__ __forceinline__ double step(double (&s)[kPhys], float a, bool& terminal) {
+    acrobot_dynamics(s, static_cast<double>(a) - 1.0);
+    terminal = __dadd_rn(-cos(s[0]), -cos(__dadd_rn(s[1], s[0]))) > 1.0;
+    return terminal ? 0.0 : -1.0;
+  }
+  // not an Acrobot action: reward 0, no terminal, and the state and observation stay where they were
+  static __device__ __forceinline__ float refused(const double (&)[kPhys], float, bool&) { return 0.f; }
   // every state component from U(-0.1, 0.1): 0.1 (2U - 1) in fp64 from the counter hash of (seed, episode, component)
   static __device__ __forceinline__ void reset_state(unsigned seed, unsigned ep, double (&s)[kPhys]) {
 #pragma unroll
@@ -126,87 +136,30 @@ struct Acrobot {
   }
 };
 
-struct AcrobotParams {
-  double* __restrict__ phys;            // (N,4) in/out: theta1, theta2, dtheta1, dtheta2
-  float* __restrict__ obs;              // (N,6) out: raw observation
-  const float* __restrict__ actions;    // (N) 0.0, 1.0 or 2.0 (torque -1, 0, +1)
-  int* __restrict__ action_error;       // (1) set to 1 when an action is none of these
-  EnvStepFields env;                    // D = 6
-};
-
-__global__ void __launch_bounds__(kAcroThreads) acrobot_step_kernel(const AcrobotParams p) {
-  const EnvStepFields& f = p.env;
-  const long long n = static_cast<long long>(blockIdx.x) * kAcroThreads + threadIdx.x;
-  float ob[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  bool local_reset = false;
-  if (n < f.N) {
-    const float a = p.actions[n];
-    bool terminal = false;
-    float r = 0.f;
-    if (a == 0.0f || a == 1.0f || a == 2.0f) {
-      double s[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) s[j] = p.phys[n * 4 + j];
-      acrobot_dynamics(s, static_cast<double>(a) - 1.0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) p.phys[n * 4 + j] = s[j];
-      Acrobot::observe(s, ob);
-      // _terminal: -cos(theta1) - cos(theta2 + theta1) > 1; reward -1, or 0 on the terminal step
-      terminal = __dadd_rn(-cos(s[0]), -cos(__dadd_rn(s[1], s[0]))) > 1.0;
-      r = static_cast<float>(__dmul_rn(terminal ? 0.0 : -1.0, static_cast<double>(f.reward_scale)));
-    } else {
-      // not an Acrobot action: flag it for the host and leave this env's state and observation where they were
-      atomicOr(p.action_error, 1);
-#pragma unroll
-      for (int j = 0; j < 6; ++j) ob[j] = p.obs[n * 6 + j];
-    }
-#pragma unroll
-    for (int j = 0; j < 6; ++j) p.obs[n * 6 + j] = ob[j];
-    local_reset = env_row_end(f, n, terminal, r);
-  }
-  update_any_reset(f, local_reset);
-  if (f.partial) env_moments<6, kAcroThreads>(f, ob);
-}
-
-__global__ void __launch_bounds__(kAcroThreads) acrobot_reset_kernel(const SelfResetParams p) {
-  env_self_reset<Acrobot>(p, static_cast<long long>(blockIdx.x) * kAcroThreads + threadIdx.x);
-}
-
 }  // namespace trl
 
-TRL_API int trl_acrobot_num_ctas(int64_t N) {
-  return static_cast<int>((N + trl::kAcroThreads - 1) / trl::kAcroThreads);
-}
+TRL_API int trl_acrobot_num_ctas(int64_t N) { return trl::env_row_ctas(N); }
 
 TRL_API int trl_acrobot_step(double* phys, float* obs, const float* actions, int* elapsed, const int* step_count,
                              float* reward, uint8_t* done, uint8_t* time_limit, int* action_error, double* partial,
                              double* batch_sums, double* norm_mean, double* norm_var, double* norm_count,
                              unsigned* ticket, int* any_reset, const int* t_ptr, int64_t N, float reward_scale,
                              int max_episode_steps, int max_episode_frames, int merge_stats, void* stream) {
-  using namespace trl;
-  TRL_REQUIRE(N >= 0 && max_episode_steps >= 1, "trl_acrobot_step: bad sizes N=%lld max_episode_steps=%d",
-              (long long)N, max_episode_steps);
-  if (N == 0) return TRL_OK;
-  TRL_REQUIRE(phys && obs && actions && elapsed && reward && done && time_limit && action_error,
-              "trl_acrobot_step: null pointer");
-  AcrobotParams p{phys, obs, actions, action_error,
-                  {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean, norm_var, norm_count,
-                   ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps, max_episode_frames, merge_stats}};
-  if (const int e = check_env_step("trl_acrobot_step", p.env)) return e;
-  acrobot_step_kernel<<<trl_acrobot_num_ctas(N), kAcroThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("acrobot_step_kernel");
+  return trl::launch_env_step<trl::Acrobot>(
+      "trl_acrobot_step", "acrobot_step_kernel",
+      {phys, obs, actions, action_error,
+       {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean, norm_var, norm_count, ticket,
+        any_reset, t_ptr, N, reward_scale, max_episode_steps, max_episode_frames, merge_stats}},
+      stream);
 }
 
 TRL_API int trl_acrobot_reset(double* phys, float* obs, int* elapsed, unsigned* episode, const unsigned* seeds,
                               const uint8_t* mask, const int* step_count, const float* next_norm, float* cur_ob,
                               const int* any_reset, const int* t_ptr, const double* norm_mean, const double* norm_var,
                               int64_t N, double clip, int raw_obs_after_reset, void* stream) {
-  using namespace trl;
-  TRL_REQUIRE(N >= 0, "trl_acrobot_reset: bad size N=%lld", (long long)N);
-  if (N == 0) return TRL_OK;
-  SelfResetParams p{phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset, t_ptr,
-                    norm_mean, norm_var, N, clip, raw_obs_after_reset};
-  if (const int e = check_self_reset("trl_acrobot_reset", p)) return e;
-  acrobot_reset_kernel<<<trl_acrobot_num_ctas(N), kAcroThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("acrobot_reset_kernel");
+  return trl::launch_env_reset<trl::Acrobot>(
+      "trl_acrobot_reset", "acrobot_reset_kernel",
+      {phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset, t_ptr, norm_mean, norm_var,
+       N, clip, raw_obs_after_reset},
+      stream);
 }

@@ -1,10 +1,17 @@
 // env_common.cuh -- what the device env kernels share: the reset counter hash, the fields and bookkeeping of a step
-// (TimeLimitAugment, the collector's reset flag, NormObs's batch moments) and the collector's next-observation rule.
-// Each env's .cu file keeps its physics, its parameter struct and its launch.
+// (TimeLimitAugment, the collector's reset flag, NormObs's batch moments), the collector's next-observation rule, and
+// the step and own-reset kernels of the one-thread-per-env classic-control envs with their launches.  Each of those
+// envs' .cu files keeps its physics in an env struct (see env_step_kernel) and its literal TRL_API entry points.
 #pragma once
+#include <type_traits>
+
 #include "reduce.cuh"
 
 namespace trl {
+
+// block size of the kernels that run one thread per env
+constexpr int kEnvRowThreads = 256;
+inline int env_row_ctas(int64_t N) { return static_cast<int>((N + kEnvRowThreads - 1) / kEnvRowThreads); }
 
 // ---- the reset counter hash (oracle/synth_env.py:hash_uniform) ------------------------------------------------------
 __host__ __device__ __forceinline__ uint32_t counter_hash(uint32_t seed, uint32_t episode, uint32_t j) {
@@ -146,10 +153,83 @@ __device__ __forceinline__ float next_observation(bool all_raw, bool normalise, 
   return static_cast<float>(fmin(fmax(y, -clip), clip));
 }
 
+// ---- the step of a classic-control env: one thread per env --------------------------------------------------------
+// Env supplies its physics:
+//   using State = double or float;     the physical state's type (float: CartPole, whose fp32 state is its observation)
+//   static constexpr int kPhys, kObs;  state and observation widths
+//   static __device__ bool accepts(float a);
+//   static __device__ double step(State (&s)[kPhys], float a, bool& terminal);  advances s, returns the unscaled reward
+//   static __device__ float refused(const State (&s)[kPhys], float reward_scale, bool& terminal);
+//                                      the reward (and terminal) of a row whose action was refused; its state stays
+//   static __device__ void observe(const State (&s)[kPhys], float (&o)[kObs]);
+template <class State>
+struct EnvStepParams {
+  State* __restrict__ phys;             // (N, kPhys) in/out physical state; for a float State the same array as obs,
+                                        // which the kernel reads and writes it through
+  float* __restrict__ obs;              // (N, kObs) in/out raw observation
+  const float* __restrict__ actions;    // (N) one action per env
+  int* __restrict__ action_error;       // (1) set to 1 when an action is refused
+  EnvStepFields env;                    // D = kObs
+};
+
+// A refused action is flagged for the host; the observation is reloaded (a float State is the observation itself) and
+// only the env's refused() decides the row's reward and terminal.
+template <class Env>
+__global__ void __launch_bounds__(kEnvRowThreads) env_step_kernel(const EnvStepParams<typename Env::State> p) {
+  constexpr int P = Env::kPhys, D = Env::kObs;
+  constexpr bool kStateIsObs = std::is_same_v<typename Env::State, float>;
+  const EnvStepFields& f = p.env;
+  const long long n = static_cast<long long>(blockIdx.x) * kEnvRowThreads + threadIdx.x;
+  float ob[D] = {};
+  bool local_reset = false;
+  if (n < f.N) {
+    typename Env::State s[P];
+#pragma unroll
+    for (int j = 0; j < P; ++j) s[j] = kStateIsObs ? p.obs[n * D + j] : p.phys[n * P + j];
+    const float a = p.actions[n];
+    bool terminal = false;
+    float r;
+    if (Env::accepts(a)) {
+      // one rounded fp64 product (nothing is added to it, so it cannot contract); CartPole's x 1.0 folds away
+      r = static_cast<float>(Env::step(s, a, terminal) * static_cast<double>(f.reward_scale));
+      if constexpr (!kStateIsObs) {
+#pragma unroll
+        for (int j = 0; j < P; ++j) p.phys[n * P + j] = s[j];
+      }
+      Env::observe(s, ob);
+    } else {
+      atomicOr(p.action_error, 1);
+      r = Env::refused(s, f.reward_scale, terminal);
+#pragma unroll
+      for (int j = 0; j < D; ++j) ob[j] = kStateIsObs ? s[j] : p.obs[n * D + j];
+    }
+#pragma unroll
+    for (int j = 0; j < D; ++j) p.obs[n * D + j] = ob[j];
+    local_reset = env_row_end(f, n, terminal, r);
+  }
+  update_any_reset(f, local_reset);
+  if (f.partial) env_moments<D, kEnvRowThreads>(f, ob);
+}
+
+// The body of a trl_<env>_step entry point `fn` after it has gathered its arguments: the argument checks, then the
+// launch of env_step_kernel<Env>; `kernel` names it in a launch error.
+template <class Env>
+int launch_env_step(const char* fn, const char* kernel, const EnvStepParams<typename Env::State>& p, void* stream) {
+  const EnvStepFields& f = p.env;
+  TRL_REQUIRE(f.N >= 0 && f.max_episode_steps >= 1, "%s: bad sizes N=%lld max_episode_steps=%d", fn, f.N,
+              f.max_episode_steps);
+  if (f.N == 0) return TRL_OK;
+  TRL_REQUIRE(p.phys && p.obs && p.actions && f.elapsed && f.reward && f.done && f.time_limit && p.action_error,
+              "%s: null pointer", fn);
+  if (const int e = check_env_step(fn, f)) return e;
+  env_step_kernel<Env><<<env_row_ctas(f.N), kEnvRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch(kernel);
+}
+
 // ---- the own reset of an env whose observation is not its state -----------------------------------------------------
-// An fp64 physical state (N, Env::kPhys) and its fp32 raw observation (N, Env::kObs).  Env supplies
+// An fp64 physical state (N, Env::kPhys) and its fp32 raw observation (N, Env::kObs).  Env supplies, besides the
+// physics of env_step_kernel,
 //   static __device__ void reset_state(unsigned seed, unsigned episode, double (&s)[kPhys]);
-//   static __device__ void observe(const double (&s)[kPhys], float (&o)[kObs]);
 struct SelfResetParams {
   double* __restrict__ phys;              // (N, kPhys)
   float* __restrict__ obs;                // (N, kObs) raw observation
@@ -169,16 +249,6 @@ struct SelfResetParams {
   double clip;
   int raw_obs_after_reset;                // reference quirk A.1 (SURVEY.md): raw obs for ALL envs after any reset
 };
-
-// The reset arguments' rules; `fn` names the entry point in the message.
-inline int check_self_reset(const char* fn, const SelfResetParams& p) {
-  TRL_REQUIRE(p.phys && p.obs && p.elapsed && p.episode && p.seeds, "%s: null pointer", fn);
-  TRL_REQUIRE(!(p.mask && p.step_count), "%s: select envs by mask or by step_count, not both", fn);
-  TRL_REQUIRE(!p.cur_ob || (p.step_count && p.next_norm && p.any_reset && p.t_ptr),
-              "%s: cur_ob needs step_count, next_norm, any_reset and t_ptr", fn);
-  TRL_REQUIRE(!p.norm_mean || p.norm_var, "%s: norm_mean given without norm_var", fn);
-  return TRL_OK;
-}
 
 // Env n's reset: selected by step_count == 0, else by mask, else always.  A selected env gets a new state from the
 // counter hash of (seed, episode), its raw observation, elapsed = 0 and episode += 1.  With cur_ob, every env's next
@@ -211,6 +281,26 @@ __device__ __forceinline__ void env_self_reset(const SelfResetParams& p, long lo
     p.cur_ob[n * D + j] =
         next_observation(all_raw, sel, raw[j], p.next_norm + n * D + j, p.norm_mean, p.norm_var, j, p.clip);
   }
+}
+
+template <class Env>
+__global__ void __launch_bounds__(kEnvRowThreads) env_reset_kernel(const SelfResetParams p) {
+  env_self_reset<Env>(p, static_cast<long long>(blockIdx.x) * kEnvRowThreads + threadIdx.x);
+}
+
+// The body of a trl_<env>_reset entry point `fn` after it has gathered its arguments: the argument checks, then the
+// launch of env_reset_kernel<Env>; `kernel` names it in a launch error.
+template <class Env>
+int launch_env_reset(const char* fn, const char* kernel, const SelfResetParams& p, void* stream) {
+  TRL_REQUIRE(p.N >= 0, "%s: bad size N=%lld", fn, p.N);
+  if (p.N == 0) return TRL_OK;
+  TRL_REQUIRE(p.phys && p.obs && p.elapsed && p.episode && p.seeds, "%s: null pointer", fn);
+  TRL_REQUIRE(!(p.mask && p.step_count), "%s: select envs by mask or by step_count, not both", fn);
+  TRL_REQUIRE(!p.cur_ob || (p.step_count && p.next_norm && p.any_reset && p.t_ptr),
+              "%s: cur_ob needs step_count, next_norm, any_reset and t_ptr", fn);
+  TRL_REQUIRE(!p.norm_mean || p.norm_var, "%s: norm_mean given without norm_var", fn);
+  env_reset_kernel<Env><<<env_row_ctas(p.N), kEnvRowThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  return check_launch(kernel);
 }
 
 }  // namespace trl

@@ -8,7 +8,7 @@
 //   RewardShift.reward                                                        /root/reference/torchrl/env/base_wrapper.py:37-41
 //   VecEnv.step / partial_reset                                               /root/reference/torchrl/env/vecenv.py:47-61
 // and, like csrc/pendulum.cu, accumulates the batch moments NormObs needs (base_wrapper.py:75-82, :44-60).
-// One kernel serves both ids; the variant is a template parameter chosen by the entry point's `continuous` flag.
+// One env struct serves both ids; the variant is a template parameter chosen by the entry point's `continuous` flag.
 // oracle/mountain_car.py is the NumPy statement this file must agree with.
 //
 // Precision: the physical state (position, velocity) is fp64; the continuous force is NormAct's affine map evaluated in
@@ -16,13 +16,12 @@
 // (NumPy 1.x promotion); every fp64 operation is rounded once in gym's order; observation and reward are rounded to fp32
 // once.
 //
-// Layout: phys (N,2) fp64, obs (N,2) fp32 raw observation; one thread per env, kCarThreads envs per CTA.  The reset has
-// its own kernel because the observation is not the state (it is the fp32 rounding of it).
+// Layout: phys (N,2) fp64, obs (N,2) fp32 raw observation; one thread per env (env_step_kernel<MountainCar<...>>).  The
+// reset has its own kernel (env_reset_kernel<MountainCar<false>>, for both ids) because the observation is not the
+// state (it is the fp32 rounding of it).
 #include "env_common.cuh"
 
 namespace trl {
-
-constexpr int kCarThreads = 256;
 
 // gym's MountainCarEnv / Continuous_MountainCarEnv constants (classic_control/mountain_car.py,
 // continuous_mountain_car.py)
@@ -42,8 +41,36 @@ __device__ __forceinline__ float car_action(float a) {
   return fminf(fmaxf(u, lb), ub);
 }
 
+template <bool kContinuous>
 struct MountainCar {
+  using State = double;
   static constexpr int kPhys = 2, kObs = 2;
+  // v0: 0.0, 1.0 or 2.0; continuous: policy-space actions, finite
+  static __device__ __forceinline__ bool accepts(float a) {
+    return kContinuous ? isfinite(a) : (a == 0.0f || a == 1.0f || a == 2.0f);
+  }
+  // v0: -1 per step; continuous: 100 on reaching the goal, minus 0.1 * action[0]**2
+  static __device__ __forceinline__ double step(double (&s)[kPhys], float a, bool& terminal) {
+    double pos = s[0], vel = s[1];
+    const double c = cos(__dmul_rn(3.0, pos));
+    double act = 0.0;                       // the continuous env's action[0], widened exactly
+    if (kContinuous) {
+      act = static_cast<double>(car_action(a));
+      const double force = fmin(fmax(act, -1.0), 1.0);
+      vel = __dadd_rn(vel, __dadd_rn(__dmul_rn(force, kCarPower), -__dmul_rn(kCarGravity, c)));
+    } else {
+      vel = __dadd_rn(vel, __dadd_rn(__dmul_rn(static_cast<double>(a) - 1.0, kCarForce), __dmul_rn(c, -kCarGravity)));
+    }
+    vel = fmin(fmax(vel, -kCarMaxSpeed), kCarMaxSpeed);
+    pos = fmin(fmax(__dadd_rn(pos, vel), kCarMinPosition), kCarMaxPosition);
+    if (pos == kCarMinPosition && vel < 0.0) vel = 0.0;       // the left wall stops the car
+    terminal = pos >= (kContinuous ? kCarGoalCont : kCarGoalV0) && vel >= 0.0;
+    s[0] = pos;
+    s[1] = vel;
+    return kContinuous ? __dadd_rn(terminal ? 100.0 : 0.0, -__dmul_rn(__dmul_rn(act, act), 0.1)) : -1.0;
+  }
+  // not an action of this env: reward 0, no terminal, and the state and observation stay where they were
+  static __device__ __forceinline__ float refused(const double (&)[kPhys], float, bool&) { return 0.f; }
   // position from U(-0.6, -0.4) as -0.6 + 0.2 U in fp64 from the counter hash of (seed, episode, 0); velocity 0
   static __device__ __forceinline__ void reset_state(unsigned seed, unsigned ep, double (&s)[kPhys]) {
     s[0] = __dadd_rn(-0.6, __dmul_rn(0.2, double(counter_uniform(seed, ep, 0))));
@@ -55,69 +82,9 @@ struct MountainCar {
   }
 };
 
-struct MountainCarParams {
-  double* __restrict__ phys;            // (N,2) in/out: position, velocity
-  float* __restrict__ obs;              // (N,2) out: raw observation
-  const float* __restrict__ actions;    // (N) v0: 0.0, 1.0 or 2.0; continuous: policy-space actions, finite
-  int* __restrict__ action_error;       // (1) set to 1 when an action is refused
-  EnvStepFields env;                    // D = 2
-};
-
-template <bool kContinuous>
-__global__ void __launch_bounds__(kCarThreads) mountain_car_step_kernel(const MountainCarParams p) {
-  const EnvStepFields& f = p.env;
-  const long long n = static_cast<long long>(blockIdx.x) * kCarThreads + threadIdx.x;
-  float ob[2] = {0.f, 0.f};
-  bool local_reset = false;
-  if (n < f.N) {
-    const float a = p.actions[n];
-    bool terminal = false;
-    float r = 0.f;
-    if (kContinuous ? isfinite(a) : (a == 0.0f || a == 1.0f || a == 2.0f)) {
-      double pos = p.phys[n * 2], vel = p.phys[n * 2 + 1];
-      const double c = cos(__dmul_rn(3.0, pos));
-      double act = 0.0;                       // the continuous env's action[0], widened exactly
-      if (kContinuous) {
-        act = static_cast<double>(car_action(a));
-        const double force = fmin(fmax(act, -1.0), 1.0);
-        vel = __dadd_rn(vel, __dadd_rn(__dmul_rn(force, kCarPower), -__dmul_rn(kCarGravity, c)));
-      } else {
-        vel = __dadd_rn(vel, __dadd_rn(__dmul_rn(static_cast<double>(a) - 1.0, kCarForce), __dmul_rn(c, -kCarGravity)));
-      }
-      vel = fmin(fmax(vel, -kCarMaxSpeed), kCarMaxSpeed);
-      pos = fmin(fmax(__dadd_rn(pos, vel), kCarMinPosition), kCarMaxPosition);
-      if (pos == kCarMinPosition && vel < 0.0) vel = 0.0;       // the left wall stops the car
-      terminal = pos >= (kContinuous ? kCarGoalCont : kCarGoalV0) && vel >= 0.0;
-      p.phys[n * 2] = pos;
-      p.phys[n * 2 + 1] = vel;
-      ob[0] = static_cast<float>(pos);
-      ob[1] = static_cast<float>(vel);
-      // v0: -1 per step; continuous: 100 on reaching the goal, minus 0.1 * action[0]**2
-      const double base = kContinuous ? __dadd_rn(terminal ? 100.0 : 0.0, -__dmul_rn(__dmul_rn(act, act), 0.1)) : -1.0;
-      r = static_cast<float>(__dmul_rn(base, static_cast<double>(f.reward_scale)));
-    } else {
-      // not an action of this env: flag it for the host and leave this env's state and observation where they were
-      atomicOr(p.action_error, 1);
-#pragma unroll
-      for (int j = 0; j < 2; ++j) ob[j] = p.obs[n * 2 + j];
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) p.obs[n * 2 + j] = ob[j];
-    local_reset = env_row_end(f, n, terminal, r);
-  }
-  update_any_reset(f, local_reset);
-  if (f.partial) env_moments<2, kCarThreads>(f, ob);
-}
-
-__global__ void __launch_bounds__(kCarThreads) mountain_car_reset_kernel(const SelfResetParams p) {
-  env_self_reset<MountainCar>(p, static_cast<long long>(blockIdx.x) * kCarThreads + threadIdx.x);
-}
-
 }  // namespace trl
 
-TRL_API int trl_mountain_car_num_ctas(int64_t N) {
-  return static_cast<int>((N + trl::kCarThreads - 1) / trl::kCarThreads);
-}
+TRL_API int trl_mountain_car_num_ctas(int64_t N) { return trl::env_row_ctas(N); }
 
 TRL_API int trl_mountain_car_step(double* phys, float* obs, const float* actions, int* elapsed, const int* step_count,
                                   float* reward, uint8_t* done, uint8_t* time_limit, int* action_error,
@@ -126,24 +93,16 @@ TRL_API int trl_mountain_car_step(double* phys, float* obs, const float* actions
                                   float reward_scale, int max_episode_steps, int max_episode_frames, int merge_stats,
                                   int continuous, void* stream) {
   using namespace trl;
-  TRL_REQUIRE(N >= 0 && max_episode_steps >= 1, "trl_mountain_car_step: bad sizes N=%lld max_episode_steps=%d",
-              (long long)N, max_episode_steps);
-  TRL_REQUIRE(continuous == 0 || continuous == 1, "trl_mountain_car_step: continuous must be 0 or 1, got %d",
-              continuous);
-  if (N == 0) return TRL_OK;
-  TRL_REQUIRE(phys && obs && actions && elapsed && reward && done && time_limit && action_error,
-              "trl_mountain_car_step: null pointer");
-  MountainCarParams p{phys, obs, actions, action_error,
-                      {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean, norm_var,
-                       norm_count, ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps, max_episode_frames,
-                       merge_stats}};
-  if (const int e = check_env_step("trl_mountain_car_step", p.env)) return e;
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (continuous)
-    mountain_car_step_kernel<true><<<trl_mountain_car_num_ctas(N), kCarThreads, 0, s>>>(p);
-  else
-    mountain_car_step_kernel<false><<<trl_mountain_car_num_ctas(N), kCarThreads, 0, s>>>(p);
-  return check_launch("mountain_car_step_kernel");
+  // refused after bad sizes (launch_env_step's first check) and before everything else
+  TRL_REQUIRE(continuous == 0 || continuous == 1 || N < 0 || max_episode_steps < 1,
+              "trl_mountain_car_step: continuous must be 0 or 1, got %d", continuous);
+  const EnvStepParams<double> p{phys, obs, actions, action_error,
+                                {elapsed, step_count, reward, done, time_limit, partial, batch_sums, norm_mean,
+                                 norm_var, norm_count, ticket, any_reset, t_ptr, N, reward_scale, max_episode_steps,
+                                 max_episode_frames, merge_stats}};
+  return continuous == 1
+             ? launch_env_step<MountainCar<true>>("trl_mountain_car_step", "mountain_car_step_kernel", p, stream)
+             : launch_env_step<MountainCar<false>>("trl_mountain_car_step", "mountain_car_step_kernel", p, stream);
 }
 
 TRL_API int trl_mountain_car_reset(double* phys, float* obs, int* elapsed, unsigned* episode, const unsigned* seeds,
@@ -151,12 +110,9 @@ TRL_API int trl_mountain_car_reset(double* phys, float* obs, int* elapsed, unsig
                                    const int* any_reset, const int* t_ptr, const double* norm_mean,
                                    const double* norm_var, int64_t N, double clip, int raw_obs_after_reset,
                                    void* stream) {
-  using namespace trl;
-  TRL_REQUIRE(N >= 0, "trl_mountain_car_reset: bad size N=%lld", (long long)N);
-  if (N == 0) return TRL_OK;
-  SelfResetParams p{phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset, t_ptr,
-                    norm_mean, norm_var, N, clip, raw_obs_after_reset};
-  if (const int e = check_self_reset("trl_mountain_car_reset", p)) return e;
-  mountain_car_reset_kernel<<<trl_mountain_car_num_ctas(N), kCarThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  return check_launch("mountain_car_reset_kernel");
+  return trl::launch_env_reset<trl::MountainCar<false>>(
+      "trl_mountain_car_reset", "mountain_car_reset_kernel",
+      {phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset, t_ptr, norm_mean, norm_var,
+       N, clip, raw_obs_after_reset},
+      stream);
 }

@@ -1,5 +1,6 @@
 """Device-resident vectorised envs with the reference's vec-env API: `DeviceVecEnv`, the base of the state-vector
-device envs (synthetic, CartPole, Pendulum, Acrobot, Mountain Car), and the synthetic env itself.
+device envs (synthetic, CartPole, Pendulum, Acrobot, Mountain Car), `SelfResettingVecEnv`, the base of those whose
+observation is not their state (Pendulum, Acrobot, Mountain Car), and the synthetic env itself.
 
 Stands where ``NormObs(VecEnv(...))`` / ``NormObs(SubProcVecEnv(...))`` stand in the reference
 (/root/reference/torchrl/env/get_env.py:70-87): same methods and attributes
@@ -254,6 +255,44 @@ class DeviceVecEnv:
             else:
                 new.__dict__[k] = copy.deepcopy(v, memo)
         return new
+
+
+class SelfResettingVecEnv(DeviceVecEnv):
+    """A state-vector device env whose observation is not its state: an fp64 physical state `phys` (N, phys_dim) beside
+    the fp32 `state`, and its own reset kernel (`resets_itself`), which the collector launches right after the finalize
+    kernel inside the captured step.  A subclass names its ops wrappers by their prefix in `kernels`
+    (ops.<kernels>_step, _reset and _num_ctas) and, in `step_extra`, the attributes passed after the step's common
+    arguments."""
+
+    # the collector's finalize kernel leaves this env's counters and observation to `collector_reset`
+    resets_itself = True
+    kernels = None
+    step_extra = ()
+
+    def __init__(self, env_id, env_nums, env_param, device, first_env, total_envs, max_episode_steps, obs_dim,
+                 phys_dim):
+        super().__init__(env_id, env_nums, env_param, device, first_env, total_envs, max_episode_steps, obs_dim, 1,
+                         getattr(ops, self.kernels + "_num_ctas")(int(env_nums)))
+        self.phys = torch.zeros(self.env_nums, phys_dim, dtype=F64, device=self.device)
+
+    def _reset_kernel(self, mask):
+        getattr(ops, self.kernels + "_reset")(self.phys, self.state, self.elapsed, self.episode, self.seeds, mask=mask)
+
+    def collector_reset(self, step_count, cur_ob, t_ptr, raw_obs_after_reset):
+        """The collector's partial reset (one launch, capturable): new episodes for the envs whose `step_count` the
+        finalize kernel just zeroed, and their next observation in `cur_ob` by collect_finalize's rules."""
+        nrm = self._obs_normalizer if self.obs_norm else None
+        getattr(ops, self.kernels + "_reset")(
+            self.phys, self.state, self.elapsed, self.episode, self.seeds, step_count=step_count,
+            next_norm=self.obs_out, cur_ob=cur_ob, any_reset=self.any_reset, t_ptr=t_ptr,
+            norm_mean=None if nrm is None else nrm._mean, norm_var=None if nrm is None else nrm._var,
+            clip=10.0 if nrm is None else nrm.clip, raw_obs_after_reset=raw_obs_after_reset)
+
+    def _step_kernel(self, actions, step_count, moments, t_ptr, reward_scale, max_episode_frames, merge):
+        getattr(ops, self.kernels + "_step")(
+            self.phys, self.state, actions.reshape(-1), self.elapsed, step_count, self.reward, self.done,
+            self.time_limit, self.action_error, *moments, self._ticket, self.any_reset, t_ptr, reward_scale,
+            self._max_episode_steps, max_episode_frames, merge, *(getattr(self, k) for k in self.step_extra))
 
 
 class SynthVecEnv(DeviceVecEnv):

@@ -972,15 +972,9 @@ def pendulum_step(phys, obs, actions, elapsed, step_count, reward, done, time_li
     [-1, 1] (a non-finite one sets action_error (1) int32).  partial / batch_sums / norm_*: the observation-normaliser
     moments (all None: not estimated); step_count / t_ptr: the collector's step counters and ring row (None outside a
     collector)."""
-    N = phys.shape[0]
-    if phys.dim() != 2 or phys.shape[1] != 2 or tuple(obs.shape) != (N, 3):
-        raise ValueError("pendulum_step: phys must be (N, 2) and obs (N, 3), got %s and %s"
-                         % (tuple(phys.shape), tuple(obs.shape)))
-    if actions.numel() != N:
-        raise ValueError("pendulum_step: one action per env expected, got %d for %d envs" % (actions.numel(), N))
-    _lib.call("trl_pendulum_step", phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error,
-              partial, batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, N, float(reward_scale),
-              int(max_episode_steps), int(max_episode_frames), int(bool(merge_stats)), _stream(), kernels=int(N > 0))
+    _env_step("pendulum_step", 2, 3, phys, obs, actions, elapsed, step_count, reward, done, time_limit, action_error,
+              partial, batch_sums, norm_mean, norm_var, norm_count, ticket, any_reset, t_ptr, reward_scale,
+              max_episode_steps, max_episode_frames, merge_stats)
 
 
 def pendulum_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=None, next_norm=None, cur_ob=None,
@@ -988,16 +982,8 @@ def pendulum_reset(phys, obs, elapsed, episode, seeds, mask=None, step_count=Non
     """New Pendulum episodes for every env (mask and step_count None), the envs of the uint8 `mask`, or those whose
     int32 `step_count` is 0 (the collector's path).  With `cur_ob` the next observation of every env is written there
     as collect_finalize writes it (next_norm / any_reset / t_ptr / norm_* / clip / raw_obs_after_reset)."""
-    N = phys.shape[0]
-    if phys.dim() != 2 or phys.shape[1] != 2 or tuple(obs.shape) != (N, 3):
-        raise ValueError("pendulum_reset: phys must be (N, 2) and obs (N, 3), got %s and %s"
-                         % (tuple(phys.shape), tuple(obs.shape)))
-    if mask is not None and step_count is not None:
-        raise ValueError("pendulum_reset: select envs by mask or by step_count, not both")
-    if cur_ob is not None and (step_count is None or next_norm is None or any_reset is None or t_ptr is None):
-        raise ValueError("pendulum_reset: cur_ob needs step_count, next_norm, any_reset and t_ptr")
-    _lib.call("trl_pendulum_reset", phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob, any_reset,
-              t_ptr, norm_mean, norm_var, N, float(clip), int(bool(raw_obs_after_reset)), _stream(), kernels=int(N > 0))
+    _env_reset("pendulum_reset", 2, 3, phys, obs, elapsed, episode, seeds, mask, step_count, next_norm, cur_ob,
+               any_reset, t_ptr, norm_mean, norm_var, clip, raw_obs_after_reset)
 
 
 def _check_phys_obs(fn, phys, obs, P, D):
