@@ -529,6 +529,22 @@ int trl_mountain_car_reset(double* phys, float* obs, int* elapsed, unsigned* epi
 /* ScaledFloatFrame (env/atari_wrapper.py:171-180): out = in * scale */
 int trl_u8_to_f32(const uint8_t* in, float* out, int64_t n, float scale, void* stream);
 
+/* ---- Atari frames stepped by host envs (env/atari_host.py; defined in oracle/atari_frames.py): WarpFrame
+ * (env/atari_wrapper.py:112-131, OpenCV's RGB2GRAY and INTER_AREA resize to 84x84, bit for bit) and FrameStack
+ * (:134-168) in one launch, one CTA per frame.  frames (M, H, W, 3) uint8 RGB, H, W >= 84, 3W % 16 == 0,
+ * H*W + 7056 <= 227 KB; stack (N, C, 84, 84) uint8 in place; both 16-byte aligned.  Frame m belongs to env
+ * env_idx[m] (env_idx NULL: env m, and M == N; ids outside [0, N) are skipped).  An env with fresh[n] != 0, or every
+ * env when fresh is NULL, gets the new frame in all C slots (FrameStack.reset); any other env's stack shifts by one
+ * frame and the new frame is appended (FrameStack.step).  tab_i = [xofs (85) | yofs (85) | xsrc | ysrc] int32 and
+ * tab_w = [xw | yw] fp32: OpenCV's area tables (computeResizeAreaTab) of W -> 84 and H -> 84 in CSR form, output
+ * column dx drawing on entries xofs[dx] .. xofs[dx+1]-1 (env/atari_host.py area_tables builds them). */
+int trl_atari_warp_stack(const uint8_t* frames, const int* env_idx, const uint8_t* fresh, uint8_t* stack,
+                         const int* tab_i, const float* tab_w, int64_t M, int64_t N, int H, int W, int C,
+                         void* stream);
+/* out[i] = lut[in[i]] as float32 (n % 4 == 0, in 4-byte and out 16-byte aligned, lut 256 floats): the pixel env's
+ * to_float, exact by construction for any map built on the host (ScaledFloatFrame's x / 255.0 - 0.5, or float(x)). */
+int trl_u8_lut_f32(const uint8_t* in, float* out, int64_t n, const float* lut, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -46,6 +46,9 @@ class PixelVecCollector(VecCollector):
         if self._boot:
             keys.append(("masks", (N, self.pf.head_num), U8))
         assert not (self.on_policy and self._dedup), "the on-policy pixel collector stores full frame stacks"
+        if self._dedup and self._host_env:
+            raise NotImplementedError("the frame-de-duplicated ring reads the env's episode step counters, which a "
+                                      "host Atari env keeps on the host: use the full-stack or prioritised ring")
         if self._dedup:
             # frame-de-duplicated ring (replay_buffers/memory_efficient.py): one frame of obs and one of next_obs per
             # row instead of two C-frame stacks
@@ -77,52 +80,87 @@ class PixelVecCollector(VecCollector):
     def _o_dim(self):
         return 1
 
-    def _step_body(self, bootstrap):
+    def _act_stage(self):
+        """The step before the env steps: ring write of obs, u8 -> f32, the action (and V(obs) on the side stream).
+        Returns the side stream V(obs) runs on, or None."""
         env, rb = self.env, self.replay_buffer
+        if self._dedup:
+            rb.write_obs(env.obs, env.elapsed)
+        else:
+            ops.ring_write(self._plan_obs, rb._top_dev)
+        env.to_float(env.obs, self._obs_f)
+        side = None
+        if self.on_policy:
+            if self._has_vf:
+                # V(obs) is only needed by the finalize kernel: a parallel branch of the captured step graph
+                main = torch.cuda.current_stream(self.device)
+                side = self._side_stream
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    self._value.copy_(self.vf(self._obs_f).reshape(-1))
+            self.pf.act_only(self._obs_f, action_out=self._act, nan_flag=self._nan_flag)
+        elif self._boot:
+            self.pf.act(self._obs_f, self.current_step, self._act, rb._masks, rb._top_dev)
+        else:
+            out = self.pf.explore(self._obs_f.unsqueeze(0), epsilon=self._eps_dev)
+            self._act.copy_(out["action"].reshape(self._act.shape).to(F32))
+        return side
+
+    def _store_stage(self, side, reset):
+        """The step after the env stepped: ring write of next_obs, V(next), finalize, then `reset()` (new episodes for
+        the envs the finalize cut), the prioritised insert and the ring advance."""
+        env, rb = self.env, self.replay_buffer
+        host = self._host_env
+        if self._dedup:
+            rb.write_next_obs(env.obs)
+        else:
+            ops.ring_write(self._plan_next, rb._top_dev)
+        v_next = None
+        if side is not None:
+            main = torch.cuda.current_stream(self.device)
+            main.wait_stream(side)              # one value net, one set of per-stream scratch: V(obs) first
+            self._v_next.copy_(self.vf(env.to_float(env.obs, self._next_f)).reshape(-1))
+            v_next = self._v_next
+        ops.collect_finalize(self._d_ob, self._d_ob, None if host else self._d_state, self._act, self._value, v_next,
+                             env.reward,
+                             env.done, env.time_limit, None if host else env.elapsed, None if host else env.episode,
+                             None if host else env.seeds, self.current_step,
+                             self.train_rew, self._epoch_reward, self._ret_log, self._n_done, None, None, None,
+                             self._d_ob, self._d_rows, self._d_rows, rb._acts,
+                             rb._values if self.on_policy else None, rb._rewards, rb._terminals,
+                             rb._time_limits, rb._top_dev, self.max_episode_frames,
+                             getattr(self, "discount", 0.0), 0.0, 10.0, self.on_policy, True)
+        reset()
+        if hasattr(rb, "mark_inserted"):
+            rb.mark_inserted()                    # prioritised ring: the new row enters with the max priority
+        ops.counter_advance(None, rb._top_dev, self._T, rb._size_dev)
+
+    def _step_body(self, bootstrap):
+        env = self.env
         with torch.no_grad():
-            if self._dedup:
-                rb.write_obs(env.obs, env.elapsed)
-            else:
-                ops.ring_write(self._plan_obs, rb._top_dev)
-            env.to_float(env.obs, self._obs_f)
-            side = None
-            if self.on_policy:
-                if self._has_vf:
-                    # V(obs) is only needed by the finalize kernel: a parallel branch of the captured step graph
-                    main = torch.cuda.current_stream(self.device)
-                    side = self._side_stream
-                    side.wait_stream(main)
-                    with torch.cuda.stream(side):
-                        self._value.copy_(self.vf(self._obs_f).reshape(-1))
-                self.pf.act_only(self._obs_f, action_out=self._act, nan_flag=self._nan_flag)
-            elif self._boot:
-                self.pf.act(self._obs_f, self.current_step, self._act, rb._masks, rb._top_dev)
-            else:
-                out = self.pf.explore(self._obs_f.unsqueeze(0), epsilon=self._eps_dev)
-                self._act.copy_(out["action"].reshape(self._act.shape).to(F32))
+            side = self._act_stage()
             env.launch_step(self._act.reshape(-1))
-            if self._dedup:
-                rb.write_next_obs(env.obs)
-            else:
-                ops.ring_write(self._plan_next, rb._top_dev)
-            v_next = None
-            if side is not None:
-                main.wait_stream(side)              # one value net, one set of per-stream scratch: V(obs) first
-                self._v_next.copy_(self.vf(env.to_float(env.obs, self._next_f)).reshape(-1))
-                v_next = self._v_next
-            ops.collect_finalize(self._d_ob, self._d_ob, self._d_state, self._act, self._value, v_next, env.reward,
-                                 env.done, env.time_limit, env.elapsed, env.episode, env.seeds, self.current_step,
-                                 self.train_rew, self._epoch_reward, self._ret_log, self._n_done, None, None, None,
-                                 self._d_ob, self._d_rows, self._d_rows, rb._acts,
-                                 rb._values if self.on_policy else None, rb._rewards, rb._terminals,
-                                 rb._time_limits, rb._top_dev, self.max_episode_frames,
-                                 getattr(self, "discount", 0.0), 0.0, 10.0, self.on_policy, True)
             # envs whose collector step counter was just zeroed need a fresh episode (done or timeout); the
             # finalize kernel already advanced their episode counter
-            env._reset(zero_is_mask=self.current_step, episode_bias=1, bump=0)
-            if hasattr(rb, "mark_inserted"):
-                rb.mark_inserted()                    # prioritised ring: the new row enters with the max priority
-            ops.counter_advance(None, rb._top_dev, self._T, rb._size_dev)
+            self._store_stage(side, lambda: env._reset(zero_is_mask=self.current_step, episode_bias=1, bump=0))
+
+    def _step_host_pixel(self):
+        """One eager step over host Atari envs (env/atari_host.py): the same stages around the host step, then the host
+        partial reset of the envs that ended (done) or were cut by max_episode_frames, from a host mirror of the step
+        counters (the finalize kernel zeroes exactly those envs' counters)."""
+        env = self.env
+
+        def reset():
+            sc = self._host_steps + 1
+            mask = env.host_done | (sc >= self.max_episode_frames)
+            if mask.any():
+                env.partial_reset(mask)
+            self._host_steps = np.where(mask, 0, sc)
+
+        with torch.no_grad():
+            side = self._act_stage()
+            env.launch_step(self._act.reshape(-1))
+            self._store_stage(side, reset)
 
     def _need_bootstrap(self):
         return False
@@ -133,6 +171,10 @@ class PixelVecCollector(VecCollector):
             self.pf.tick()                               # host-side epsilon schedule -> device scalar
             self._eps_host[0] = float(self.pf.epsilon)
             self._eps_dev.copy_(self._eps_host, non_blocking=True)
+        if self._host_env:
+            self._step_host_pixel()
+            self.replay_buffer.advance_host(1)
+            return
         # "reference_cpu" sampling draws on the host (torch.multinomial): not capturable
         eager = not self.use_cuda_graph or (self.on_policy and D.get_noise_mode() == "reference_cpu")
         if eager:

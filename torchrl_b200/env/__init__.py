@@ -8,4 +8,5 @@ from .pendulum import PendulumVecEnv  # noqa: F401
 from .acrobot import AcrobotVecEnv  # noqa: F401
 from .mountain_car import MountainCarVecEnv  # noqa: F401
 from .bridge import HostEnvBridge  # noqa: F401
+from .atari_host import AtariHostVecEnv  # noqa: F401
 from ..hostenv import VecEnv as HostVecEnv, SubProcVecEnv as HostSubProcVecEnv  # noqa: F401

@@ -1085,6 +1085,30 @@ def u8_to_f32(x, scale, out=None):
     return out
 
 
+def atari_warp_stack(frames, stack, tab_i, tab_w, env_idx=None, fresh=None):
+    """WarpFrame + FrameStack in one launch (csrc/atari_frames.cu): frames (M, H, W, 3) uint8 RGB -> gray, 84x84
+    INTER_AREA -> the (N, C, 84, 84) uint8 stack of env env_idx[m] (None: env m), filling every slot of a fresh env
+    (fresh None: all envs fresh) and shifting in the new frame for the others.  tab_i / tab_w: area_tables(H, W) of
+    env/atari_host.py on the device.  One launch, none when M == 0."""
+    M, H, W, three = frames.shape
+    N, C = stack.shape[:2]
+    if three != 3 or tuple(stack.shape[2:]) != (84, 84):
+        raise ValueError("atari_warp_stack: frames (M, H, W, 3) and stack (N, C, 84, 84), got %s and %s"
+                         % (tuple(frames.shape), tuple(stack.shape)))
+    _lib.call("trl_atari_warp_stack", frames, env_idx, fresh, stack, tab_i, tab_w, M, N, H, W, C, _stream(),
+              kernels=int(M > 0))
+
+
+def u8_lut_f32(x, lut, out=None):
+    """out = lut[x] as float32 (lut: 256 floats on the device).  One launch."""
+    if out is None:
+        out = torch.empty(x.shape, dtype=F32, device=x.device)
+    if out.numel() != x.numel() or lut.numel() != 256:
+        raise ValueError("u8_lut_f32: out must match x and lut must hold 256 entries")
+    _lib.call("trl_u8_lut_f32", x, out, x.numel(), lut, _stream(), kernels=int(x.numel() > 0))
+    return out
+
+
 # ------------------------------------------------------------------------------------------ frame-stack ring
 def frame_ring_write(stack, ring, top, age=None, elapsed=None, hist=None, hist_count=None, size=None):
     """Newest frame of every env's (N, C, ...) uint8 stack -> row *top of ring (T, N, F); age / elapsed: also the age
