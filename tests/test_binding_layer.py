@@ -94,7 +94,6 @@ def _multi_kernel_calls():
     return {
         "skinny_tn": lambda: ops.skinny_tn(g, x, dw, None, False, tn(K)),
         "skinny_act_wgrad": lambda: ops.skinny_act_wgrad(g, y, x, dw, db, 1, tn(K)),
-        "skinny_n_dgrad_act": lambda: ops.skinny_n_dgrad_act(g_out, w_out, y, gz, db, 1, da),
         "skinny_n_dgrad_act_wgrad": lambda: ops.skinny_n_dgrad_act_wgrad(g_out, w_out, y, 1, gz, db, dw3, db3, da,
                                                                          tn(N)),
         "skinny_reduce_jobs": lambda: (ops.skinny_act_wgrad_partial(g, y, x, 1, part),

@@ -249,11 +249,10 @@ _FORK_STREAMS = {}
 
 class backward_fork:
     """Scope around ONE `torch.autograd.backward` call of an MLP with a fused tail: the weight-gradient work that nothing
-    downstream in that backward pass depends on (the 256 x 256 wgrad GEMM, and the output layer's dW / db where they
-    are not formed in the dgrad-act pass) is issued on a
-    companion stream while the dgrad GEMM and the first-layer backward continue on the calling stream; the scope's
-    exit joins the two (under graph capture: a parallel branch).  Tensors the companion stream reads are kept alive
-    until the join.  Outside such a scope the backward is strictly sequential."""
+    downstream in that backward pass depends on (the 256 x 256 wgrad GEMM) is issued on a companion stream while the
+    dgrad GEMM and the first-layer backward continue on the calling stream; the scope's exit joins the two (under
+    graph capture: a parallel branch).  Tensors the companion stream reads are kept alive until the join.  Outside
+    such a scope the backward is strictly sequential."""
 
     def __enter__(self):
         global _FORK
@@ -372,15 +371,10 @@ def _can_defer(*outs):
     return _DEFER is not None and all(o is not None for o in outs)
 
 
-def skinny_tn(a, b, out=None, colsum=None, out_transposed=False, may_defer=False):
+def skinny_tn(a, b, out=None, colsum=None, out_transposed=False):
     """out = a^T @ b for a (M,H), b (M,K<=32) [+ colsum = b.sum(0)]: csrc/skinny.cu, two deterministic stages."""
     M, H = a.shape
     K = b.shape[1]
-    if may_defer and _can_defer(out) and len(_DEFER) < 64:
-        ws = _scratch("tn", a.device, M, H, K, job=0)
-        ops.skinny_tn_partial(a, b, colsum is not None, ws)
-        _DEFER.append((0, ws, out, colsum, M, H, K, int(bool(out_transposed))))
-        return out
     if out is None:
         out = torch.empty((K, H) if out_transposed else (H, K), dtype=torch.float32, device=a.device)
     return ops.skinny_tn(a, b, out, colsum, out_transposed, _scratch("tn", a.device, M, H, K))
@@ -524,16 +518,18 @@ class _MLPTail(torch.autograd.Function):
         h1 = act1(x W1^T + b1)  (csrc/skinny.cu k_fwd; only when w1 is given, x then needs no gradient)
         y2 = act(h1 W2^T + b2)  (wgmma 3xTF32, bias + activation in the epilogue)
         out = y2 W3^T + b3      (csrc/skinny.cu n_fwd)
-    so that the backward can fuse the output-layer dgrad with the activation backward of the hidden layer
-    (trl_skinny_n_dgrad_act: gz2 and db2 in one pass, the (M, 256) dgrad matrix is never stored un-activated; at
-    H = 256 trl_skinny_n_dgrad_act_wgrad also forms the output layer's dW3 / db3 slab partials in that pass over y2,
-    bit for bit those of skinny_tn, so y2 is read once and the companion stream carries the wgrad alone), and,
-    with the first layer, the dgrad dH1 = gz2 W2 with the first layer's weight / bias gradient: inside
-    `transposed_planes()` trl_gemm3_pair_dgrad_act_wgrad reduces dH1 to dW1 / db1 slab partials in its epilogue, so
-    dH1 is never stored (elsewhere: mm_dgrad, then the skinny first-layer backward, the same bits)."""
+    The hidden layer is 256 wide: that is the width which admits the wgmma GEMM (tail_ok), and the width the output
+    layer's fused backward serves.  So the backward runs the output layer's whole backward and the activation backward
+    of the hidden layer as one pass over y2 (trl_skinny_n_dgrad_act_wgrad: gz2 and db2, the (M, 256) dgrad matrix
+    never stored un-activated, and the output layer's dW3 / db3 slab partials, bit for bit those of skinny_tn; the
+    companion stream carries the wgrad alone), and, with the first layer, the dgrad dH1 = gz2 W2 with the first
+    layer's weight / bias gradient: inside `transposed_planes()` trl_gemm3_pair_dgrad_act_wgrad reduces dH1 to
+    dW1 / db1 slab partials in its epilogue, so dH1 is never stored (elsewhere: mm_dgrad, then the skinny first-layer
+    backward, the same bits)."""
 
     @staticmethod
     def forward(ctx, x, w1, b1, act1, w2, b2, w3, b3, act):
+        assert w2.shape[0] == 256 == w3.shape[1], "_MLPTail needs a 256-wide hidden layer"
         h1 = ops.skinny_k_fwd(x, w1, b1, act1) if w1 is not None else x
         y2 = mm_fwd(h1, w2, bias=b2, act=act)
         out = ops.skinny_n_fwd(y2, w3, b3)
@@ -554,45 +550,30 @@ class _MLPTail(torch.autograd.Function):
         db2 = db2_out if db2_out is not None else torch.empty(H, dtype=torch.float32, device=dev)
         db3 = db3_out if db3_out is not None else torch.empty(N, dtype=torch.float32, device=dev)
         gz = torch.empty_like(y2)
-        # H = 256: dW3 (N,H) = g^T y2 and db3 = sum g come out of the same pass over y2 (skinny_tn's slab partials)
-        w3_fused = H == 256
-        if w3_fused:
-            dw3 = dw3_out if dw3_out is not None else torch.empty(N, H, dtype=torch.float32, device=dev)
-        if w3_fused and _can_defer(db2_out, dw3_out, db3_out) and len(_DEFER) < 63:     # skinny_tn's bound on jobs
+        dw3 = dw3_out if dw3_out is not None else torch.empty(N, H, dtype=torch.float32, device=dev)
+        # gz2, db2 and dW3 (N,H) = g^T y2, db3 = sum g in one pass over y2
+        if _can_defer(db2_out, dw3_out, db3_out) and len(_DEFER) < 63:     # two more jobs, at most 64 pending
             ws = _scratch("dgrad_act", dev, M, H, job=2)
             _DEFER.append((2, ws, None, db2, M, H, 0, 0))
             ws3 = _scratch("tn", dev, M, H, N, job=0)
             _DEFER.append((0, ws3, dw3, db3, M, H, N, 1))
             ops.skinny_n_dgrad_act_wgrad_partial(g, w3, y2, ctx.act, gz, ws, ws3)
-        elif w3_fused:
+        else:
             ops.skinny_n_dgrad_act_wgrad(g, w3, y2, ctx.act, gz, db2, dw3, db3, _scratch("dgrad_act", dev, M, H),
                                          _scratch("tn", dev, M, H, N))
-        elif _can_defer(db2_out):
-            ws = _scratch("dgrad_act", dev, M, H, job=2)
-            ops.skinny_n_dgrad_act_partial(g, w3, y2, gz, ctx.act, ws)
-            _DEFER.append((2, ws, None, db2, M, H, 0, 0))
-        else:
-            ops.skinny_n_dgrad_act(g, w3, y2, gz, db2, ctx.act, _scratch("dgrad_act", dev, M, H))
         first = w1 is not None
         want_dx = ctx.needs_input_grad[0] and not first
-        fk = _fork_here()
-        if fk is not None and dw2_out is not None and dw3_out is not None:
-            # the weight gradients that feed nothing but the optimizer: companion stream (see backward_fork)
+        fk = _fork_here() if dw2_out is not None and dw3_out is not None else None
+        if fk is not None:
+            # the weight gradient that feeds nothing but the optimizer: companion stream (see backward_fork)
             fk.side.wait_stream(fk.main)
             with torch.cuda.stream(fk.side):
-                if not w3_fused:
-                    dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True, may_defer=db3_out is not None)
                 dw2 = wgrad(gz, x, out=dw2_out)
-            fk.keep += [gz, x] if w3_fused else [gz, g, y2, x]
+            fk.keep += [gz, x]
             fk.used = True
-            first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
-            dx = mm_dgrad(gz, w2) if want_dx else None
-        else:
-            if not w3_fused:
-                dw3 = skinny_tn(y2, g, out=dw3_out, colsum=db3, out_transposed=True,   # dW3 (N,H) = g^T y2, db3 = sum g
-                                may_defer=dw3_out is not None and db3_out is not None)
-            first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
-            dx = mm_dgrad(gz, w2) if want_dx else None
+        first_grads = _first_layer_bwd(ctx, gz, x0, w1, x, w2) if first else None
+        dx = mm_dgrad(gz, w2) if want_dx else None
+        if fk is None:
             dw2 = wgrad(gz, x, out=dw2_out)
         tail = (None if dw2_out is not None else dw2, None if db2_out is not None else db2,
                 None if dw3_out is not None else dw3, None if db3_out is not None else db3, None)

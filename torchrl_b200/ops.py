@@ -862,13 +862,6 @@ def skinny_tn(a, b, out, colsum, out_transposed, scratch):
     return out
 
 
-def skinny_tn_partial(a, b, want_colsum, scratch):
-    """The slabs of skinny_tn (reduce job kind 0)."""
-    M, H = a.shape
-    K = b.shape[1]
-    _lib.call("trl_skinny_tn_partial", a, b, M, H, K, int(bool(want_colsum)), scratch, _stream())
-
-
 def skinny_act_wgrad(g, y, x, dw, db, act, scratch):
     """The first layer's dW (H,K) = (g * act'(y))^T x and db = colsum(g * act'(y)) in one pass over g and y (M,H);
     scratch: skinny_tn_scratch_floats(M, H, K) floats."""
@@ -884,24 +877,10 @@ def skinny_act_wgrad_partial(g, y, x, act, scratch):
     _lib.call("trl_skinny_act_wgrad_partial", g, y, x, M, H, K, int(act), scratch, _stream())
 
 
-def skinny_n_dgrad_act(g, w, y, gz, db, act, scratch):
-    """gz (M,H) = (g (M,N) @ w (N,H)) * act'(y) and db = colsum(gz); scratch: skinny_dgrad_act_scratch_floats(M, H)."""
-    M, H = y.shape
-    N = w.shape[0]
-    _lib.call("trl_skinny_n_dgrad_act", g, w, y, gz, db, M, H, N, int(act), scratch, _stream(), kernels=2)
-
-
-def skinny_n_dgrad_act_partial(g, w, y, gz, act, scratch):
-    """gz of skinny_n_dgrad_act and the slabs of its db (reduce job kind 2)."""
-    M, H = y.shape
-    N = w.shape[0]
-    _lib.call("trl_skinny_n_dgrad_act_partial", g, w, y, gz, M, H, N, int(act), scratch, _stream())
-
-
 def skinny_reduce_jobs(jobs):
     """The slab sums of up to 8 jobs (kind, scratch, out, colsum, M, H, K, out_transposed) in one launch: kind 0 =
-    skinny_tn_partial (colsum None or (K)), 1 = skinny_act_wgrad_partial (colsum = db (H)), 2 =
-    skinny_n_dgrad_act_partial (colsum = db (H), out None)."""
+    skinny_tn's slabs (colsum None or (K); skinny_n_dgrad_act_wgrad_partial's w_scratch), 1 = skinny_act_wgrad_partial
+    (colsum = db (H)), 2 = skinny_n_dgrad_act_wgrad_partial's db_scratch (colsum = db (H), out None)."""
     n = len(jobs)
     assert n <= 8
     ci = ctypes.c_int
